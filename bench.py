@@ -6,6 +6,7 @@ synthetic 550x550 frames, yolact_base (ResNet101-FPN), batch 8 per GPU (BASELINE
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference ...      # the reference algorithm on the host CPU cores
+    python bench.py ... --dump-outputs DIR    # also write what the timed path returned in its last step (DIR/<name>.npy)
 
 One step = one batch through the whole path.  Prints ONE JSON line (rank 0).  See DESIGN.md
 "Measurement" for what each key means; in short:
@@ -14,9 +15,9 @@ One step = one batch through the whole path.  Prints ONE JSON line (rank 0).  Se
             protocol: H2D, `preds = net(x)`, per image `postprocess(preds, w, h, b)`, D2H of classes / scores /
             boxes / fp32 masks [:top_k] (eval.py:264-281), host-synchronised every step
   e2e_bits  (secondary) the batched extension API shipping ALL 100 masks per image 1 bit/pixel
-  roofline  tcgen05 conv stack: algorithmic FLOPs (BASELINE.md section 3) / CUDA-event time of the conv-stack
-            graph, against the measured cuBLAS bf16 peak of MEASURED_PEAKS.json (burst when the sampled clocks
-            are unthrottled, sustained otherwise)
+  roofline  tensor-core conv stack: algorithmic FLOPs (BASELINE.md section 3) / CUDA-event time of the conv-stack
+            graph, against the measured cuBLAS bf16 peak of MEASURED_PEAKS.json when present (burst when the sampled
+            clocks are unthrottled, sustained otherwise), else the H100 SXM data-sheet dense fp16 rate
   fast_mode_f16tc  (secondary) the single-pass fp16 mode, which does NOT meet the 1e-3 tolerance
   cpu_baseline / --impl reference  the oracle port (torch-CPU fp32 conv stack + torch-CPU Detect/postprocess) on
             the same config and batch, all host threads; the reference arm imports no yolact_b200 module
@@ -57,19 +58,22 @@ def parse():
     ap.add_argument("--batch", type=int, default=8, help="images per GPU per step")
     ap.add_argument("--size", type=int, default=0, help="image size (default: the config's max_size)")
     ap.add_argument("--precision", default="f16x3", choices=["f16x3", "f16tc", "f32"],
-                    help="f16x3: split-precision tcgen05 (meets the reference tolerance; the headline mode); "
-                         "f16tc: single-pass fp16 tcgen05 (fast mode); f32: CUDA-core fp32")
+                    help="f16x3: split-precision tensor cores (meets the reference tolerance; the headline mode); "
+                         "f16tc: single-pass fp16 tensor cores (fast mode); f32: CUDA-core fp32")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-fast-mode", action="store_true", help="skip the secondary single-pass fp16 measurement")
     ap.add_argument("--cpu-sample", type=int, default=16, help="images in the cpu_baseline sample")
     ap.add_argument("--top-k", dest="top_k", type=int, default=5,
                     help="detections per image copied to the host in the e2e loop (eval.py --top_k default: 5)")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the outputs of the timed path's last step as DIR/<name>.npy "
+                         "(float32 / float64; the fp32 masks as a fixed seeded sample)")
     return ap.parse_args()
 
 
 # ---------------------------------------------------------------------------------------------
 class ClockSampler(object):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -263,6 +267,29 @@ def reference_arm(args, rank):
     return 0
 
 
+MASK_SAMPLE = 1 << 21   # fp32 mask values kept by --dump-outputs (8 MB; the full [B, 100, H, W] tensor is ~1 GB)
+
+
+def dump_outputs(out_dir, out):
+    """What the timed path returned in its last step, as DIR/<name>.npy: boxes, mask coefficients, class ids, scores,
+    detection counts and the masks' pixel boxes in full, the fp32 masks as a fixed seeded sample of MASK_SAMPLE elements (masks_sample[i] =
+    masks.flatten()[masks_sample_index[i]])."""
+    import numpy as np
+    import torch
+    box, coef, cls, score, count, (masks, boxes_px) = out
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"boxes": box, "coefficients": coef, "classes": cls, "scores": score, "counts": count, "boxes_px": boxes_px}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
+    flat = masks.reshape(-1)
+    g = torch.Generator().manual_seed(0)
+    idx = torch.randint(0, flat.numel(), (min(MASK_SAMPLE, flat.numel()),), generator=g)
+    np.save(os.path.join(out_dir, "masks_sample.npy"), flat[idx.to(flat.device)].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "masks_sample_index.npy"), idx.double().numpy())
+    np.save(os.path.join(out_dir, "masks_shape.npy"), np.array(masks.shape, dtype=np.float64))
+
+
 # ---------------------------------------------------------------------------------------------
 def main():
     args = parse()
@@ -308,7 +335,7 @@ def main():
     net = make_net(args.precision)
     sd = {k: v.detach().cpu() for k, v in net.state_dict().items()}
 
-    n_rot = 6  # 6 distinct input batches (6 x 29 MB = 174 MB > 126 MB L2) rotate through the loop
+    n_rot = 6  # 6 distinct input batches (6 x 29 MB = 174 MB > 50 MB L2) rotate through the loop
     xs = [deterministic_input(B, size, size, 1234 + 100 * rank + i).to(dev) for i in range(n_rot)]
     M, k = cfg.max_num_detections, cfg.mask_dim
     # Two compute streams: the mask assembly of step i (HBM-write bound) runs on s_post while the conv stack of step
@@ -353,6 +380,8 @@ def main():
             ms = float(t.item())
         return ms
 
+    last = {}
+
     def timed(fn, steps, warmup):
         for i in range(warmup):
             fn(i)
@@ -360,7 +389,7 @@ def main():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for i in range(steps):
-            fn(warmup + i)
+            last["out"] = fn(warmup + i)
         if s_post is not None:
             torch.cuda.current_stream().wait_stream(s_post)   # the last steps' mask assembly is inside the timed region
         e1.record()
@@ -377,6 +406,8 @@ def main():
     # kernels launched inside the TIMED region only (the counter also saw the warm-up steps of `timed`)
     launches = (net.launch_count() + output_utils.launch_count() - l0) * args.steps // (args.steps + max(3, args.warmup))
     fps = world * B * args.steps / (ms / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["out"])
     hold[0] = hold[1] = None
 
     # ---- e2e (headline): the reference-facing API with HOST frames, eval.py's --benchmark protocol --------------------
@@ -536,7 +567,7 @@ def main():
     ms_bits, wall_bits = timed_api(step_bits, bits_drain, args.steps, 3)
     fps_bits = world * B * args.steps / (ms_bits / 1e3)
 
-    # ---- roofline of the dominant kernel family (tcgen05 conv stack), timed live with CUDA events
+    # ---- roofline of the dominant kernel family (tensor-core conv stack), timed live with CUDA events
     def conv_ms(net_):
         net_.train()
         r = timed(lambda i: net_.forward_conv_only(xs[i % n_rot]), args.steps, 3)
@@ -556,10 +587,10 @@ def main():
                        not set(clocks.get("reasons") or []) & {"hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"})
     if peaks:
         peak = peaks.get("bf16_tflops") if (unthrottled or rank != 0) else peaks.get("bf16_tflops_sustained")
-        peak = peak or peaks.get("bf16_tflops_sustained") or 1400.0
+        peak = peak or peaks.get("bf16_tflops_sustained") or 989.0
         peak_src = "MEASURED_PEAKS.json %s cuBLAS bf16" % ("burst (clocks unthrottled during the timed region)" if unthrottled else "sustained")
     else:
-        peak, peak_src = 1400.0, "fallback ~1.4 PF sustained (B200_PROFILING.md)"
+        peak, peak_src = 989.0, "H100 SXM data sheet, dense fp16 (not measured)"
     traffic = None
     try:
         tj = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json")))
@@ -579,12 +610,12 @@ def main():
     line = dict(base)
     line.update({
         "value": fps, "ms_per_step": ms / args.steps,
-        "dtype": {"f16x3": "f16x3 (fp16 hi+lo operand pairs, 3 tcgen05 passes, fp32 accumulate: fp32-equivalent, parity-tested at 1e-3)",
+        "dtype": {"f16x3": "f16x3 (fp16 hi+lo operand pairs, 3 wgmma passes, fp32 accumulate: fp32-equivalent, parity-tested at 1e-3)",
                   "f16tc": "f16", "f32": "f32"}[args.precision],
         "config": {"workload": workload_string(cfg, size, B), "global_batch": world * B, "image_size": size,
                    "parallelism": "dp%d" % world, "detections_per_image": M, "precision": args.precision,
                    "mask_format_value": "f32 [n,h,w], all %d detections" % M,
-                   "l2": "6 rotating input batches (174 MB) and ~2 GB of activations+masks per step exceed the 126 MB L2",
+                   "l2": "6 rotating input batches (174 MB) and ~2 GB of activations+masks per step exceed the 50 MB L2",
                    "cuda_graph": True,
                    "streams": "mask assembly of step i overlaps the conv stack of step i+1 (2 compute streams)" if overlap
                               else "single compute stream"},
@@ -608,7 +639,7 @@ def main():
         "roofline": roofline,
     })
 
-    # ---- fast mode (secondary, labelled): single-pass fp16 tcgen05, outside the 1e-3 tolerance
+    # ---- fast mode (secondary, labelled): single-pass fp16 tensor cores, outside the 1e-3 tolerance
     if args.precision == "f16x3" and not args.no_fast_mode:
         del net
         hold[0] = hold[1] = None
@@ -622,7 +653,7 @@ def main():
             "value": world * B * args.steps / (ms_f / 1e3), "unit": "frames/s", "ms_per_step": ms_f / args.steps,
             "ms_conv_stack_per_step": ms_fc / args.steps, "conv_tflops": ach_f, "conv_frac_of_peak": ach_f / peak,
             "note": "single-pass fp16 operands: head tensors ~2e-3 of range from the fp32 reference, class ids not "
-                    "bit-exact (profiles/parity_r02.md) -- NOT the headline"}
+                    "bit-exact -- NOT the headline"}
 
     # ---- cpu_baseline (rank 0, N == 1 only): bounded sample of the same workload on the host cores
     if rank == 0 and world == 1 and not args.no_cpu_baseline:

@@ -1,7 +1,7 @@
 /* Plain-C client of the boundary (include/yolact_b200.h): what a cgo / JNI / FFI binding would do.
  *   gcc -std=c99 -Wall -Iinclude examples/c_abi_demo.c -o c_abi_demo yolact_b200/libyolact_b200.so -Wl,-rpath,$PWD/yolact_b200
  * Creates an ops-only handle (no backbone) and runs row-wise softmax on the device through the library's own
- * kernels; on a machine without a B200 it reports the library's error message and exits 0. */
+ * kernels; on a machine without an H100 it reports the library's error message and exits 0. */
 #include <stdio.h>
 #include <string.h>
 

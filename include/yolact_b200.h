@@ -1,5 +1,5 @@
 /*
- * yolact_b200.h -- C ABI of the B200-native YOLACT inference path.
+ * yolact_b200.h -- C ABI of the H100-native YOLACT inference path.
  *
  * This is the drop-in boundary (SURVEY.md section 8b).  Every entry point takes
  * plain pointers / sizes / a cudaStream_t passed as void*; there are no torch
@@ -66,11 +66,11 @@ typedef enum { YB_BACKBONE_NONE = -1, YB_BACKBONE_RESNET = 0, YB_BACKBONE_DARKNE
 
 /* Arithmetic mode of the convolution stack.
  *   YB_PREC_F32  : fp32 activations, fp32 FMA on CUDA cores (reference-order arithmetic, slow; second opinion)
- *   YB_PREC_F16TC: fp16 activations/weights, fp32 accumulation on tcgen05 tensor cores: one MMA pass, 11-bit
+ *   YB_PREC_F16TC: fp16 activations/weights, fp32 accumulation on the tensor cores (wgmma): one MMA pass, 11-bit
  *                  operands -- the fast mode; head tensors within ~2e-3 of range of the fp32 reference
- *   YB_PREC_F16X3: split precision on tcgen05 (the default of the Python API): every activation and weight is
- *                  an fp16 pair hi + lo (22 significand bits), each k-block issues hi*hi + lo*hi + hi*lo into one
- *                  fp32 TMEM accumulator -- fp32-equivalent results (1e-3 on boxes/masks, identical class ids
+ *   YB_PREC_F16X3: split precision on the tensor cores (the default of the Python API): every activation and weight is
+ *                  an fp16 pair hi + lo (22 significand bits), each k-block issues hi*hi + lo*hi + hi*lo into fp32
+ *                  register accumulators -- fp32-equivalent results (1e-3 on boxes/masks, identical class ids
  *                  against the fp32 reference) at three MMA passes and twice the operand bytes */
 typedef enum { YB_PREC_F32 = 0, YB_PREC_F16TC = 1, YB_PREC_F16X3 = 2 } yb_precision;
 
@@ -274,8 +274,8 @@ YB_API int yb_dcn_forward(yb_handle* h, const float* d_input, const float* d_wei
 /* Single convolution through the same kernels the network uses (test / microbench hook).
  * x NCHW fp32 [B,Ci,H,W], w OIHW fp32 (host), bias fp32[Co] (host, nullable),
  * residual NCHW fp32 [B,Co,Ho,Wo] (device, nullable), y NCHW fp32 [B,Co,Ho,Wo].
- * act: 0 none, 1 relu, 2 tanh, 3 leaky_relu(0.1).  precision: 0 fp32 CUDA cores, 1 fp16 tcgen05 (YB_PREC_F16TC),
- * 2 fp16 CUDA cores, 3 split-precision tcgen05 (YB_PREC_F16X3).
+ * act: 0 none, 1 relu, 2 tanh, 3 leaky_relu(0.1).  precision: 0 fp32 CUDA cores, 1 fp16 tensor cores (YB_PREC_F16TC),
+ * 2 fp16 CUDA cores, 3 split-precision tensor cores (YB_PREC_F16X3).
  * iters > 1 repeats the conv kernel and returns the mean kernel time (ms) in *ms (nullable). */
 YB_API int yb_conv2d(yb_handle* h, const float* d_x, const float* h_w, const float* h_bias,
               const float* d_residual, float* d_y, int B, int Ci, int H, int W, int Co,

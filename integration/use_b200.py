@@ -1,4 +1,4 @@
-"""Route the reference's eval.py through the B200 path without editing a line of it (INTEGRATION.md section 1).
+"""Route the reference's eval.py through the H100 path without editing a line of it (INTEGRATION.md section 1).
 
     import integration.use_b200 as ub
     ub.install("/path/to/yolact")          # BEFORE `import eval`

@@ -469,12 +469,53 @@ def gen_state_keys():
         json.dump(out, f)
 
 
+# the raw fields of a reference cfg that yolact_b200.config.from_reference_cfg reads (incl. the switches it rejects)
+CFG_FIELDS = ("name", "max_size", "num_classes", "mask_dim", "use_maskiou", "rescore_mask", "rescore_bbox", "nms_top_k",
+              "nms_conf_thresh", "nms_thresh", "max_num_detections", "eval_mask_branch", "mask_proto_debug",
+              "preserve_aspect_ratio", "use_prediction_module", "use_yolo_regressors", "use_mask_scoring",
+              "use_instance_coeff", "use_focal_loss", "use_objectness_score", "mask_proto_use_grid",
+              "mask_proto_coeff_gate", "mask_proto_prototypes_as_features", "mask_proto_split_prototypes_by_head",
+              "mask_proto_bias", "share_prediction_module")
+BACKBONE_FIELDS = ("args", "selected_layers", "pred_scales", "pred_aspect_ratios", "use_square_anchors")
+TRANSFORM_FIELDS = ("normalize", "to_float", "subtract_means", "channel_order")
+
+
+def gen_reference_cfg():
+    """The raw fields of the reference's own cfg object of every named config that
+    yolact_b200.config.from_reference_cfg reads (tests/test_reference_cfg_snapshot.py rebuilds duck-typed cfgs from
+    them and runs the converter).  Fields a cfg does not have are left out (the converter's getattr defaults apply)."""
+    import json
+    from data import config as rc
+
+    def plain(v):
+        if isinstance(v, (list, tuple)):
+            return [plain(x) for x in v]
+        if isinstance(v, (bool, int, str)) or v is None:
+            return v
+        return float(v)
+
+    def fields(obj, names):
+        return {k: plain(getattr(obj, k)) for k in names if hasattr(obj, k)}
+    out = {}
+    for name in ("yolact_base_config", "yolact_im700_config", "yolact_darknet53_config", "yolact_resnet50_config",
+                 "yolact_plus_base_config", "yolact_plus_resnet50_config"):
+        c = getattr(rc, name)
+        b = c.backbone
+        out[name] = dict(fields(c, CFG_FIELDS), fpn={"num_features": int(c.fpn.num_features)},
+                         backbone=dict(fields(b, BACKBONE_FIELDS), type=b.type.__name__,
+                                       transform=fields(b.transform, TRANSFORM_FIELDS)))
+    os.makedirs(OUT, exist_ok=True)
+    with open(os.path.join(OUT, "reference_cfg.json"), "w") as f:
+        json.dump(out, f, indent=1, sort_keys=True)
+
 if __name__ == "__main__":
     install_shims()
     torch.set_num_threads(8)
     which = sys.argv[1:] or ["units", "nets"]
     if "keys" in which or "units" in which:
         gen_state_keys()
+    if "cfg" in which or "units" in which:
+        gen_reference_cfg()
     if "units" in which:
         gen_detect_unit()
         gen_postprocess_unit()

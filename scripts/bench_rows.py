@@ -13,7 +13,7 @@ from yolact_b200.output_utils import assemble_masks, _ops_handle
 from yolact_b200 import _lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-peak = 6500.0
+peak = 3350.0   # H100 SXM data-sheet HBM3 bandwidth (GB/s) unless MEASURED_PEAKS.json says otherwise
 try:
     pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     peak = float(pk.get("hbm_gbs", peak))
@@ -91,7 +91,7 @@ cols = r.uniform(0, 1, (15, 3)).astype(np.float32)
 ms = timeit(lambda: display_blend(frame, bits[:15], cols, 0.45, w=550))
 rows.append(("display_blend 15 masks @550^2 (bits)", ms, 550 * 550 * (12 + 3) + 15 * words * 4))
 
-print("# section-8f row kernels, device time (CUDA events), B200; HBM peak used: %.0f GB/s\n" % peak)
+print("# section-8f row kernels, device time (CUDA events), %s; HBM peak used: %.0f GB/s\n" % (torch.cuda.get_device_name(), peak))
 print("| kernel | ms | algorithmic MB | GB/s | frac of HBM peak |\n|---|---:|---:|---:|---:|")
 for name, ms, by in rows:
     gbs = by / ms / 1e6

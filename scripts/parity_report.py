@@ -1,11 +1,10 @@
 #!/usr/bin/env python
 """Full-size parity report: GPU path (a precision mode) vs the CPU oracle on the BASELINE configs.
 
-    python scripts/parity_report.py --precisions f16tc,f16x3 --out gpurun_out/parity.json
+    python scripts/parity_report.py --precisions f16tc,f16x3 --out parity.json
 
 One row per (config, precision): raw head-tensor error (max |d| / max |ref|), class ids equal, keep-set
-agreement, max |dbox|, max |dscore|, flipped mask pixels.  The markdown committed under profiles/ is this
-script's stdout.
+agreement, max |dbox|, max |dscore|, flipped mask pixels, as a markdown table on stdout.
 """
 import argparse
 import json

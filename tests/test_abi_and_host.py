@@ -154,7 +154,7 @@ def test_product_never_imports_oracle():
 
 
 def test_graft_entry_build_check_passes():
-    """The driver's "does it build" entry point: (re)builds the library if a source is newer, loads it, checks the ABI
+    """The "does it build" entry point: (re)builds the library if a source is newer, loads it, checks the ABI
     version against the header and imports the oracle -- must hold on a machine without a GPU."""
     import __graft_entry__ as g
     assert g.build() is None

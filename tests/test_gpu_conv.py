@@ -1,4 +1,4 @@
-"""Convolution kernels through the C ABI (yb_conv2d): SIMT fp32 vs torch fp32, tcgen05 fp16 vs the SIMT
+"""Convolution kernels through the C ABI (yb_conv2d): SIMT fp32 vs torch fp32, tensor-core (wgmma) fp16 vs the SIMT
 fp16 kernel (same quantised operands, different summation order) and vs torch on fp16-rounded inputs."""
 import ctypes
 
@@ -113,17 +113,17 @@ TC_CASES = [
 ]
 
 
-# kernel scheduling variants: default heuristic; few persistent CTAs (several tiles per CTA, TMEM double
-# buffering) with the default and with a narrow N tile
+# kernel scheduling variants: default heuristic; few persistent CTAs (several tiles per CTA) with the default and
+# with a narrow N tile
 TC_MODES = {
     "default": {},
     "persistent_grid3": {"YB_CONV2D_GRID": "3"},
     "persistent_grid5_bn64": {"YB_CONV2D_GRID": "5", "YB_CONV2D_BN": "64"},
-    # CTA pairs (cluster of 2, tcgen05 cta_group::2, M = 256): default grid, and 2 clusters walking many units
-    # (TMEM double buffering across the pair, odd M-tile counts -> a padding tile in the last pair)
+    # CTA pairs (cluster of 2 sharing the weight tile by TMA multicast): default grid, and 2 clusters walking many units
+    # (odd M-tile counts -> a padding tile in the last pair)
     "pair": {"YB_CONV2D_PAIR": "1"},
     "pair_grid4_bn128": {"YB_CONV2D_PAIR": "1", "YB_CONV2D_GRID": "4", "YB_CONV2D_BN": "128"},
-    # two epilogue groups (8 epilogue warps, even / odd 64-channel chunks), alone, persistent and with CTA pairs
+    # two MMA warpgroups (each owns 64 rows of the tile), alone, persistent and with CTA pairs
     "epi2": {"YB_CONV2D_EPI": "2"},
     "epi2_grid3_bn256": {"YB_CONV2D_EPI": "2", "YB_CONV2D_GRID": "3", "YB_CONV2D_BN": "256"},
     "pair_epi2": {"YB_CONV2D_PAIR": "1", "YB_CONV2D_EPI": "2"},
@@ -158,8 +158,8 @@ def test_tcgen05_matches_simt_f16_and_torch(ops, case, mode, monkeypatch):
     scale = max(1.0, ref.abs().max().item())
     assert torch.isfinite(y_tc).all()
     # both round the result to fp16 (rel 2^-11): allow 2 ulp of the largest value + accumulation noise
-    assert (y_tc - ref).abs().max() < 3e-3 * scale, "tcgen05 vs torch(fp16 operands)"
-    assert (y_tc - y_simt).abs().max() < 3e-3 * scale, "tcgen05 vs SIMT fp16"
+    assert (y_tc - ref).abs().max() < 3e-3 * scale, "tensor cores vs torch(fp16 operands)"
+    assert (y_tc - y_simt).abs().max() < 3e-3 * scale, "tensor cores vs SIMT fp16"
 
 
 # ---- split precision (YB_PREC_F16X3): fp16 hi+lo operand pairs, three MMA passes -> fp32-equivalent results -----
@@ -195,7 +195,7 @@ def test_tcgen05_split_matches_torch_fp32(ops, case, mode, monkeypatch):
     scale = max(1.0, ref.abs().max().item())
     assert torch.isfinite(y).all()
     err = (y - ref).abs().max().item()
-    assert err < 2e-5 * scale, "split tcgen05 vs torch fp32: %.3e of range" % (err / scale)
+    assert err < 2e-5 * scale, "split tensor cores vs torch fp32: %.3e of range" % (err / scale)
 
 
 def test_tcgen05_split_small_and_large_magnitudes(ops):

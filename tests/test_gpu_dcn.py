@@ -44,13 +44,13 @@ def test_dcn_f16_paths_vs_oracle(C, stride):
     ref = O.dcn_v2_forward(x, off, msk, w, bias, stride, 1, 1)
     t = lambda a: torch.from_numpy(a).cuda()
     y = dcn_v2_conv(t(x), t(off), t(msk), t(w), t(bias), stride, 1, 1, 1, precision="f16tc").cpu().numpy()
-    # C % 64 == 0 -> gather + tcgen05 contraction; else the fused SIMT fp16 kernel.  fp16 operands.
+    # C % 64 == 0 -> gather + tensor-core contraction; else the fused SIMT fp16 kernel.  fp16 operands.
     assert np.abs(y - ref).max() < 1e-2 * max(1.0, np.abs(ref).max())
 
 
 @pytest.mark.parametrize("C,stride", [(64, 1), (128, 2)])
 def test_dcn_split_precision_vs_oracle(C, stride):
-    """YB_PREC_F16X3: gather of hi+lo samples -> split columns -> three-pass tcgen05 contraction; fp32-equivalent."""
+    """YB_PREC_F16X3: gather of hi+lo samples -> split columns -> three-pass tensor-core contraction; fp32-equivalent."""
     r = np.random.RandomState(7 * C + stride)
     B, H, W, Co = 2, 21, 19, 96
     x = r.standard_normal((B, C, H, W)).astype(np.float32)

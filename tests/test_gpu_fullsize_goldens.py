@@ -3,7 +3,7 @@
 yolact_im700@700, yolact_plus_base@550), through the reference-facing API: net(x) in eval mode + postprocess().
 
   * f16x3 (the benched mode): north_star's bar -- class ids identical (ranks may swap only between scores closer than
-    2e-5), boxes / scores within 1e-3 (measured ~1e-5), < 1e-3 mismatching mask pixels, raw heads within 2e-4.
+    2e-5), boxes / scores within 1e-3, < 1e-3 mismatching mask pixels, raw heads within 2e-4.
   * f16tc (fast mode): reported, loosely bounded.
 """
 import numpy as np

@@ -61,7 +61,7 @@ def _worker(rank, world, port, q):
 def test_sharded_run_plus_nccl_gather_equals_single_gpu():
     n = torch.cuda.device_count()
     if n < 2:
-        pytest.skip("needs >= 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs")
     world = 2 if n < 4 else 4
     import torch.multiprocessing as mp
     with socket.socket() as s:

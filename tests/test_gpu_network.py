@@ -1,10 +1,10 @@
 """Whole path through the reference-facing API (yolact_b200.Yolact / postprocess) against the
 reference's golden outputs.
 
-  * precision='f16x3' (split-precision tcgen05, the default and benched mode) and precision='f32' (fp32 CUDA-core
+  * precision='f16x3' (split-precision tensor-core, the default and benched mode) and precision='f32' (fp32 CUDA-core
     second opinion): raw head tensors within 1e-4 of the reference, class ids bit-exact, boxes/scores within 2e-5
     (north_star asks for 1e-3), binarised masks < 1e-3 mismatching pixels.
-  * precision='f16tc' (single-pass fp16 tcgen05, the fast mode): fp16 operands, fp32 accumulation.  Tolerances are
+  * precision='f16tc' (single-pass fp16 tensor-core, the fast mode): fp16 operands, fp32 accumulation.  Tolerances are
     written next to each assert; discrete outputs (class ids, NMS keep set) are reported as agreement
     ratios because they are discontinuous in the scores (SURVEY.md section 7, hard part 1).
 """
@@ -42,8 +42,8 @@ def build(case, precision):
 
 
 EXACT_MODES = ["f16x3", "f32"]
-# measured (profiles/parity_r02.md): f32 (CUDA-core FMA) ~2e-6 of range on the head tensors, f16x3 (split-precision
-# tcgen05: each MMA pass accumulates with the tensor core's own fp32 rounding) ~3e-5; north_star asks for 1e-3.
+# f32 (CUDA-core FMA) and f16x3 (split-precision tensor cores: each MMA pass accumulates with the tensor core's own fp32
+# rounding) both sit far inside these bounds; north_star asks for 1e-3.
 RAW_TOL = {"f32": 1e-4, "f16x3": 2e-4}
 DET_ATOL = {"f32": 2e-5, "f16x3": 2e-4}
 

@@ -1,4 +1,4 @@
-"""Full-size end-to-end parity of the BENCHED precision mode (f16x3, split-precision tcgen05) on the BASELINE.json
+"""Full-size end-to-end parity of the BENCHED precision mode (f16x3, split-precision tensor-core) on the BASELINE.json
 configs: `net(x)` in eval mode + `postprocess()` on the GPU against the CPU oracle (pinned to the reference by the
 goldens), with north_star's bar: class ids identical, boxes / scores within 1e-3, < 1e-3 mismatching mask pixels.
 The single-pass fp16 mode is measured by the same code and only bounded loosely (it is the labelled fast mode)."""

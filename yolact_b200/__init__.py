@@ -1,4 +1,4 @@
-"""yolact_b200 -- B200-native (sm_100a) YOLACT inference path behind the reference's
+"""yolact_b200 -- H100-native (sm_90a) YOLACT inference path behind the reference's
 Yolact.forward() / Detect() / postprocess() surface.  See DESIGN.md and INTEGRATION.md."""
 from .config import cfg, set_cfg, CONFIGS, MEANS, STD  # noqa: F401
 

@@ -1,6 +1,6 @@
 """ctypes binding of libyolact_b200.so (the C ABI in include/yolact_b200.h).
 
-The product path has NO CPU fallback: if the shared library is missing or no B200 is visible the
+The product path has NO CPU fallback: if the shared library is missing or no H100 is visible the
 calls below raise -- they never route to the oracle or to PyTorch ops.
 """
 import ctypes
@@ -112,7 +112,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise YbError(
             "yolact_b200: %s is missing. Build it with `python -m yolact_b200.build` "
-            "(nvcc, sm_100a). There is no CPU fallback." % LIB_PATH)
+            "(nvcc, sm_90a). There is no CPU fallback." % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported

@@ -46,7 +46,7 @@ class FastBaseTransform(torch.nn.Module):
 
     def forward(self, img):
         if not img.is_cuda:
-            raise _lib.YbError("yolact_b200.FastBaseTransform runs on CUDA (B200) only; there is no CPU path.")
+            raise _lib.YbError("yolact_b200.FastBaseTransform runs on CUDA (H100) only; there is no CPU path.")
         if getattr(self.cfg, "channel_order", "RGB") != "RGB":
             raise NotImplementedError   # utils/augmentations.py:648-649
         B, H, W, C = (int(s) for s in img.shape)

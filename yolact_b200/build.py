@@ -1,10 +1,10 @@
-"""In-tree build of the CUDA extension (sm_100a only) and of the C oracle.
+"""In-tree build of the CUDA extension (sm_90a, Hopper H100, only).
 
     python -m yolact_b200.build            # incremental
     python -m yolact_b200.build --force
 
 Produces yolact_b200/libyolact_b200.so (C ABI of include/yolact_b200.h).  nvcc cross-compiles
-without a GPU; the .so is git-ignored but travels to the GPU box with the repo snapshot.
+without a GPU; the .so and the objects are build products (git-ignored).
 """
 import os
 import subprocess
@@ -21,7 +21,7 @@ SOURCES = ["capi.cu", "engine.cu", "tc_conv.cu", "stem_tc.cu", "simt_conv.cu", "
 HEADERS = ["common.cuh", "kernels.cuh", "engine.cuh", "tc_common.cuh", os.path.join(ROOT, "include", "yolact_b200.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-std=c++17", "-O3", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "-Xcompiler", "-fvisibility=hidden",

@@ -1,7 +1,7 @@
 """Configuration snapshot for the inference path.
 
 The reference keeps a global mutable `cfg` (data/config.py:810) that the model both reads and writes
-(yolact.py:425,445,567-568).  The B200 path takes an immutable snapshot of the ~30 keys it needs
+(yolact.py:425,445,567-568).  The H100 path takes an immutable snapshot of the ~30 keys it needs
 (SURVEY.md Appendix C) at construction -- either from one of the named configs below or from any
 object that quacks like the reference's `cfg` (`from_reference_cfg`).
 
@@ -96,7 +96,7 @@ def set_cfg(name):
 def from_reference_cfg(rcfg):
     """Snapshot a reference-style cfg object (duck-typed) into this package's Config.
 
-    Asserts the combination of switches the B200 path implements (every published config satisfies
+    Asserts the combination of switches the H100 path implements (every published config satisfies
     it); anything else must keep using the reference graph.
     """
     b = rcfg.backbone

@@ -145,7 +145,7 @@ struct TempPool {  // RAII device temporaries for the op-level hooks
   }
 };
 
-inline int grid1d(int64_t n) { return (int)std::min<int64_t>(148 * 16, (n + 255) / 256); }
+inline int grid1d(int64_t n) { return (int)std::min<int64_t>(132 * 16, (n + 255) / 256); }
 
 }  // namespace
 
@@ -176,14 +176,13 @@ int yb_create(const yb_config* cfg, int device, yb_handle** out) {
   YB_REQUIRE(device >= 0 && device < n, "yb_create: bad device index");
   cudaDeviceProp prop;
   YB_CHECK_CUDA(cudaGetDeviceProperties(&prop, device));
-  YB_REQUIRE(prop.major == 10, "yb_create: this library is built for sm_100a (Blackwell B200) only");
+  YB_REQUIRE(prop.major == 9 && prop.minor == 0, "yb_create: this library is built for sm_90a (Hopper H100) only");
   std::unique_ptr<yb_handle> h(new yb_handle());
   h->cfg = *cfg;
   h->device = device;
   h->ops_only = (cfg->backbone == YB_BACKBONE_NONE);
-  // measured defaults (profiles/r2_*): programmatic dependent launch gains 3.6 % of the conv stack in the single-pass
-  // fp16 mode and loses 1.5 % in the split mode (whose plans fill the SM, nothing can become resident early); stream-K
-  // gains 1.6 % in the split mode and nothing in the fp16 mode
+  // defaults: programmatic dependent launch in the single-pass fp16 mode, stream-K candidates in the split mode (whose
+  // plans fill the SM, so nothing can become resident early).  Not measured on the H100; YB_PDL / YB_SK switch them.
   h->pdl = (cfg->precision == YB_PREC_F16TC);
   h->sk_candidates = (cfg->precision == YB_PREC_F16X3);
   if (const char* at = getenv("YB_AUTOTUNE")) h->autotune = (atoi(at) != 0);
@@ -662,7 +661,7 @@ int yb_conv2d(yb_handle* h, const float* d_x, const float* h_w, const float* h_b
   YB_API_BEGIN
   YB_REQUIRE(h && d_x && h_w && d_y, "yb_conv2d: null argument");
   YB_REQUIRE(precision >= 0 && precision <= 3,
-             "yb_conv2d: precision must be 0 (f32 simt), 1 (f16 tcgen05), 2 (f16 simt), 3 (split-precision tcgen05)");
+             "yb_conv2d: precision must be 0 (f32 simt), 1 (f16 tensor cores), 2 (f16 simt), 3 (split-precision tensor cores)");
   const int sp = (precision == 3) ? 1 : 0;
   CallGuard g(h);
   cudaStream_t s = (cudaStream_t)stream;
@@ -711,7 +710,7 @@ int yb_conv2d(yb_handle* h, const float* d_x, const float* h_w, const float* h_b
   std::function<void()> run;
   TcConvPlan* plan = nullptr;
   if (precision == 1 || precision == 3) {
-    YB_REQUIRE(tc_conv_supported(p), "yb_conv2d: shape not supported by the tcgen05 kernel (Cin % 64, taps <= 9)");
+    YB_REQUIRE(tc_conv_supported(p), "yb_conv2d: shape not supported by the tensor-core kernel (Cin % 64, taps <= 9)");
     std::vector<__half> pk(K * Co * (sp ? 2 : 1));
     if (sp) {
       float mx = 0.f;

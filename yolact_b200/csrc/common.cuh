@@ -1,4 +1,4 @@
-// Shared helpers for the yolact_b200 CUDA sources (sm_100a only).
+// Shared helpers for the yolact_b200 CUDA sources (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -72,10 +72,10 @@ __device__ __forceinline__ __half from_f32<__half>(float v) {
 // Split-precision operands (YB_PREC_F16X3): a value v is stored as a pair of fp16 numbers (hi, lo') with
 //     hi = rn(v),   lo' = rn((v - hi) * 2^11),   v ~= hi + lo' * 2^-11        (22 significand bits).
 // The lo plane is kept PRE-SCALED by 2^11: the unscaled residual (<= 2^-12 |v|) is an fp16 SUBNORMAL for every
-// |v| < 0.25 and the tensor core flushes fp16 subnormal inputs to zero (measured: head tensors 5e-5 of range off, the
-// arithmetic's own bound is 1e-7), and tcgen05.mma kind::f16 rejects a bf16 A with an fp16 B (illegal instruction), so
-// a wider-exponent lo format is not an option.  The kernels therefore accumulate the two cross terms
-// lo'_a * hi_w + hi_a * lo'_w in a SECOND fp32 TMEM accumulator and combine  acc_hi + 2^-11 * acc_lo  in the epilogue.
+// |v| < 0.25 and the tensor core flushes fp16 subnormal inputs to zero, and the fp16 MMA takes both operands in the
+// same 16-bit format (no bf16 A with an fp16 B), so a wider-exponent lo format is not an option.  The kernels therefore
+// accumulate the two cross terms lo'_a * hi_w + hi_a * lo'_w in a SECOND fp32 accumulator and combine
+// acc_hi + 2^-11 * acc_lo  in the epilogue.
 // Weights are additionally multiplied by a per-layer power of two (engine.cu split_exponent) so that hi uses the upper
 // fp16 exponent range.  A pixel of a split NHWC tensor is [hi(C) | lo'(C)], i.e. 2*C halfs.
 #define YB_LO_SCALE 2048.f

@@ -11,11 +11,9 @@
 //  * launch_dcn_simt: fully fused gather + contraction on CUDA cores (fp32 parity mode, and the
 //    on-device second opinion for the tensor-core path).
 //  * launch_dcn_gather_f16: gather to fp16 NHWC columns [B,Ho,Wo,9*C] (2 B/element instead of
-//    4, channel-contiguous 16-byte stores) consumed by the tcgen05 kernel as a 1x1 conv, K = 9*C.
-//    Round-1 path, kept behind YB_DCN_FUSED=0 as the A/B partner of the fused kernel (dcn_tc.cu), which is the default:
-//    one launch, no column buffer, 4.6 % faster on yolact_plus_base (profiles/r2_call4_summary.txt).  (A
-//    warp-cooperative variant of this gather was validated in round 2 -- +2.8 % -- and removed: the fused kernel
-//    supersedes it.)
+//    4, channel-contiguous 16-byte stores) consumed by the tensor-core kernel as a 1x1 conv, K = 9*C.
+//    Kept behind YB_DCN_FUSED=0 as the A/B partner of the fused kernel (dcn_tc.cu), which is the default: one launch,
+//    no column buffer.
 #include <stdlib.h>
 #include <string>
 #include "kernels.cuh"
@@ -263,7 +261,7 @@ void launch_dcn_gather_f16(const __half* x, const float* om, __half* cols, int B
   YB_REQUIRE(C % 8 == 0, "dcn gather: C must be a multiple of 8");
   const int64_t total = (int64_t)B * Ho * Wo * 9 * (C / 8);
   int64_t g = (total + 255) / 256;
-  if (g > 148 * 32) g = 148 * 32;
+  if (g > 132 * 32) g = 132 * 32;
   dcn_gather_f16_kernel<<<(unsigned)g, 256, 0, stream>>>(x, om, cols, B, H, W, C, Ho, Wo, stride, pad, dil, mask_logits, split);
   YB_CHECK_LAUNCH();
   if (lc) lc->n++;

@@ -1,26 +1,25 @@
-// Fused DCNv2 (modulated deformable 3x3 convolution, deformable_groups = 1) on tcgen05: deformable gather ->
+// Fused DCNv2 (modulated deformable 3x3 convolution, deformable_groups = 1) on the tensor cores (wgmma): deformable gather ->
 // shared-memory A stage -> tensor-core contraction -> bias + ReLU, ONE kernel, no column buffer.
 //
 // Reference: DCN.forward (external/DCNv2/dcn_v2.py:118-128), modulated_deformable_im2col_gpu_kernel
 // (external/DCNv2/src/cuda/dcn_v2_im2col_cuda.cu:125-195, bilinear sampler :25-54) followed by the batched SGEMM + bias
 // of dcn_v2_cuda_forward (src/cuda/dcn_v2_cuda.cu:123-163).  The reference materialises the sampled columns
-// [B, 9*C, Ho*Wo] fp32 in HBM between the two; round 1 of this repo wrote them as fp16 (88 MB per layer at 69x69) and ran
-// a 1x1 tensor-core conv over them.  Here they never leave the SM:
+// [B, 9*C, Ho*Wo] fp32 in HBM between the two (the YB_DCN_FUSED=0 path of dcn.cu writes them as fp16 and runs a 1x1
+// tensor-core conv over them).  Here they never leave the SM:
 //
 //   GEMM view   D[128 output pixels, BN couts] = sum over taps t (9) and 64-channel chunks kc of
 //               A_t,kc[128, 64] * W[BN, t*C + kc*64 .. +64]^T,
 //               A_t,kc[m, c] = mask(m,t) * bilinear(x, pos(m,t))[kc*64 + c]          (fp32 math, reference op order)
-//   warp 0      TMA producer of the weight tiles (B operand, [Cout][9*C] K-major)
-//   warp 1      TMEM allocation + single-thread tcgen05.mma issue, tcgen05.commit frees the stage
-//   warps 2..9  gather: warp w owns 16 tile rows.  Once per tap, lanes 0..15 each compute the sampling geometry of ONE
+//   warp 8      TMA producer of the weight tiles (B operand, [Cout][9*C] K-major)
+//   warps 0..7  two warpgroups; each gathers the A rows of its 64-row half of the tile and multiplies them with wgmma
+//               while it gathers the next k-block.  Gather: warp w owns 16 tile rows.  Once per tap, lanes 0..15 each compute the sampling geometry of ONE
 //               row (4 corner offsets, 4 bilinear weights, the modulation mask) from the 27 offset/mask channels; for
 //               every 64-channel chunk the geometry reaches the lanes that need it by WARP SHUFFLE (8 lanes share a
 //               row: one 16-byte vector of 8 channels each), the four corners are fetched with 16-byte loads, blended
 //               (fp32 in the split mode, packed half2 in the fp16 mode) and written as one swizzled 16-byte piece of the K-major SWIZZLE_128B A tile -- the layout
-//               tcgen05.mma consumes directly.  Geometry is computed once per (pixel, tap) instead of once per
+//               wgmma consumes directly.  Geometry is computed once per (pixel, tap) instead of once per
 //               (pixel, tap, 8 channels) as in the per-thread gather.
-//   epilogue    the same 8 warps: TMEM -> registers -> (* out_scale) + bias -> ReLU -> one full 128-byte line per
-//               thread and 64-channel chunk (even chunks: warps 2..5, odd chunks: warps 6..9).
+//   epilogue    each warpgroup: accumulator registers -> (* out_scale) + bias -> ReLU -> its rows' channel pairs.
 //   SPLIT       (YB_PREC_F16X3) x and y are [hi(C) | lo(C)] pairs, the sample is hi + lo, the A stage holds a hi (fp16)
 //               and a lo (2^11-scaled fp16) tile, the weights [Cout][hi(9C) | lo(9C)], three MMA passes per k-block.
 #include "tc_common.cuh"
@@ -35,7 +34,7 @@ constexpr int DM = 128;                 // tile rows (output pixels)
 constexpr int DK = 64;                  // channels per k-block (one 128-byte swizzle row)
 constexpr int A_TILE = DM * DK * 2;     // 16 KB
 constexpr int GATHER_WARPS = 8;
-constexpr int DTHREADS = 64 + 32 * GATHER_WARPS;
+constexpr int DTHREADS = 32 * GATHER_WARPS + 32;
 constexpr int MAX_DSTAGES = 6;
 
 struct alignas(64) DcnParams {
@@ -49,7 +48,6 @@ struct alignas(64) DcnParams {
   int stride, pad, dil;
   int act, mask_logits;
   int stages, kchunks;
-  uint32_t idesc;
   float out_scale;
 };
 
@@ -68,10 +66,10 @@ dcn_tc_kernel(const __grid_constant__ DcnParams p) {
   constexpr int NPL = SPLIT ? 2 : 1;
   constexpr int B_PLANE = BN * DK * 2;
   constexpr int STAGE = NPL * (A_TILE + B_PLANE);
+  static_assert(NPL * BN / 2 <= 128, "accumulator tile exceeds the register budget");
 
   extern __shared__ uint8_t smem_dyn[];
-  __shared__ uint64_t a_full[MAX_DSTAGES], b_full[MAX_DSTAGES], empty_bar[MAX_DSTAGES], tmem_full;
-  __shared__ uint32_t s_tmem;
+  __shared__ uint64_t b_full[MAX_DSTAGES], empty_bar[MAX_DSTAGES];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -82,21 +80,15 @@ dcn_tc_kernel(const __grid_constant__ DcnParams p) {
 
   if (tid == 0) {
     for (int s = 0; s < stages; ++s) {
-      mbar_init(&a_full[s], GATHER_WARPS);
       mbar_init(&b_full[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);   // both warpgroups have read the weight tile
     }
-    mbar_init(&tmem_full, 1);
     fence_barrier_init();
     tma_prefetch_desc(&p.tmW);
   }
-  if (warp == 1) tmem_alloc<NPL * BN>(&s_tmem);   // split: second accumulator for the lo cross terms (common.cuh)
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
 
-  if (warp == 0) {
+  if (warp == GATHER_WARPS) {
     // ===================== weight tiles (TMA) =====================
     if (lane == 0) {
       for (int kb = 0; kb < num_kb; ++kb) {
@@ -110,36 +102,15 @@ dcn_tc_kernel(const __grid_constant__ DcnParams p) {
           tma_load_3d(sb + pl * B_PLANE, &p.tmW, &b_full[s], tap * p.C + kc * DK + pl * 9 * p.C, n0, 0);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % stages, it = kb / stages;
-        mbar_wait(&b_full[s], (uint32_t)(it & 1));
-        mbar_wait(&a_full[s], (uint32_t)(it & 1));
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + (size_t)s * STAGE);
-        const uint32_t sb = sa + NPL * A_TILE;
-        const uint64_t da = make_sw128_desc(sa), db = make_sw128_desc(sb);
-#pragma unroll
-        for (int k = 0; k < DK / 16; ++k)
-          umma_f16(tmem_base, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), p.idesc, (kb > 0 || k > 0) ? 1u : 0u);
-        if (SPLIT) {
-          const uint64_t dal = make_sw128_desc(sa + A_TILE), dbl = make_sw128_desc(sb + B_PLANE);
-#pragma unroll
-          for (int k = 0; k < DK / 16; ++k)   // A_lo * W_hi -> second accumulator
-            umma_f16(tmem_base + BN, dal + (uint64_t)(2 * k), db + (uint64_t)(2 * k), p.idesc, (kb > 0 || k > 0) ? 1u : 0u);
-#pragma unroll
-          for (int k = 0; k < DK / 16; ++k)   // A_hi * W_lo -> second accumulator
-            umma_f16(tmem_base + BN, da + (uint64_t)(2 * k), dbl + (uint64_t)(2 * k), p.idesc, 1u);
-        }
-        umma_commit(&empty_bar[s]);
-      }
-      umma_commit(&tmem_full);
-    }
   } else {
     // ===================== gather warps =====================
-    const int gw = warp - 2;                        // 0..7: rows [16*gw, 16*gw + 16)
+    const int gw = warp;                            // 0..7: rows [16*gw, 16*gw + 16)
+    const int wgi = warp >> 2;                      // warpgroup: rows [64*wgi, 64*wgi + 64)
+    float acc[NPL][BN / 2];
+#pragma unroll
+    for (int pl = 0; pl < NPL; ++pl)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[pl][i] = 0.f;
     const int PS = NPL * p.C;                       // halfs per input pixel
     // geometry owner: lanes 0..15 <-> row 16*gw + lane
     const long long gm = m0 + gw * 16 + (lane & 15);
@@ -160,7 +131,7 @@ dcn_tc_kernel(const __grid_constant__ DcnParams p) {
     // Corner offsets are ALWAYS valid addresses (an out-of-range corner points at this image's pixel 0 and carries
     // weight 0, which is what the reference's `if (h_low >= 0 && ...) v = ...` amounts to): the corner loads of a
     // k-block are then unconditional and the compiler issues them back to back -- with a branch per corner every load
-    // waited for the previous one (measured: 3.4 us per k-block, 124 us for a 35x35 layer).
+    // would wait for the previous one.
     // The modulation mask is folded into the four bilinear weights (one rounding of difference to the reference's
     // (sum) * mask, far below the fp16 / split resolution).
     int ao[4][4];        // [item][corner] pixel offsets of this lane's 4 rows, refreshed once per tap by shuffle
@@ -222,7 +193,7 @@ dcn_tc_kernel(const __grid_constant__ DcnParams p) {
           }
         }
       }
-      mbar_wait(&empty_bar[s], (uint32_t)(it & 1) ^ 1u);   // the MMAs that read this stage have completed
+      // (this warpgroup's wgmmas of k-block kb - stages have completed: at most one group is in flight, stages >= 2)
       uint8_t* sa = smem + (size_t)s * STAGE;
       const __half* xc = p.x + kc * DK + piece * 8;
       if (!SPLIT) {
@@ -280,79 +251,73 @@ dcn_tc_kernel(const __grid_constant__ DcnParams p) {
           *reinterpret_cast<uint4*>(sa + A_TILE + off) = ol;
         }
       }
-      fence_proxy_async();   // generic-proxy smem writes -> visible to tcgen05.mma (async proxy)
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&a_full[s]);
+      fence_proxy_async();   // generic-proxy smem writes -> visible to wgmma (async proxy)
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wgi) : "memory");   // the warpgroup's 64 rows are staged
+      mbar_wait(&b_full[s], (uint32_t)(it & 1));
+      {
+        const uint32_t sa32 = smem_u32(sa) + (uint32_t)wgi * (64u * 128u);
+        const uint32_t sb32 = smem_u32(sa) + (uint32_t)(NPL * A_TILE);
+        const uint64_t da = make_sw128_desc(sa32), db = make_sw128_desc(sb32);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < DK / 16; ++k) Wgmma<BN>::mma(acc[0], da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1u);
+        if (SPLIT) {
+          const uint64_t dal = make_sw128_desc(sa32 + A_TILE), dbl = make_sw128_desc(sb32 + B_PLANE);
+#pragma unroll
+          for (int k = 0; k < DK / 16; ++k)   // A_lo * W_hi -> second accumulator
+            Wgmma<BN>::mma(acc[NPL - 1], dal + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1u);
+#pragma unroll
+          for (int k = 0; k < DK / 16; ++k)   // A_hi * W_lo -> second accumulator
+            Wgmma<BN>::mma(acc[NPL - 1], da + (uint64_t)(2 * k), dbl + (uint64_t)(2 * k), 1u);
+        }
+        wgmma_commit();
+      }
+      if (kb > 0) {   // k-block kb - 1 has been read: its weight tile can be refilled
+        wgmma_wait<1>();
+        if ((tid & 127) == 0) mbar_arrive(&empty_bar[(kb - 1) % stages]);
+      }
     }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int pl = 0; pl < NPL; ++pl) fence_regs<BN / 2>(acc[pl]);
 
     // ===================== epilogue =====================
-    mbar_wait(&tmem_full, 0);
-    tc_fence_after();
-    const int quad = warp & 3;
-    const int hgrp = (warp - 2) >> 2;               // warps 2..5: even 64-channel chunks, warps 6..9: odd chunks
-    const int row = quad * 32 + lane;
-    const long long m = m0 + row;
-    const int nchunks = (min(BN, p.Cout - n0) + 63) >> 6;
-    __half* yrow = p.y + m * (long long)(NPL * p.Cout) + n0;
-    for (int c = hgrp; c < nchunks; c += 2) {
-      uint32_t r0[32], r1[32];
-      tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(c * 64), r0);
-      tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(c * 64 + 32), r1);
-      if (SPLIT) {
-        uint32_t q2[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(BN + c * 64), q2);
+    const int wq = warp & 3;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) r0[j] = __float_as_uint(__fmaf_rn(__uint_as_float(q2[j]), YB_LO_INV, __uint_as_float(r0[j])));
-        tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(BN + c * 64 + 32), q2);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) r1[j] = __float_as_uint(__fmaf_rn(__uint_as_float(q2[j]), YB_LO_INV, __uint_as_float(r1[j])));
-      }
+    for (int hh = 0; hh < 2; ++hh) {
+      const int row = wgi * 64 + wq * 16 + (lane >> 2) + 8 * hh;
+      const long long m = m0 + row;
       if (m >= p.M) continue;
+      __half* yrow = p.y + m * (long long)(NPL * p.Cout) + n0;
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        uint4 o, ol;
-        __half2* o2 = reinterpret_cast<__half2*>(&o);
-        __half2* ol2 = reinterpret_cast<__half2*>(&ol);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int col = q * 8 + 2 * j;
-          const int ch = n0 + c * 64 + col;
-          float v0 = __uint_as_float(col < 32 ? r0[col] : r1[col - 32]);
-          float v1 = __uint_as_float(col + 1 < 32 ? r0[col + 1] : r1[col + 1 - 32]);
-          if (SPLIT) {
-            v0 *= p.out_scale;
-            v1 *= p.out_scale;
-          }
-          v0 = apply_act(v0 + ((p.bias && ch < p.Cout) ? __ldg(p.bias + ch) : 0.f), p.act);
-          v1 = apply_act(v1 + ((p.bias && ch + 1 < p.Cout) ? __ldg(p.bias + ch + 1) : 0.f), p.act);
-          const float c0 = fminf(fmaxf(v0, -65504.f), 65504.f), c1 = fminf(fmaxf(v1, -65504.f), 65504.f);
-          o2[j] = __floats2half2_rn(c0, c1);
-          if (SPLIT) {
-            const float2 hf = __half22float2(o2[j]);
-            ol2[j] = lo2_from_f32(c0 - hf.x, c1 - hf.y);
-          }
+      for (int j = 0; j < BN / 8; ++j) {
+        if (n0 + 8 * j >= p.Cout) break;   // Cout % 8 == 0 is required by the launcher
+        const int col = 8 * j + 2 * (lane & 3);
+        const int ch = n0 + col;
+        const int i = 4 * j + 2 * hh;
+        float v0 = acc[0][i], v1 = acc[0][i + 1];
+        if (SPLIT) {
+          v0 = __fmaf_rn(acc[NPL - 1][i], YB_LO_INV, v0) * p.out_scale;
+          v1 = __fmaf_rn(acc[NPL - 1][i + 1], YB_LO_INV, v1) * p.out_scale;
         }
-        const int cbase = c * 64 + q * 8;
-        if (n0 + cbase + 8 <= p.Cout) {   // Cout % 8 == 0 is required by the launcher
-          *reinterpret_cast<uint4*>(yrow + cbase) = o;
-          if (SPLIT) *reinterpret_cast<uint4*>(yrow + p.Cout + cbase) = ol;
+        v0 = apply_act(v0 + (p.bias ? __ldg(p.bias + ch) : 0.f), p.act);
+        v1 = apply_act(v1 + (p.bias ? __ldg(p.bias + ch + 1) : 0.f), p.act);
+        const float c0 = fminf(fmaxf(v0, -65504.f), 65504.f), c1 = fminf(fmaxf(v1, -65504.f), 65504.f);
+        const __half2 o = __floats2half2_rn(c0, c1);
+        *reinterpret_cast<__half2*>(yrow + col) = o;
+        if (SPLIT) {
+          const float2 hf = __half22float2(o);
+          *reinterpret_cast<__half2*>(yrow + p.Cout + col) = lo2_from_f32(c0 - hf.x, c1 - hf.y);
         }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<NPL * BN>(tmem_base);
-  }
 }
-
 template <int BN, bool SPLIT>
 void launch_dcn_variant(const DcnParams& prm, size_t smem, dim3 grid, cudaStream_t stream) {
   static PerDeviceOnce attr;
   if (attr.first())
-    YB_CHECK_CUDA(cudaFuncSetAttribute(dcn_tc_kernel<BN, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(224 * 1024)));
+    YB_CHECK_CUDA(cudaFuncSetAttribute(dcn_tc_kernel<BN, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(226 * 1024)));
   dcn_tc_kernel<BN, SPLIT><<<grid, DTHREADS, smem, stream>>>(prm);
 }
 
@@ -360,7 +325,7 @@ void launch_dcn_variant(const DcnParams& prm, size_t smem, dim3 grid, cudaStream
 
 struct DcnTcPlan {
   DcnParams prm;
-  int BN = 256;
+  int BN = 128;
   int split = 0;
   size_t smem = 0;
   dim3 grid;
@@ -378,8 +343,9 @@ DcnTcPlan* dcn_tc_plan_create(const __half* x, const float* om, const __half* w_
   memset(&q, 0, sizeof(q));
   plan->split = split ? 1 : 0;
   const int npl = split ? 2 : 1;
-  int BN = Cout >= 256 ? 256 : (Cout > 64 ? 128 : 64);
-  if (bn_override == 64 || bn_override == 128 || bn_override == 256) BN = bn_override;
+  // N tile <= 128: the accumulators of a 64-row half stay within 128 registers per thread in both modes
+  int BN = Cout > 64 ? 128 : 64;
+  if (bn_override == 64 || bn_override == 128) BN = bn_override;
   plan->BN = BN;
   q.x = x;
   q.om = om;
@@ -400,10 +366,9 @@ DcnTcPlan* dcn_tc_plan_create(const __half* x, const float* om, const __half* w_
   q.mask_logits = mask_logits;
   q.kchunks = C / DK;
   q.out_scale = split ? out_scale : 1.f;
-  q.idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(DM >> 4) << 24);
   const int stage = npl * (A_TILE + BN * DK * 2);
-  int stages = std::min(MAX_DSTAGES, (221 * 1024) / stage);
-  stages = std::max(1, std::min(stages, 9 * q.kchunks));
+  int stages = std::min(MAX_DSTAGES, (225 * 1024) / stage);
+  stages = std::max(2, std::min(stages, 9 * q.kchunks));   // >= 2: a warpgroup keeps one wgmma group in flight
   q.stages = stages;
   plan->smem = (size_t)stages * stage + 1024;
   plan->grid = dim3((unsigned)((q.M + DM - 1) / DM), (unsigned)ceil_div(Cout, BN), 1);
@@ -421,13 +386,11 @@ void launch_dcn_tc(const DcnTcPlan* plan, cudaStream_t stream, LaunchCounter* lc
   const DcnParams& q = plan->prm;
   if (plan->split) {
     switch (plan->BN) {
-      case 256: launch_dcn_variant<256, true>(q, plan->smem, plan->grid, stream); break;
       case 128: launch_dcn_variant<128, true>(q, plan->smem, plan->grid, stream); break;
       default: launch_dcn_variant<64, true>(q, plan->smem, plan->grid, stream); break;
     }
   } else {
     switch (plan->BN) {
-      case 256: launch_dcn_variant<256, false>(q, plan->smem, plan->grid, stream); break;
       case 128: launch_dcn_variant<128, false>(q, plan->smem, plan->grid, stream); break;
       default: launch_dcn_variant<64, false>(q, plan->smem, plan->grid, stream); break;
     }

@@ -91,7 +91,7 @@ void launch_multi_copy(const void* const* src, void* const* dst, const size_t* b
     s.n++;
   }
   if (s.n == 0) return;
-  int gx = (int)std::min<size_t>(148 * 8, (mx / 16 + 255) / 256 + 1);
+  int gx = (int)std::min<size_t>(132 * 8, (mx / 16 + 255) / 256 + 1);
   multi_copy_kernel<<<dim3(gx, s.n), 256, 0, stream>>>(s);
   YB_CHECK_LAUNCH();
   if (lc) lc->n++;
@@ -174,7 +174,7 @@ struct NetBuilder {
   yb_handle* h;
   Executor* ex;
   bool dry;
-  bool f16;     // fp16 storage + tcgen05 kernels (YB_PREC_F16TC and YB_PREC_F16X3)
+  bool f16;     // fp16 storage + tensor-core kernels (YB_PREC_F16TC and YB_PREC_F16X3)
   bool split;   // YB_PREC_F16X3: split-precision activations / weights, three MMA passes
   int lane = 0;
   void push(Op& op) {
@@ -221,7 +221,7 @@ struct NetBuilder {
     p.x = in.ptr;
     p.x_nchw_f32 = in_nchw ? 1 : 0;
     p.split = in.split ? 1 : 0;
-    // in.C may be a zero-padded channel count (the tcgen05 stem pads a 32-channel output to 64, see stem_tc)
+    // in.C may be a zero-padded channel count (the tensor-core stem pads a 32-channel output to 64, see stem_tc)
     const bool tc = f16 && !in_nchw && (in.C % 64 == 0) && !in.f32;
     YB_REQUIRE(!split || tc || in_nchw, ("conv " + key + ": the split-precision mode has tensor-core kernels only").c_str());
     const bool simt_half = f16 && !tc && !in.f32;
@@ -231,7 +231,7 @@ struct NetBuilder {
                        : h->get_conv(key, bn, /*want_tc=*/tc, /*want_f32=*/!tc && !simt_half, /*want_f16=*/simt_half, 0,
                                      /*cin_pad=*/tc ? in.C : 0,
                                      // a half-precision output narrower than 64 channels (Darknet's first block: 32)
-                                     // is written as zero-padded 64-channel pixels for the tcgen05 conv that follows
+                                     // is written as zero-padded 64-channel pixels for the tensor-core conv that follows
                                      /*cout_pad=*/(tc && !out_f32 && !ospec && !residual) ? ((h->peek_cout(key) + 63) / 64) * 64 : 0);
     YB_REQUIRE((w.Cin == in.C || (tc && w.cin_pad == in.C)) && w.KH == k && w.KW == k,
                ("conv " + key + ": weight shape mismatch").c_str());
@@ -252,7 +252,7 @@ struct NetBuilder {
       p.y_batch_stride = ospec->batch_stride;
       p.y_pix_stride = ospec->pix_stride;
     } else {
-      // the tcgen05 stem zero-pads its pixels to a multiple of 64 channels for the tensor-core conv that follows
+      // the tensor-core stem zero-pads its pixels to a multiple of 64 channels for the tensor-core conv that follows
       const int out_c = stem_tc ? ((w.Cout + 63) / 64) * 64 : cout_eff;
       out = alloc_act(in.B, p.Ho, p.Wo, out_c, out_f32);
       p.y = out.ptr;
@@ -375,7 +375,7 @@ struct NetBuilder {
       };
       push(op);
     } else if (h->dcn_fused && dcn_tc_supported(in.C, w.Cout)) {
-      // one kernel: warp-shuffled tap geometry -> bilinear samples straight into the swizzled A stage -> tcgen05
+      // one kernel: warp-shuffled tap geometry -> bilinear samples straight into the swizzled A stage -> wgmma
       const int sp = in.split ? 1 : 0;
       DcnTcPlan* dp = dcn_tc_plan_create((const __half*)in.ptr, (const float*)om.ptr, w.w_tc, w.bias, (__half*)out.ptr, in.B,
                                          in.H, in.W, in.C, Ho, Wo, w.Cout, stride, 1, 1, ACT_RELU, 1, sp, w.out_scale);
@@ -387,7 +387,7 @@ struct NetBuilder {
       op.fn = [dp, lc](cudaStream_t s) { launch_dcn_tc(dp, s, lc); };
       push(op);
     } else {
-      // gather -> fp16 columns [B,Ho,Wo,9C]; contraction = 1x1 conv with K = 9C on tcgen05
+      // gather -> fp16 columns [B,Ho,Wo,9C]; contraction = 1x1 conv with K = 9C on the tensor cores
       Act cols = alloc_act(in.B, Ho, Wo, 9 * in.C);
       Op g;
       g.is_conv = true;
@@ -501,7 +501,7 @@ struct NetBuilder {
         return nullptr;
       TcConvPlan* pl = nullptr;
       try {
-        pl = tc_conv_plan_create(q, op.w_tc, (q.Cout % 128 == 0) ? 128 : 64, 2, 148, 0, 2, 0, 0, /*chain=*/1);
+        pl = tc_conv_plan_create(q, op.w_tc, (q.Cout % 128 == 0) ? 128 : 64, 2, 0, 0, 2, 0, 0, /*chain=*/1);
       } catch (const Error&) {
         return nullptr;
       }
@@ -509,9 +509,6 @@ struct NetBuilder {
         tc_conv_plan_destroy(pl);
         return nullptr;
       }
-      // (64-wide tiles for the layers with fewer than two rounds of 128-wide ones -- so that the tiles their consumers
-      // wait for were written two rounds earlier -- halve the dependency waits but lose overall: 4.35 vs 3.74 ms for the
-      // trunk chain, profiles/r2_call19_summary.txt)
       return pl;
     };
     size_t i = begin;
@@ -552,8 +549,7 @@ struct NetBuilder {
           }
         }
       }
-      // candidates: two epilogue groups + three operand stages, or four groups + two stages (split precision); timed
-      // against the separately tuned launches
+      // the chain, timed against the separately tuned launches
       TcChain* chain = nullptr;
       bool use = false;
       {
@@ -573,35 +569,18 @@ struct NetBuilder {
           return ms / 5.f;
         };
         float ms_chain = 1e30f;
-        // measured (profiles/r2_call16_summary.txt): four groups + two stages lose to two groups + three stages on every
-        // chain of every config, so only YB_CHAIN_GROUPS=4 / =0 (time both) still builds the four-group variant
-        const int force_groups = getenv("YB_CHAIN_GROUPS") ? atoi(getenv("YB_CHAIN_GROUPS")) : 2;
-        for (int groups = 2; groups <= 4; groups += 2) {
-          if (force_groups && groups != force_groups) continue;
-          TcChain* cand = nullptr;
-          try {
-            cand = tc_chain_create(cpl, dep_a, dep_r, groups);
-          } catch (const Error&) {
-            cand = nullptr;
-          }
-          if (cand && !tc_chain_graph_ok(cand)) {   // cooperative launches cannot be captured here: no chains
-            tc_chain_destroy(cand);
-            cand = nullptr;
-          }
-          if (!cand) continue;
-          const float ms = time_it([&]() { launch_tc_chain(cand, 0, nullptr); });
-          if (getenv("YB_CHAIN_STATS")) {
-            const std::string nm = ops[i].name.substr(0, ops[i].name.find(' ')) + " groups=" + std::to_string(groups);
-            tc_chain_print_stats(cand, nm.c_str());
-          }
-          if (getenv("YB_CHAIN_VERBOSE")) fprintf(stderr, "[yolact_b200]   %d epilogue groups: %.3f ms\n", groups, ms);
-          if (ms < ms_chain) {
-            if (chain) tc_chain_destroy(chain);
-            chain = cand;
-            ms_chain = ms;
-          } else {
-            tc_chain_destroy(cand);
-          }
+        try {
+          chain = tc_chain_create(cpl, dep_a, dep_r);
+        } catch (const Error&) {
+          chain = nullptr;
+        }
+        if (chain && !tc_chain_graph_ok(chain)) {   // cooperative launches cannot be captured here: no chains
+          tc_chain_destroy(chain);
+          chain = nullptr;
+        }
+        if (chain) {
+          ms_chain = time_it([&]() { launch_tc_chain(chain, 0, nullptr); });
+          if (getenv("YB_CHAIN_STATS")) tc_chain_print_stats(chain, ops[i].name.substr(0, ops[i].name.find(' ')).c_str());
         }
         if (chain) {
           const float ms_sep = time_it([&]() {
@@ -609,9 +588,9 @@ struct NetBuilder {
           });
           use = (h->chain_mode == 2) || ms_chain < ms_sep;
           if (getenv("YB_CHAIN_VERBOSE"))
-            fprintf(stderr, "[yolact_b200] chain %s .. %s (%zu layers): chain %.3f ms (%d groups), separate %.3f ms -> %s\n",
+            fprintf(stderr, "[yolact_b200] chain %s .. %s (%zu layers): chain %.3f ms, separate %.3f ms -> %s\n",
                     ops[i].name.substr(0, ops[i].name.find(' ')).c_str(), ops[k - 1].name.substr(0, ops[k - 1].name.find(' ')).c_str(), n,
-                    ms_chain, tc_chain_groups(chain), ms_sep, use ? "chain" : "separate");
+                    ms_chain, ms_sep, use ? "chain" : "separate");
         }
         h->lc.n = lc_before;   // (the separate launches counted themselves)
         cudaEventDestroy(e0);
@@ -629,7 +608,7 @@ struct NetBuilder {
       op.is_conv = true;
       op.lane = ops[i].lane;
       op.name = "chain x" + std::to_string(n) + " [" + ops[i].name.substr(0, ops[i].name.find(' ')) + " .. " +
-                ops[k - 1].name.substr(0, ops[k - 1].name.find(' ')) + "] tc BN=128/64 g=148 epi" + std::to_string(tc_chain_groups(chain));
+                ops[k - 1].name.substr(0, ops[k - 1].name.find(' ')) + "] tc BN=128/64";
       {
         double gf = 0.0;
         for (size_t j = i; j < k; ++j) {
@@ -660,7 +639,7 @@ struct NetBuilder {
     return ws;
   }
 
-  // Plan-time autotuning of the tcgen05 kernel's N tile and pipeline depth: each candidate is timed on the
+  // Plan-time autotuning of the tensor-core kernel's N tile and pipeline depth: each candidate is timed on the
   // layer's real buffers (contents irrelevant) with CUDA events; the fastest plan is kept.  Small layers
   // are launch/wave-quantisation bound and large-K ones L2-bandwidth bound, so no single rule fits.
   TcConvPlan* autotune_tc(const ConvProblem& p, const __half* w) {
@@ -679,14 +658,14 @@ struct NetBuilder {
     }
     const int bns[4] = {256, 128, 64, 32};
     const int sts[3] = {0, 3, 2};
-    const int grids[3] = {148, 296, 1 << 30};
+    const int grids[3] = {device_sms(), 2 * device_sms(), 1 << 30};
     TcConvPlan* best = nullptr;
     float best_ms = 1e30f;
     std::set<std::string> seen;
     cudaEvent_t e0, e1;
     YB_CHECK_CUDA(cudaEventCreate(&e0));
     YB_CHECK_CUDA(cudaEventCreate(&e1));
-    // extra candidates: CTA pairs (cta_group::2, persistent grid only) and two epilogue groups per CTA
+    // extra candidates: CTA pairs (clusters of two, persistent grid only) and two MMA warpgroups per CTA
     const int npair = h->pair_candidates ? 2 : 1;
     const int nepi = h->epi2_candidates ? 2 : 1;
     // YB_PDL=1 (experimental): every single-CTA candidate is timed with programmatic dependent launch on a private
@@ -709,8 +688,8 @@ struct NetBuilder {
         for (int gi = 0; gi < (pi ? 1 : 3); ++gi) {
           if (bns[bi] > 64 && bns[bi] >= 2 * p.Cout) continue;
           if (pi && bns[bi] < 64) continue;
-          if (ei && (bns[bi] < 64 || gi == 1)) continue;   // 320-thread CTAs: one per SM
-          if (di && (pi || ei || gi == 1)) continue;        // PDL-friendly: single CTAs, one epilogue group, <= 1 CTA/SM of its own
+          if (ei && (bns[bi] < 64 || gi == 1)) continue;   // 384-thread CTAs: one per SM
+          if (di && (pi || ei || gi == 1)) continue;        // PDL-friendly: single CTAs, one MMA warpgroup, <= 1 CTA/SM of its own
           if (ki && (gi != 0 || di || h->pdl)) continue;    // stream-K: one CTA (cluster) per SM (TPC), no PDL
           TcConvPlan* cand = nullptr;
           try {
@@ -885,7 +864,7 @@ void build_network(yb_handle* h, Executor* ex, bool dry) {
     const std::string hn = "prediction_layers.0";
     Act u = nb.conv(hn + ".upfeature.0", "", Pl[l], 3, 1, 1, ACT_RELU);
     if (nb.f16 && h->fuse_heads) {
-      // bbox + conf + mask convs share their input: one tcgen05 launch with Cout = A*(4+C+k), the epilogue
+      // bbox + conf + mask convs share their input: one tensor-core launch with Cout = A*(4+C+k), the epilogue
       // routes channel ranges to the three concatenated fp32 tensors (tanh on the mask coefficients)
       nb.fused_head(hn, u, ex->loc ? ex->loc + level_off[l] * 4 : nullptr, ex->conf ? ex->conf + level_off[l] * NC : nullptr,
                     ex->coef ? ex->coef + level_off[l] * MD : nullptr, ex->P, A, NC, MD);
@@ -994,8 +973,8 @@ ConvW& yb_handle::get_conv(const std::string& conv_key, const std::string& bn_ke
   const HostTensor& w = need(this, conv_key + ".weight");
   YB_REQUIRE(w.shape.size() == 4, ("weight " + conv_key + " is not 4-D").c_str());
   const int Co = (int)w.shape[0], Ci = (int)w.shape[1], KH = (int)w.shape[2], KW = (int)w.shape[3];
-  const int CiP = (want_tc && pack == 0 && cin_pad > Ci) ? cin_pad : Ci;   // row length of the tcgen05 packing
-  const int CoP = (want_tc && pack == 0 && cout_pad > Co) ? cout_pad : Co;  // rows of the tcgen05 packing (zeros beyond Co)
+  const int CiP = (want_tc && pack == 0 && cin_pad > Ci) ? cin_pad : Ci;   // row length of the tensor-core packing
+  const int CoP = (want_tc && pack == 0 && cout_pad > Co) ? cout_pad : Co;  // rows of the tensor-core packing (zeros beyond Co)
   if (cw.Cout == 0) {
     cw.cout_pad = CoP;
     cw.cin_pad = CiP;

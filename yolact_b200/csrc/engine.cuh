@@ -27,12 +27,12 @@ struct HostTensor {
 struct ConvW {
   int Cin = 0, Cout = 0, KH = 0, KW = 0;
   int cout_pad = 0;          // w_tc / bias carry this many output channels (zero rows beyond Cout): a 32-channel layer
-                             // then writes 64-channel pixels the next tcgen05 conv can consume; 0 = Cout
+                             // then writes 64-channel pixels the next tensor-core conv can consume; 0 = Cout
   int cin_pad = 0;           // w_tc rows are padded with zeros to this many input channels (a multiple of 64) when the
                              // producer writes zero-padded pixels (Darknet: 32 -> 64); 0 = Cin
   float* w_f32 = nullptr;    // [KH*KW*Cin][Cout]           (SIMT fp32)
   __half* w_f16 = nullptr;   // [KH*KW*Cin][Cout]           (SIMT fp16)
-  __half* w_tc = nullptr;    // [KH*KW][Cout][Cin]          (tcgen05), or [1][Cout][9*Cin] for DCN
+  __half* w_tc = nullptr;    // [KH*KW][Cout][Cin]          (tensor cores), or [1][Cout][9*Cin] for DCN
   float* bias = nullptr;     // [Cout] or null
   int pack = 0;              // 0 normal, 1 DCN ([Cout][9*Cin]), 2 stem ([Cout][Kpad], OIHW order)
   // YB_PREC_F16X3: w_tc holds [..][hi(K) | lo(K)] fp16 pairs of w * 2^e (e chosen so that max |w| * 2^e < 2^15:
@@ -113,20 +113,20 @@ struct yb_handle {
   bool use_graphs = true;
   bool profiling = false;
   bool fuse_heads = true;   // YB_FUSE_HEADS=0: three separate head convs per level
-  bool pdl = false;         // programmatic dependent launch between consecutive tcgen05 convs: on in the fp16 mode (YB_PDL=0/1)
+  bool pdl = false;         // programmatic dependent launch between consecutive tensor-core convs: on in the fp16 mode (YB_PDL=0/1)
   bool stem_on_tc = true;   // YB_STEM_TC=0 falls back to the SIMT stem
-  bool dcn_fused = true;    // YB_DCN_FUSED=0: separate gather kernel + fp16 column buffer + 1x1 tcgen05 contraction (round 1)
-  int stem_wg = 0;          // YB_STEM_WG=1|2: worker threads per output pixel in the 7x7 stem; 0 = 1 (f16: 2 measured slower, 0.176 vs 0.154 ms), 2 in the split mode
-  bool autotune = true;     // YB_AUTOTUNE=0 disables plan-time autotuning of the tcgen05 tiles
-  bool pair_candidates = true;    // YB_PAIR=0: the autotuner skips CTA-pair (cta_group::2) plans
-  bool epi2_candidates = true;    // YB_EPI2=0: the autotuner skips plans with two epilogue groups (320 threads)
+  bool dcn_fused = true;    // YB_DCN_FUSED=0: separate gather kernel + fp16 column buffer + 1x1 tensor-core contraction
+  int stem_wg = 0;          // YB_STEM_WG=1|2: worker threads per output pixel in the 7x7 stem; 0 = 1 in the fp16 mode, 2 in the split mode
+  bool autotune = true;     // YB_AUTOTUNE=0 disables plan-time autotuning of the tensor-core tiles
+  bool pair_candidates = true;    // YB_PAIR=0: the autotuner skips CTA-pair (cluster of two) plans
+  bool epi2_candidates = true;    // YB_EPI2=0: the autotuner skips plans with two MMA warpgroups (384 threads)
   float last_total_ms = 0.f, last_conv_ms = 0.f;
   yb::LaunchCounter lc;
   std::map<std::string, yb::HostTensor> host;
   std::map<std::string, yb::ConvW> convs;
   std::map<std::string, std::unique_ptr<yb::Executor>> execs;
   std::vector<void*> weight_allocs;
-  std::map<std::string, std::array<int, 7>> tune_cache;  // layer shape -> (BN, stages, grid, pair, epilogue groups, pdl-friendly, stream-K) from the autotuner
+  std::map<std::string, std::array<int, 7>> tune_cache;  // layer shape -> (BN, stages, grid, pair, MMA warpgroups, pdl-friendly, stream-K) from the autotuner
   bool sk_candidates = true;      // the autotuner times stream-K plans: on in the split mode (YB_SK=0/1)
   int chain_mode = 1;             // runs of consecutive convs as one chain launch: 0 never, 1 when timed faster, 2 always (YB_CHAIN)
   cudaStream_t tune_stream = nullptr;   // private stream of the autotuner when PDL candidates are timed

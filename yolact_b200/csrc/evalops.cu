@@ -309,7 +309,7 @@ display_blend_kernel(const float* __restrict__ img, int img_is_255, const void* 
 
 inline int grid_for(int64_t total, int block) {
   int64_t g = (total + block - 1) / block;
-  const int64_t cap = 148 * 16;
+  const int64_t cap = 132 * 16;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 

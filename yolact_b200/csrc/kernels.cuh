@@ -7,7 +7,7 @@
 namespace yb {
 
 // -------------------------------------------------------------------------------------------
-// Convolution problem description shared by the SIMT and the tcgen05 kernels.
+// Convolution problem description shared by the SIMT and the tensor-core (wgmma) kernels.
 // Activations are NHWC.  Output addressing is  y[b * y_batch_stride + pix * y_pix_stride + c]
 // (elements), which lets the 5 head levels write straight into the concatenated
 // [B, P, D] tensors the reference builds with permute+view+cat (yolact.py:169-173,633-634).
@@ -26,12 +26,12 @@ struct ConvProblem {
   const float* bias = nullptr;     // [Cout] fp32 (BN folded), nullable
   const void* residual = nullptr;  // dense NHWC [B,Ho,Wo,Cout], activation dtype, nullable
   int res_after_act = 0;           // 1: y = act(conv) + residual (DarkNetBlock, backbone.py:246-247)
-  // split precision (tcgen05 kernel only, YB_PREC_F16X3): x / residual / half outputs are [hi(C) | lo(C)] fp16 pairs
+  // split precision (tensor-core kernel only, YB_PREC_F16X3): x / residual / half outputs are [hi(C) | lo(C)] fp16 pairs
   // per pixel (y_pix_stride and y_batch_stride count halfs and include both planes), weights are packed
   // [tap][Cout][hi(Cin) | lo(Cin)] and pre-multiplied by 1 / out_scale (a power of two)
   int split = 0;
   float out_scale = 1.f;
-  // fused prediction head (tcgen05 kernel only): output channels [seg_begin, seg_end) of segment i go to the
+  // fused prediction head (tensor-core kernel only): output channels [seg_begin, seg_end) of segment i go to the
   // fp32 tensor seg_y[i] with its own strides and activation; y / y_* are ignored when nseg > 0
   int nseg = 0;
   int seg_begin[3] = {0, 0, 0}, seg_end[3] = {0, 0, 0}, seg_ps[3] = {0, 0, 0}, seg_act[3] = {0, 0, 0};
@@ -49,15 +49,16 @@ enum SimtTypes : int {
 void launch_simt_conv(const ConvProblem& p, const void* w, int types, cudaStream_t stream,
                       LaunchCounter* lc);
 
-// ---- tcgen05 implicit-GEMM convolution (fp16 in, fp32 accumulate) ----------------------------
+// ---- wgmma implicit-GEMM convolution (fp16 in, fp32 accumulate) ------------------------------
 struct TcConvPlan;  // opaque: tensor maps + tiling; built once per (layer, shape, pointers)
+int device_sms();   // SMs of the current device
 // w_packed: device half [KH*KW][Cout][Cin] ([KH*KW][Cout][2*Cin] when p.split). Requires Cin % 64 == 0.
 // bn_override in {32,64,128,256} / stages_override > 0 pin the N tile / pipeline depth (autotuner); 0 = heuristic.
-// grid_override > 0 caps the number of (persistent) CTAs; default 148 = one per SM.
-// pair_override > 0: CTA pairs (cluster of 2, tcgen05 cta_group::2, UMMA M = 256; each CTA stages half the weight tile).
+// grid_override > 0 caps the number of (persistent) CTAs; default device_sms() = one per SM.
+// pair_override > 0: CTA pairs (cluster of 2; each CTA loads half the weight tile and multicasts it to both).
 TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, int bn_override = 0,
                                 int stages_override = 0, int grid_override = 0, int pair_override = 0,
-                                int epi_override = 0,    // epi_override == 2: two 4-warp epilogue groups (320 threads)
+                                int epi_override = 0,    // epi_override == 2: two MMA warpgroups (384 threads)
                                 int pdl_override = 0,    // > 0: plan sized for 2 CTAs/SM + programmatic dependent launch
                                 int sk_override = 0,     // > 0: stream-K (needs tc_conv_plan_set_sk_workspace before launch)
                                 int chain_override = 0); // > 0: a chain-kernel plan (residual read from global memory in every mode)
@@ -78,9 +79,7 @@ void launch_tc_conv(const TcConvPlan* plan, cudaStream_t stream, LaunchCounter* 
 // dependency counters instead of kernel boundaries (tc_conv.cu, "chain kernel"); the plans must outlive the chain
 struct TcChain;
 bool tc_conv_plan_chainable(const TcConvPlan* plan);
-TcChain* tc_chain_create(const std::vector<const TcConvPlan*>& plans, const std::vector<int>& dep_a, const std::vector<int>& dep_r,
-                         int groups = 2);   // epilogue groups per CTA: 2 (three split-precision stages) or 4 (two stages)
-int tc_chain_groups(const TcChain* chain);
+TcChain* tc_chain_create(const std::vector<const TcConvPlan*>& plans, const std::vector<int>& dep_a, const std::vector<int>& dep_r);
 void tc_chain_destroy(TcChain* chain);
 int tc_chain_layers(const TcChain* chain);
 bool tc_chain_graph_ok(const TcChain* chain);
@@ -88,7 +87,7 @@ void tc_chain_print_stats(TcChain* chain, const char* name);
 void tc_chain_debug_deps(int B, int Hin, int Win, int k, int stride, int pad, int producer_flat, int m, int32_t* out);
 void launch_tc_chain(const TcChain* chain, cudaStream_t stream, LaunchCounter* lc);
 
-// ---- stem on tcgen05 (3-channel NCHW fp32 frame -> NHWC fp16) ---------------------------------------
+// ---- stem on the tensor cores (3-channel NCHW fp32 frame -> NHWC fp16) -------------------------------
 struct StemTcPlan;
 bool stem_tc_supported(int ks, int stride, int pad, int cin, int cout);
 int stem_tc_kpad(int ks);   // K = 3*ks*ks rounded up to 64
@@ -98,7 +97,7 @@ StemTcPlan* stem_tc_plan_create(const float* x_nchw, const __half* w_packed, con
                                 int H, int W, int ks, int stride, int pad, int cout, int act, int split = 0,
                                 float out_scale = 1.f, int cpad = 0);   // cpad > cout: zero-padded output pixels
 void stem_tc_plan_destroy(StemTcPlan* plan);
-void stem_tc_plan_set_worker_groups(StemTcPlan* plan, int wg);   // 2: two threads per pixel (7x7 stem)
+void stem_tc_plan_set_worker_groups(StemTcPlan* plan, int wg);   // 2 / 4: two / four threads per pixel (7x7 stem)
 void launch_stem_tc(const StemTcPlan* plan, cudaStream_t stream, LaunchCounter* lc);
 
 // ---- pointwise -------------------------------------------------------------------------------
@@ -194,12 +193,12 @@ void launch_dcn_simt(const T* x, const float* om, const T* w, const float* bias,
                      int W, int C, int Ho, int Wo, int Cout, int stride, int pad, int dil, int act,
                      int mask_logits, cudaStream_t stream, LaunchCounter* lc);
 // Deformable gather only: writes the modulated, bilinearly sampled columns as NHWC half
-// [B,Ho,Wo,9*C] (tap-major) so the tcgen05 1x1 contraction can consume them.
+// [B,Ho,Wo,9*C] (tap-major) so the tensor-core 1x1 contraction can consume them.
 void launch_dcn_gather_f16(const __half* x, const float* om, __half* cols, int B, int H, int W,
                            int C, int Ho, int Wo, int stride, int pad, int dil, int mask_logits,
                            cudaStream_t stream, LaunchCounter* lc, int split = 0);
 
-// ---- fused DCNv2 on tcgen05 (dcn_tc.cu): gather -> smem A stage -> MMA -> bias/act, no column buffer ----------------
+// ---- fused DCNv2 on the tensor cores (dcn_tc.cu): gather -> smem A stage -> MMA -> bias/act, no column buffer ----------------
 struct DcnTcPlan;
 bool dcn_tc_supported(int C, int Cout);
 // x NHWC half [B,H,W,C] (split: [.., hi(C) | lo(C)]), om fp32 [B,Ho,Wo,27], w_packed [Cout][9*C] half with k = tap*C + c

@@ -341,7 +341,7 @@ void launch_mask_assembly(const float* proto, int ph, int pw, int k, const float
     // so the band's prototype rows are reused from L1.  YB_MASK_CTAS_PER_SM overrides the target (tuning hook).
     static const int ctas_per_sm = getenv("YB_MASK_CTAS_PER_SM") ? std::max(1, atoi(getenv("YB_MASK_CTAS_PER_SM"))) : 32;
     int group = n;
-    while (group > 8 && (int64_t)bands * ceil_div(n, group) * batch < (int64_t)ctas_per_sm * 148) group = (group + 1) / 2;
+    while (group > 8 && (int64_t)bands * ceil_div(n, group) * batch < (int64_t)ctas_per_sm * 132) group = (group + 1) / 2;
     dim3 grid(bands, ceil_div(n, group), batch);
     const size_t plane = (size_t)out_h * out_w;
     const long long img_stride = (long long)n * (mask_format == YB_MASK_F32 ? plane * 4

@@ -257,7 +257,7 @@ __global__ void fill_u32_kernel(uint32_t* p, uint32_t v, int64_t n) {
 
 inline int grid_for(int64_t total, int block) {
   int64_t g = (total + block - 1) / block;
-  const int64_t cap = 148 * 16;
+  const int64_t cap = 132 * 16;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 

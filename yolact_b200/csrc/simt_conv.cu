@@ -1,8 +1,8 @@
 // Generic implicit-GEMM convolution on CUDA cores (fp32 FMA, fp32 accumulation).
 //
 // Role in the design (DESIGN.md): (1) the whole network in YB_PREC_F32 parity mode, (2) the layers
-// the tcgen05 kernel does not take in YB_PREC_F16TC mode (7x7 stem with Cin=3, FastMaskIoUNet),
-// (3) on-device second opinion for the tcgen05 kernel in tests.
+// the tensor-core kernel does not take in YB_PREC_F16TC mode (7x7 stem with Cin=3, FastMaskIoUNet),
+// (3) on-device second opinion for the tensor-core kernel in tests.
 //
 // Reference semantics: nn.Conv2d (cross-correlation, zero padding) + folded BatchNorm2d bias
 // (backbone.py:37-57) + optional residual add + activation.

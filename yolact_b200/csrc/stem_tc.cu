@@ -1,20 +1,17 @@
-// Network stem on tcgen05: conv KxK over the 3-channel NCHW fp32 input frame (+ folded BN + activation)
-// -> NHWC fp16.  ResNet: 7x7/2 pad 3, 3->64, ReLU (backbone.py:77-79,129-131).  Darknet: 3x3/1 pad 1,
+// Network stem on the tensor cores (wgmma): conv KxK over the 3-channel NCHW fp32 input frame (+ folded BN +
+// activation) -> NHWC fp16.  ResNet: 7x7/2 pad 3, 3->64, ReLU (backbone.py:77-79,129-131).  Darknet: 3x3/1 pad 1,
 // 3->32, LeakyReLU(0.1) (backbone.py:267, :222-233).
 //
 // Cin = 3 is useless for TMA (6 bytes per pixel) so the A operand is built by the CUDA cores:
 // each of the 128 worker threads owns one output pixel, gathers its KxKx3 patch straight from the
 // fp32 NCHW frame (zero padding by predication, layout conversion and fp32->fp16 cast fused in),
-// (with WG = 2 worker groups, two threads share a pixel: alternate 16-byte k-groups of the patch, and half of
-// the output channels each in the epilogue -- twice the warps in flight for the latency-bound gather)
-// and writes it as one K-major SWIZZLE_128B row of the UMMA A tile in shared memory
-// (k = c*K*K + r*K + s, the OIHW flattening, so the weights need no permutation).  A fifth warp
-// TMA-loads the [Cout][Kpad] weight tile, issues ceil(K/16) tcgen05.mma (M=128, N=Cout) and commits;
-// the workers then read their accumulator row from TMEM and store one full 64/128-byte line each.
+// (with WG = 2 / 4 worker warpgroups, two / four threads share a pixel: alternate 16-byte k-groups of the patch --
+// more warps in flight for the latency-bound gather)
+// and writes it as one K-major SWIZZLE_128B row of the wgmma A tile in shared memory
+// (k = c*K*K + r*K + s, the OIHW flattening, so the weights need no permutation).  Thread 0 TMA-loads the
+// [Cout][Kpad] weight tile meanwhile; then warpgroup w runs ceil(K/16) wgmmas (M = 64, N = Cout) for the 64-row
+// halves w, w + WG of the tile and stores its rows' pixels from the accumulator registers.
 // Several CTAs per SM overlap gather / MMA / epilogue of different tiles.
-// (Measured and removed in round 2: an 8 x 16 tile variant that staged the shared input patch in shared memory first --
-// 0.225 vs 0.16 ms in the fp16 mode, 0.39 vs 0.39 ms in the split mode: the gather is not the bound, the serial
-// gather -> MMA -> store chain of a single-tile CTA is; in the split mode the 144 KB of operand tiles allow one CTA per SM.)
 #include "tc_common.cuh"
 
 namespace yb {
@@ -24,7 +21,7 @@ using namespace tc;
 namespace {
 
 constexpr int ST_M = 128;
-// threads = 128 * WG workers (TMEM lane quadrant == warp % 4) + one MMA warp
+// threads = 128 * WG workers (warpgroups)
 
 struct alignas(64) StemParams {
   CUtensorMap tmW;
@@ -35,22 +32,16 @@ struct alignas(64) StemParams {
   int cpad;               // channels per output pixel (>= COUT, multiple of 8; channels COUT..cpad-1 are written as zeros so
                           // that a tensor-core conv with Cin % 64 == 0 can consume a 32-channel stem, e.g. Darknet's)
   long long M;
-  uint32_t idesc;
   int act;
   float out_scale;   // split: weights are pre-multiplied by 1 / out_scale (a power of two)
 };
 
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
 // SPLIT (YB_PREC_F16X3): the patch is written as a hi and a lo fp16 tile, the weights come as [Cout][hi(Kpad) | lo(Kpad)],
-// three MMA passes (hi*hi + lo*hi + hi*lo) accumulate in one fp32 tile and the output pixel is [hi(COUT) | lo(COUT)].
+// three MMA passes (hi*hi into one accumulator, lo*hi + hi*lo into a second one) and the output pixel is [hi(COUT) | lo(COUT)].
 template <int KS, int STRIDE, int PAD, int COUT, int WG, bool SPLIT>
-__global__ void __launch_bounds__(128 * WG + 32)
+__global__ void __launch_bounds__(128 * WG)
 stem_tc_kernel(const __grid_constant__ StemParams p) {
   constexpr int NPL = SPLIT ? 2 : 1;
-  constexpr int MMA_WARP = 4 * WG;
   constexpr int K = 3 * KS * KS;
   constexpr int ATOMS = (K + 63) / 64;
   constexpr int KSTEPS = (K + 15) / 16;
@@ -58,52 +49,23 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
   constexpr int B_ATOM_BYTES = COUT * 128;
 
   extern __shared__ uint8_t smem_dyn[];
-  __shared__ uint64_t a_full, b_full, tmem_full;
-  __shared__ uint32_t s_tmem;
+  __shared__ uint64_t b_full;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
   uint8_t* sA = smem;                               // [plane][atom]
   uint8_t* sB = smem + NPL * ATOMS * A_ATOM_BYTES;  // [plane][atom]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (tid == 0) {
-    mbar_init(&a_full, 128 * WG);
     mbar_init(&b_full, 1);
-    mbar_init(&tmem_full, 1);
     fence_barrier_init();
-    tma_prefetch_desc(&p.tmW);
+    mbar_expect_tx(&b_full, NPL * ATOMS * B_ATOM_BYTES);
+    for (int pl = 0; pl < NPL; ++pl)
+      for (int a = 0; a < ATOMS; ++a)
+        tma_load_3d(sB + (pl * ATOMS + a) * B_ATOM_BYTES, &p.tmW, &b_full, pl * ATOMS * 64 + a * 64, 0, 0);
   }
-  if (warp == MMA_WARP) tmem_alloc<NPL * COUT>(&s_tmem);   // split: second accumulator for the lo cross terms
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
-
-  if (warp == MMA_WARP) {
-    if (lane == 0) {
-      mbar_expect_tx(&b_full, NPL * ATOMS * B_ATOM_BYTES);
-      for (int pl = 0; pl < NPL; ++pl)
-        for (int a = 0; a < ATOMS; ++a)
-          tma_load_3d(sB + (pl * ATOMS + a) * B_ATOM_BYTES, &p.tmW, &b_full, pl * ATOMS * 64 + a * 64, 0, 0);
-      mbar_wait(&b_full, 0);
-      mbar_wait(&a_full, 0);
-      tc_fence_after();
-#pragma unroll
-      for (int pass = 0; pass < (SPLIT ? 3 : 1); ++pass) {
-        const int pa = (pass == 1) ? 1 : 0, pb = (pass == 2) ? 1 : 0;   // hi*hi, lo*hi, hi*lo
-#pragma unroll
-        for (int j = 0; j < KSTEPS; ++j) {
-          const int atom = j >> 2, kk = j & 3;
-          const uint64_t da = make_sw128_desc(smem_u32(sA + (pa * ATOMS + atom) * A_ATOM_BYTES)) + (uint64_t)(2 * kk);
-          const uint64_t db = make_sw128_desc(smem_u32(sB + (pb * ATOMS + atom) * B_ATOM_BYTES)) + (uint64_t)(2 * kk);
-          // hi*hi -> accumulator 0; lo*hi and hi*lo -> accumulator 1 (COUT columns further), see common.cuh
-          umma_f16(tmem_base + (pass > 0 ? COUT : 0), da, db, p.idesc, (pass == 2 || j > 0) ? 1u : 0u);
-        }
-      }
-      umma_commit(&tmem_full);
-    }
-  } else {
+  {
     const int row = tid & 127;
-    const int wg = tid >> 7;   // worker group: which half of the k-groups / output channels this thread handles
+    const int wg = tid >> 7;   // worker group: which k-groups of the patch this thread gathers
     const long long m = (long long)blockIdx.x * ST_M + row;
     const bool valid = m < p.M;
     int b = 0, ho = 0, wo = 0;
@@ -153,61 +115,68 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
       *reinterpret_cast<uint4*>(sA + atom * A_ATOM_BYTES + aoff) = pk;
       if (SPLIT) *reinterpret_cast<uint4*>(sA + (ATOMS + atom) * A_ATOM_BYTES + aoff) = pkl;
     }
-    fence_proxy_async();   // generic-proxy smem writes -> visible to tcgen05.mma (async proxy)
-    mbar_arrive(&a_full);
-
-    // ---- epilogue: one accumulator row per thread -> bias -> activation -> one contiguous line
-    mbar_wait(&tmem_full, 0);
-    tc_fence_after();
     __half* yrow = p.y + m * (long long)(p.cpad * NPL);
-    if (valid && (WG == 1 || wg == 0))
+    if (valid && wg == 0)
       for (int c0 = COUT; c0 < p.cpad; c0 += 8) {   // zero padding channels (both planes)
         *reinterpret_cast<uint4*>(yrow + c0) = make_uint4(0u, 0u, 0u, 0u);
         if (SPLIT) *reinterpret_cast<uint4*>(yrow + p.cpad + c0) = make_uint4(0u, 0u, 0u, 0u);
       }
+  }
+  fence_proxy_async();   // generic-proxy smem writes -> visible to wgmma (async proxy)
+  __syncthreads();
+  mbar_wait(&b_full, 0);
+
+  // ---- MMA + epilogue: 64-row half h of the tile -> bias -> activation -> this thread's channel pairs of its two rows
+  const int wgi = warp >> 2, wq = warp & 3;
+  for (int h = wgi; h < 2; h += WG) {
+    float acc[NPL][COUT / 2];
 #pragma unroll
-    for (int c0 = 0; c0 < COUT; c0 += 32) {
-      if (WG > 1 && ((c0 >> 5) % WG) != wg) continue;   // warp-uniform
-      uint32_t r[32];
-      tmem_ld32(tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)c0, r);
-      if (SPLIT) {
-        uint32_t q2[32];
-        tmem_ld32(tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(COUT + c0), q2);
+    for (int pl = 0; pl < NPL; ++pl)
 #pragma unroll
-        for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__fmaf_rn(__uint_as_float(q2[j]), YB_LO_INV, __uint_as_float(r[j])));
-      }
-      if (!valid) continue;
+      for (int i = 0; i < COUT / 2; ++i) acc[pl][i] = 0.f;
+    wgmma_fence();
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        uint4 o, ol;
-        __half2* o2 = reinterpret_cast<__half2*>(&o);
-        __half2* ol2 = reinterpret_cast<__half2*>(&ol);
+    for (int pass = 0; pass < (SPLIT ? 3 : 1); ++pass) {
+      const int pa = (pass == 1) ? 1 : 0, pb = (pass == 2) ? 1 : 0;   // hi*hi, lo*hi, hi*lo
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int col = c0 + q * 8 + 2 * j;
-          float v0 = __uint_as_float(r[q * 8 + 2 * j]), v1 = __uint_as_float(r[q * 8 + 2 * j + 1]);
-          if (SPLIT) {
-            v0 *= p.out_scale;
-            v1 *= p.out_scale;
-          }
-          v0 = apply_act(v0 + (p.bias ? __ldg(p.bias + col) : 0.f), p.act);
-          v1 = apply_act(v1 + (p.bias ? __ldg(p.bias + col + 1) : 0.f), p.act);
-          o2[j] = __halves2half2(from_f32<__half>(v0), from_f32<__half>(v1));
-          if (SPLIT) {
-            const float2 hf = __half22float2(o2[j]);
-            ol2[j] = lo2_from_f32(fabsf(v0) > 65504.f ? 0.f : v0 - hf.x, fabsf(v1) > 65504.f ? 0.f : v1 - hf.y);   // lo' = residual * 2^11
-          }
-        }
-        reinterpret_cast<uint4*>(yrow + c0)[q] = o;
-        if (SPLIT) reinterpret_cast<uint4*>(yrow + p.cpad + c0)[q] = ol;
+      for (int j = 0; j < KSTEPS; ++j) {
+        const int atom = j >> 2, kk = j & 3;
+        const uint64_t da = make_sw128_desc(smem_u32(sA + (pa * ATOMS + atom) * A_ATOM_BYTES + h * 64 * 128)) + (uint64_t)(2 * kk);
+        const uint64_t db = make_sw128_desc(smem_u32(sB + (pb * ATOMS + atom) * B_ATOM_BYTES)) + (uint64_t)(2 * kk);
+        // hi*hi -> accumulator 0; lo*hi and hi*lo -> accumulator 1, see common.cuh
+        Wgmma<COUT>::mma(acc[pass > 0 ? NPL - 1 : 0], da, db, 1u);
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    tmem_dealloc<NPL * COUT>(tmem_base);
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int pl = 0; pl < NPL; ++pl) fence_regs<COUT / 2>(acc[pl]);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int row = h * 64 + wq * 16 + (lane >> 2) + 8 * hh;
+      const long long m = (long long)blockIdx.x * ST_M + row;
+      if (m >= p.M) continue;
+      __half* yrow = p.y + m * (long long)(p.cpad * NPL);
+#pragma unroll
+      for (int j = 0; j < COUT / 8; ++j) {
+        const int col = 8 * j + 2 * (lane & 3);
+        const int i = 4 * j + 2 * hh;
+        float v0 = acc[0][i], v1 = acc[0][i + 1];
+        if (SPLIT) {
+          v0 = __fmaf_rn(acc[NPL - 1][i], YB_LO_INV, v0) * p.out_scale;
+          v1 = __fmaf_rn(acc[NPL - 1][i + 1], YB_LO_INV, v1) * p.out_scale;
+        }
+        v0 = apply_act(v0 + (p.bias ? __ldg(p.bias + col) : 0.f), p.act);
+        v1 = apply_act(v1 + (p.bias ? __ldg(p.bias + col + 1) : 0.f), p.act);
+        const __half2 o = __halves2half2(from_f32<__half>(v0), from_f32<__half>(v1));
+        *reinterpret_cast<__half2*>(yrow + col) = o;
+        if (SPLIT) {
+          const float2 hf = __half22float2(o);
+          *reinterpret_cast<__half2*>(yrow + p.cpad + col) =
+              lo2_from_f32(fabsf(v0) > 65504.f ? 0.f : v0 - hf.x, fabsf(v1) > 65504.f ? 0.f : v1 - hf.y);   // lo' = residual * 2^11
+        }
+      }
+    }
   }
 }
 
@@ -221,7 +190,7 @@ void launch_variant(const StemParams& prm, cudaStream_t stream) {
     YB_CHECK_CUDA(cudaFuncSetAttribute(stem_tc_kernel<KS, STRIDE, PAD, COUT, WG, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)smem));
   const unsigned grid = (unsigned)((prm.M + ST_M - 1) / ST_M);
-  stem_tc_kernel<KS, STRIDE, PAD, COUT, WG, SPLIT><<<grid, 128 * WG + 32, smem, stream>>>(prm);
+  stem_tc_kernel<KS, STRIDE, PAD, COUT, WG, SPLIT><<<grid, 128 * WG, smem, stream>>>(prm);
 }
 
 }  // namespace
@@ -263,7 +232,6 @@ StemTcPlan* stem_tc_plan_create(const float* x_nchw, const __half* w_packed, con
   q.act = act;
   q.out_scale = split ? out_scale : 1.f;
   plan->split = split ? 1 : 0;
-  q.idesc = (1u << 4) | ((uint32_t)(cout >> 3) << 17) | ((uint32_t)(ST_M >> 4) << 24);
   const int kpad = stem_tc_kpad(ks);
   const uint64_t kp = (uint64_t)kpad * (split ? 2 : 1);   // [cout][hi(kpad) | lo(kpad)]
   uint64_t dims[3] = {kp, (uint64_t)cout, 1};

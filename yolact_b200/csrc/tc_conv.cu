@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution on 5th-generation tensor cores (tcgen05 + TMEM + TMA), sm_100a.
+// Implicit-GEMM convolution on Hopper tensor cores (wgmma + TMA + mbarrier), sm_90a.
 //
 // Replaces cuDNN nn.Conv2d + BatchNorm2d + ReLU (+ residual add) of the reference's backbone /
 // FPN / protonet / prediction head (backbone.py:37-57,126-139; yolact.py:311-361,133-212;
@@ -6,23 +6,22 @@
 //
 // GEMM view (no im2col buffer anywhere):
 //   D[M = output pixels of one spatial tile, N = Cout tile] = sum over taps (r,s) and 64-channel
-//   chunks of  A_tap[M, 64] * W_tap[N, 64]^T,   fp16 operands, fp32 accumulation in TMEM.
+//   chunks of  A_tap[M, 64] * W_tap[N, 64]^T,   fp16 operands, fp32 accumulation in registers.
 // A operand: the activation tensor is NHWC fp16; a 4-D TMA tensor map {C, W, H, B} loads the box
 //   {64 channels, tw, th, 1} whose origin is shifted by the tap offset.  Out-of-bounds rows /
 //   columns (the conv's zero padding) are zero-filled by TMA itself.  tw*th <= 128 rows land in
 //   shared memory as 128-byte rows with the 128B swizzle == the canonical K-major SWIZZLE_128B
-//   UMMA layout, so the MMA consumes them with no repacking.
+//   wgmma layout, so the MMA consumes them with no repacking.
 //   Stride-2 convs use one tensor map per input phase (py,px) (a strided *view* of the same
 //   buffer: element strides doubled), and the tap table selects (phase map, dx, dy).
 // B operand: weights packed [tap][Cout][Cin] fp16, 3-D map, box {64, BN, 1}.
-// Pipeline: warp 0 = TMA producer, warp 1 = TMEM alloc + single-thread tcgen05.mma issue,
-//   warps 2..5 = epilogue (tcgen05.ld -> +bias -> +residual -> activation -> 16-byte stores).
-//   `stages`-deep mbarrier ring (full/empty), tcgen05.commit releases shared memory slots.
-// CTA pairs (PAIR = true): a cluster of two CTAs on one TPC computes two adjacent M tiles of the same N tile
-//   with ONE tcgen05.mma.cta_group::2 (M = 256).  Each CTA loads its own A tile and only HALF of the weight
-//   tile, so the bytes a CTA pulls from L2 per k-block drop from 16 KB + BN*128 to 16 KB + BN*64 -- the conv
-//   stack at batch 8 is L2->SM bandwidth bound, not tensor bound (DESIGN.md section 5).  The even CTA issues
-//   the MMAs; both CTAs' TMA loads signal ITS full barrier; tcgen05.commit multicasts to both CTAs' barriers.
+// Pipeline: warpgroup 0 = TMA producer (one thread), warpgroups 1..H = wgmma on their 64-row halves of the tile,
+//   then the epilogue from the accumulator registers (+bias -> +residual -> activation -> staged TMA stores).
+//   `stages`-deep mbarrier ring (full/empty); each MMA warpgroup frees a slot once its wgmmas have read it.
+// CTA pairs (PAIR = true): a cluster of two CTAs computes two adjacent M tiles of the same N tile; each CTA loads
+//   its own A tile and HALF of the weight tile, multicast into both CTAs, so the bytes a CTA pulls from L2 per
+//   k-block drop from 16 KB + BN*128 to 16 KB + BN*64.  A slot is refilled once the MMA warpgroups of BOTH CTAs
+//   have released it.
 // Chain kernel (tc_chain_kernel, further down): a run of consecutive layers -- the whole ResNet trunk after the
 //   max-pool -- in ONE persistent cooperative launch; the layers' parameter blocks live in global memory, the work
 //   units of all layers are dealt round-robin to the CTAs, dependencies are tracked per M tile with counters.
@@ -38,9 +37,7 @@ namespace {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;              // fp16 elements = 128 bytes = one swizzle row
-constexpr int UMMA_K = 16;
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
-constexpr int NUM_THREADS = 192;         // 2 + 4*H warps: producer, MMA issuer, H epilogue groups (H = 1 here)
 constexpr int MAX_TAPS = 9;
 constexpr int MAX_STAGES = 8;
 
@@ -49,26 +46,22 @@ struct alignas(64) TcParams {
   CUtensorMap tmB;
   CUtensorMap tmY;      // output tile store  (epi_tma)
   CUtensorMap tmR;      // residual tile load (epi_tma && residual)
-  CUtensorMap tmY32;    // output tile store in 32-channel boxes, 64-byte swizzle (chain kernel: 8 KB staging tiles)
   int epi_tma;          // 1: fp16 NHWC output goes smem -> TMA store, residual comes in by TMA
   int out_off;          // byte offset of the 2 x 16 KB epilogue staging tiles inside dynamic smem
   int res_off;          // byte offset of the residual staging buffers inside dynamic smem
   int m_tiles, n_tiles; // tile = m_tile * n_tiles + n_tile
-  int acc_stages;       // TMEM accumulator buffers (2 when a CTA processes several tiles)
   int nseg;             // > 0: output channels are split over several fp32 tensors (fused prediction head)
   int seg_begin[3], seg_end[3], seg_ps[3], seg_act[3];
   long long seg_bs[3];
   float* seg_y[3];
-  int tmem_cols;        // power of two >= acc_stages * BN
   int pdl;              // launched with programmatic stream serialization
-  int pair;             // 1: CTA pairs (cluster of 2, tcgen05 cta_group::2, UMMA M = 256)
+  int pair;             // 1: CTA pairs (cluster of 2 sharing the weight tile by multicast)
   int nb;               // batch extent of the tile grid (1 when flattened): tiles with b >= nb are padding
   int ntaps, kchunks, stages;
   int tap_map[MAX_TAPS], tap_dx[MAX_TAPS], tap_dy[MAX_TAPS];
   int tw, th, tiles_x, tiles_y;
   int Ho, Wo, Cout;
   int a_box_bytes;      // tw*th*128
-  uint32_t idesc;
   // epilogue
   void* y;
   const float* bias;
@@ -87,13 +80,13 @@ struct alignas(64) TcParams {
   float out_scale;
   // stream-K (sk != 0): the units' k-block iterations are dealt out in equal contiguous shares, one share per CTA /
   // cluster; a share that ends inside a unit leaves an fp32 partial tile in sk_ws (one slot of 128 x BN floats per
-  // CTA) and raises sk_flags[2 * slot + epilogue group]; the CTA holding the unit's FIRST k-blocks adds the partials
-  // and runs the epilogue
+  // CTA) and raises sk_flags[2 * slot]; the CTA holding the unit's FIRST k-blocks adds the partials and runs the
+  // epilogue
   int sk;
   float* sk_ws;
   int* sk_flags;
-  // split plans with two epilogue groups on a flattened (1x1, stride 1) layout read the residual straight from global
-  // memory: its staging tiles (2 x 32 KB) would leave a single pipeline stage beside the two output staging buffers
+  // split plans with two MMA warpgroups on a flattened (1x1, stride 1) layout read the residual straight from global
+  // memory instead of through staging tiles (one more pipeline stage)
   int res_direct;
   int bn;               // N tile (the kernel template's BN; the chain kernel reads it per layer)
 };
@@ -102,24 +95,16 @@ struct alignas(64) TcParams {
 // kernel
 // ---------------------------------------------------------------------------------------------
 // Persistent: CTA c processes tiles c, c + gridDim.x, ...  (tile = m_tile * n_tiles + n_tile).
-// Three concurrent pipelines: smem ring (TMA producer <-> MMA), TMEM accumulator ring of
-// `acc_stages` buffers (MMA <-> epilogue), and the epilogue's own double-buffered staging tiles,
-// so the loads of tile i+1, the MMAs of tile i and the stores of tile i-1 overlap.
-__device__ __forceinline__ void tmem_alloc_dyn(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_dyn(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
+// Warpgroup 0 is the TMA producer (one thread issues), warpgroups 1..H are the MMA warpgroups: each owns 2/H of the
+// tile's two 64-row halves, accumulates them with wgmma in registers and runs the epilogue of its rows.  The producer
+// runs up to `stages` k-blocks ahead across tile boundaries, so the loads of tile i+1 overlap the epilogue of tile i.
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-
+__device__ __forceinline__ void mma_bar_sync(int nthreads) { asm volatile("bar.sync 1, %0;" ::"r"(nthreads) : "memory"); }
 
 // activation with a compile-time selector (the generic apply_act() is a runtime switch: far too
-// expensive inside the 64-element epilogue loops)
+// expensive inside the epilogue loops)
 template <int ACT>
 __device__ __forceinline__ float act_t(float v) {
   if (ACT == ACT_RELU) return fmaxf(v, 0.f);
@@ -133,153 +118,212 @@ __device__ __forceinline__ __half2 pack_sat(float a, float b) {
   b = fminf(fmaxf(b, -65504.f), 65504.f);
   return __floats2half2_rn(a, b);
 }
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-        "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-        "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// One 64-channel chunk of one accumulator row: (* out_scale) +bias (smem, broadcast), +residual (swizzled smem
-// tile), activation, fp16 pack, swizzled 16-byte stores into the output staging tile.  SPLIT: the residual is
-// hi + lo from two tiles and the result is written as hi / lo = rn(v - hi) into two staging tiles.
-// res_g (res_direct plans): this row's 64 residual channels in GLOBAL memory (hi plane; the lo plane res_lo_off halfs
-// further) instead of a staged tile.
-template <int ACT, bool RES_AFTER, bool SPLIT>
-__device__ __forceinline__ void epi_chunk(const uint32_t* r0, const uint32_t* r1, const float* sbias,
-                                          const uint8_t* res_tile, uint8_t* out_tile, uint32_t row, uint32_t sw,
-                                          float out_scale, const __half* res_g = nullptr, int res_lo_off = 0) {
+// The k-blocks [k0, k1) of one tile: acc[mh][plane] of 64-row half (cw + mh * H) of the tile.  SPLIT: A_hi*W_hi into
+// plane 0, A_lo*W_hi + A_hi*W_lo into plane 1 (combined as acc0 + 2^-11 * acc1 by the caller; the lo*lo term is below
+// fp32 resolution).  Each stage is handed back to the producer(s) once the wgmmas that read it have completed.
+template <int BN, int MH, int H, bool SPLIT, bool PAIR, int NACC>
+__device__ __forceinline__ void mma_tile(float (&acc)[MH][SPLIT ? 2 : 1][NACC], uint8_t* smem, uint64_t* full_bar,
+                                         uint64_t* empty_bar, int stages, int stage_bytes, int a_bytes, int b_plane_bytes,
+                                         uint32_t& kbg, int nkb, int cw, bool signaller) {
+  constexpr int NPL = SPLIT ? 2 : 1;
 #pragma unroll
-  for (int j8 = 0; j8 < 8; ++j8) {
-    const float4 b0 = *reinterpret_cast<const float4*>(sbias + j8 * 8);
-    const float4 b1 = *reinterpret_cast<const float4*>(sbias + j8 * 8 + 4);
-    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-    float v[8];
+  for (int mh = 0; mh < MH; ++mh)
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int col = j8 * 8 + j;
-      const float a = __uint_as_float(col < 32 ? r0[col] : r1[col - 32]);
-      v[j] = SPLIT ? __fmaf_rn(a, out_scale, bb[j]) : a + bb[j];
-      if (RES_AFTER) v[j] = act_t<ACT>(v[j]);
+    for (int pl = 0; pl < NPL; ++pl)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[mh][pl][i] = 0.f;
+  auto release = [&](uint32_t s) {
+    if (!signaller) return;
+    if (PAIR) {   // the stage's weight half of EACH CTA is refilled by both producers: free it in both
+      mbar_arrive_cluster(mapa_u32(smem_u32(&empty_bar[s]), 0));
+      mbar_arrive_cluster(mapa_u32(smem_u32(&empty_bar[s]), 1));
+    } else {
+      mbar_arrive(&empty_bar[s]);
     }
-    const uint32_t off = row * 128u + (((uint32_t)j8 ^ sw) << 4);
-    if (res_tile || res_g) {
-      const uint4 raw = res_tile ? *reinterpret_cast<const uint4*>(res_tile + off)
-                                 : __ldcg(reinterpret_cast<const uint4*>(res_g + j8 * 8));   // L2: inside a chain other SMs wrote it during this launch
-      const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
+  };
+  for (int kb = 0; kb < nkb; ++kb, ++kbg) {
+    const uint32_t s = kbg % (uint32_t)stages;
+    mbar_wait(&full_bar[s], (kbg / (uint32_t)stages) & 1u);
+    const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
+    const uint32_t sb = sa + (uint32_t)a_bytes;
+    wgmma_fence();
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 f = __half22float2(h2[j]);
-        v[2 * j] += f.x;
-        v[2 * j + 1] += f.y;
-      }
+    for (int mh = 0; mh < MH; ++mh) {
+      const uint32_t half_off = (uint32_t)(cw + mh * H) * (64u * 128u);
+      const uint64_t da = make_sw128_desc(sa + half_off);
+      const uint64_t db = make_sw128_desc(sb);
+#pragma unroll
+      for (int k = 0; k < BLOCK_K / 16; ++k) Wgmma<BN>::mma(acc[mh][0], da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1u);
       if (SPLIT) {
-        const uint4 rawl = res_tile ? *reinterpret_cast<const uint4*>(res_tile + A_STAGE_BYTES + off)
-                                    : __ldcg(reinterpret_cast<const uint4*>(res_g + res_lo_off + j8 * 8));
-        const __half2* l2 = reinterpret_cast<const __half2*>(&rawl);
+        const uint64_t dal = make_sw128_desc(sa + (uint32_t)A_STAGE_BYTES + half_off);
+        const uint64_t dbl = make_sw128_desc(sb + (uint32_t)b_plane_bytes);
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float2 f = lo2_to_f32(l2[j]);   // lo plane: 2^11-scaled
-          v[2 * j] += f.x;
-          v[2 * j + 1] += f.y;
-        }
+        for (int k = 0; k < BLOCK_K / 16; ++k)
+          Wgmma<BN>::mma(acc[mh][NPL - 1], dal + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1u);
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / 16; ++k)
+          Wgmma<BN>::mma(acc[mh][NPL - 1], da + (uint64_t)(2 * k), dbl + (uint64_t)(2 * k), 1u);
       }
     }
-    if (!RES_AFTER) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = act_t<ACT>(v[j]);
+    wgmma_commit();
+    if (stages == 1) {   // a single stage: the next k-block can only land once these wgmmas have read this one
+      wgmma_wait<0>();
+      release(s);
+    } else if (kb > 0) {   // the previous k-block's wgmmas are done: its stage can be refilled
+      wgmma_wait<1>();
+      release((kbg - 1) % (uint32_t)stages);
     }
-    uint4 o;
-    __half2* o2 = reinterpret_cast<__half2*>(&o);
+  }
+  wgmma_wait<0>();
+  if (nkb > 0 && stages > 1) release((kbg - 1) % (uint32_t)stages);
 #pragma unroll
-    for (int j = 0; j < 4; ++j) o2[j] = pack_sat(v[2 * j], v[2 * j + 1]);
-    *reinterpret_cast<uint4*>(out_tile + off) = o;
-    if (SPLIT) {
-      uint4 ol;
-      __half2* l2 = reinterpret_cast<__half2*>(&ol);
+  for (int mh = 0; mh < MH; ++mh)
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 hf = __half22float2(o2[j]);
-        // hi saturates at +-65504 (pack_sat); the residual is taken against the clamped value, so a saturated
-        // element gets lo = 0 and hi + lo stays finite
-        const float c0 = fminf(fmaxf(v[2 * j], -65504.f), 65504.f), c1 = fminf(fmaxf(v[2 * j + 1], -65504.f), 65504.f);
-        l2[j] = lo2_from_f32(c0 - hf.x, c1 - hf.y);   // lo plane: residual * 2^11 (see common.cuh)
-      }
-      *reinterpret_cast<uint4*>(out_tile + A_STAGE_BYTES + off) = ol;
-    }
+    for (int pl = 0; pl < NPL; ++pl) fence_regs<BN / 2>(acc[mh][pl]);
+  if (SPLIT) {
+#pragma unroll
+    for (int mh = 0; mh < MH; ++mh)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[mh][0][i] = __fmaf_rn(acc[mh][NPL - 1][i], YB_LO_INV, acc[mh][0][i]);
   }
 }
 
-// Chain-kernel variant: a 32-channel chunk of one accumulator row (r: the combined fp32 accumulator) into an 8 KB staging
-// tile of 128 rows x 64 bytes with the 64-byte TMA swizzle (16-byte unit index ^= (row >> 1) & 3); the lo plane's tile
-// follows the hi plane's.  The residual always comes from global memory (res_g: this row's 32 channels, hi plane).
-// (Requesting the residual of all of a group's chunks up front, into registers, was measured SLOWER -- 4.01 vs 3.69 ms
-// for the 105-layer trunk chain, profiles/r2_call17_summary.txt: 168 registers, and the burst of loads delays the TMA.)
-constexpr int CHUNK32_BYTES = BLOCK_M * 32 * 2;   // 8 KB
-template <int ACT, bool RES_AFTER, bool SPLIT>
-__device__ __forceinline__ void epi_chunk32(const uint32_t* r, const float* sbias, uint8_t* out_tile, uint32_t row,
-                                            float out_scale, const __half* res_g, int res_lo_off) {
-  const uint32_t sw = (row >> 1) & 3u;
+// Staged epilogue of the 64-channel chunks [0, nchunks) of a tile: (* out_scale) + bias, + residual (a swizzled smem
+// tile loaded by TMA, or -- res_g, flattened layouts -- straight from global memory), activation, fp16 pack into the
+// swizzled 128-row staging tile, one TMA store per chunk (and plane) by thread 0 of the MMA warpgroups (OOB rows are
+// clipped by the tensor map).  SPLIT: the result is written as hi / lo = rn(v - hi) into two staging tiles.
+// g: chunks staged by this CTA so far (buffer = g % NBUF).  has_res_tile: res_tmap holds the residual; the load of the
+// tile's chunk 0 was issued before its main loop, chunk c + 1 is requested here.
+struct EpiArgs {
+  const CUtensorMap* tmY;
+  const CUtensorMap* tmR;
+  uint64_t* res_full_bar;
+  uint8_t* out_base;
+  uint8_t* res_base;
+  const float* bias;
+  const __half* res_g;   // res_direct: residual of pixel (x0 + row), channel n0, hi plane (lo plane Cout halfs further)
+  int res_pix_stride;    // halfs per residual pixel (both planes)
+  uint32_t res_tx;       // bytes of one residual chunk (all planes): the box holds tw*th rows, not always 128
+  int Wo, Cout, n0, x0, y0, b, nchunks, nbuf;
+  float out_scale;
+};
+template <int ACT, bool RES_AFTER, bool SPLIT, int BN, int MH, int H, int NACC>
+__device__ __forceinline__ void epi_staged(float (&acc)[MH][SPLIT ? 2 : 1][NACC], const EpiArgs& e, bool has_res_tile,
+                                           uint32_t& g, int cw, int ct, int lane, int wq) {
+  constexpr int NPL = SPLIT ? 2 : 1;
+  const int nthreads = 128 * H;
 #pragma unroll
-  for (int j8 = 0; j8 < 4; ++j8) {
-    const float4 b0 = *reinterpret_cast<const float4*>(sbias + j8 * 8);
-    const float4 b1 = *reinterpret_cast<const float4*>(sbias + j8 * 8 + 4);
-    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-    float v[8];
+  for (int c = 0; c < BN / 64; ++c) {
+    if (c >= e.nchunks) break;
+    const uint32_t buf = (e.nbuf == 1) ? 0u : (g & 1u);
+    uint8_t* out_tile = e.out_base + buf * (NPL * A_STAGE_BYTES);
+    const uint8_t* res_tile = e.res_base + buf * (NPL * A_STAGE_BYTES);
+    if (g >= (uint32_t)e.nbuf) {
+      if (ct == 0) {
+        if (e.nbuf == 1) bulk_wait_read<0>(); else bulk_wait_read<1>();   // the store that last used this tile has read it
+      }
+      mma_bar_sync(nthreads);
+    }
+    if (has_res_tile) {
+      if (ct == 0 && e.nbuf == 2 && c + 1 < e.nchunks) {   // next chunk's residual into the other buffer
+        const uint32_t nb = (g + 1) & 1u;
+        mbar_expect_tx(&e.res_full_bar[nb], e.res_tx);
+#pragma unroll
+        for (int pl = 0; pl < NPL; ++pl)
+          tma_load_4d(e.res_base + nb * (NPL * A_STAGE_BYTES) + pl * A_STAGE_BYTES, e.tmR, &e.res_full_bar[nb],
+                      e.n0 + (c + 1) * 64 + pl * e.Cout, e.x0, e.y0, e.b);
+      }
+      mbar_wait(&e.res_full_bar[buf], (e.nbuf == 1) ? (g & 1u) : ((g >> 1) & 1u));
+    }
+    const int nbase = e.n0 + c * 64;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const float a = __uint_as_float(r[j8 * 8 + j]);
-      v[j] = SPLIT ? __fmaf_rn(a, out_scale, bb[j]) : a + bb[j];
-      if (RES_AFTER) v[j] = act_t<ACT>(v[j]);
-    }
-    if (res_g) {
-      const uint4 raw = __ldcg(reinterpret_cast<const uint4*>(res_g + j8 * 8));   // L2: other SMs wrote it during this launch
-      const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
+      const int col = 8 * j + 2 * (lane & 3);
+      const float b0 = (e.bias && nbase + col < e.Cout) ? __ldg(e.bias + nbase + col) : 0.f;
+      const float b1 = (e.bias && nbase + col + 1 < e.Cout) ? __ldg(e.bias + nbase + col + 1) : 0.f;
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 f = __half22float2(h2[j]);
-        v[2 * j] += f.x;
-        v[2 * j + 1] += f.y;
-      }
-      if (SPLIT) {
-        const uint4 rawl = __ldcg(reinterpret_cast<const uint4*>(res_g + res_lo_off + j8 * 8));
-        const __half2* l2 = reinterpret_cast<const __half2*>(&rawl);
+      for (int mh = 0; mh < MH; ++mh)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float2 f = lo2_to_f32(l2[j]);
-          v[2 * j] += f.x;
-          v[2 * j + 1] += f.y;
+        for (int h = 0; h < 2; ++h) {
+          const int row = (cw + mh * H) * 64 + wq * 16 + (lane >> 2) + 8 * h;
+          const int i = (c * 8 + j) * 4 + 2 * h;
+          float v0 = SPLIT ? __fmaf_rn(acc[mh][0][i], e.out_scale, b0) : acc[mh][0][i] + b0;
+          float v1 = SPLIT ? __fmaf_rn(acc[mh][0][i + 1], e.out_scale, b1) : acc[mh][0][i + 1] + b1;
+          if (RES_AFTER) {
+            v0 = act_t<ACT>(v0);
+            v1 = act_t<ACT>(v1);
+          }
+          const uint32_t off = (uint32_t)row * 128u + ((((uint32_t)j) ^ ((uint32_t)row & 7u)) << 4) + (uint32_t)(lane & 3) * 4u;
+          if (has_res_tile || e.res_g) {
+            __half2 rh, rl;
+            if (has_res_tile) {
+              rh = *reinterpret_cast<const __half2*>(res_tile + off);
+              if (SPLIT) rl = *reinterpret_cast<const __half2*>(res_tile + A_STAGE_BYTES + off);
+            } else if (e.x0 + row < e.Wo) {   // L2: inside a chain other SMs wrote it during this launch
+              const __half* rp = e.res_g + (size_t)row * e.res_pix_stride + c * 64 + col;
+              const unsigned int u = __ldcg(reinterpret_cast<const unsigned int*>(rp));
+              rh = *reinterpret_cast<const __half2*>(&u);
+              if (SPLIT) {
+                const unsigned int ul = __ldcg(reinterpret_cast<const unsigned int*>(rp + e.Cout));
+                rl = *reinterpret_cast<const __half2*>(&ul);
+              }
+            } else {
+              rh = rl = __floats2half2_rn(0.f, 0.f);
+            }
+            const float2 f = __half22float2(rh);
+            v0 += f.x;
+            v1 += f.y;
+            if (SPLIT) {
+              const float2 fl = lo2_to_f32(rl);   // lo plane: 2^11-scaled
+              v0 += fl.x;
+              v1 += fl.y;
+            }
+          }
+          if (!RES_AFTER) {
+            v0 = act_t<ACT>(v0);
+            v1 = act_t<ACT>(v1);
+          }
+          const __half2 o = pack_sat(v0, v1);
+          *reinterpret_cast<__half2*>(out_tile + off) = o;
+          if (SPLIT) {
+            // hi saturates at +-65504 (pack_sat); the residual is taken against the clamped value, so a saturated
+            // element gets lo = 0 and hi + lo stays finite
+            const float2 hf = __half22float2(o);
+            const float c0 = fminf(fmaxf(v0, -65504.f), 65504.f), c1 = fminf(fmaxf(v1, -65504.f), 65504.f);
+            *reinterpret_cast<__half2*>(out_tile + A_STAGE_BYTES + off) = lo2_from_f32(c0 - hf.x, c1 - hf.y);
+          }
         }
+    }
+    fence_proxy_async();   // generic-proxy smem writes -> visible to the TMA (async proxy)
+    mma_bar_sync(nthreads);
+    if (ct == 0) {
+      tma_store_4d(e.tmY, out_tile, nbase, e.x0, e.y0, e.b);
+      if (SPLIT) tma_store_4d(e.tmY, out_tile + A_STAGE_BYTES, nbase + e.Cout, e.x0, e.y0, e.b);
+      bulk_commit();
+      if (has_res_tile && e.nbuf == 1 && c + 1 < e.nchunks) {   // single buffer: refill it now that it has been read
+        mbar_expect_tx(&e.res_full_bar[0], e.res_tx);
+#pragma unroll
+        for (int pl = 0; pl < NPL; ++pl)
+          tma_load_4d(e.res_base + pl * A_STAGE_BYTES, e.tmR, &e.res_full_bar[0], e.n0 + (c + 1) * 64 + pl * e.Cout, e.x0,
+                      e.y0, e.b);
       }
     }
-    if (!RES_AFTER) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = act_t<ACT>(v[j]);
-    }
-    const uint32_t off = row * 64u + (((uint32_t)j8 ^ sw) << 4);
-    uint4 o;
-    __half2* o2 = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) o2[j] = pack_sat(v[2 * j], v[2 * j + 1]);
-    *reinterpret_cast<uint4*>(out_tile + off) = o;
-    if (SPLIT) {
-      uint4 ol;
-      __half2* l2 = reinterpret_cast<__half2*>(&ol);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 hf = __half22float2(o2[j]);
-        const float c0 = fminf(fmaxf(v[2 * j], -65504.f), 65504.f), c1 = fminf(fmaxf(v[2 * j + 1], -65504.f), 65504.f);
-        l2[j] = lo2_from_f32(c0 - hf.x, c1 - hf.y);
-      }
-      *reinterpret_cast<uint4*>(out_tile + CHUNK32_BYTES + off) = ol;
-    }
+    ++g;
+  }
+}
+
+template <bool SPLIT, int BN, int MH, int H, int NACC>
+__device__ __forceinline__ void epi_staged_act(int act, int raa, float (&acc)[MH][SPLIT ? 2 : 1][NACC], const EpiArgs& e,
+                                               bool has_res_tile, uint32_t& g, int cw, int ct, int lane, int wq) {
+  switch (act) {
+    case ACT_RELU: epi_staged<ACT_RELU, false, SPLIT, BN, MH, H>(acc, e, has_res_tile, g, cw, ct, lane, wq); break;
+    case ACT_LEAKY:
+      if (raa) epi_staged<ACT_LEAKY, true, SPLIT, BN, MH, H>(acc, e, has_res_tile, g, cw, ct, lane, wq);
+      else epi_staged<ACT_LEAKY, false, SPLIT, BN, MH, H>(acc, e, has_res_tile, g, cw, ct, lane, wq);
+      break;
+    case ACT_TANH: epi_staged<ACT_TANH, false, SPLIT, BN, MH, H>(acc, e, has_res_tile, g, cw, ct, lane, wq); break;
+    default: epi_staged<ACT_NONE, false, SPLIT, BN, MH, H>(acc, e, has_res_tile, g, cw, ct, lane, wq); break;
   }
 }
 
@@ -345,63 +389,48 @@ struct WorkIter {
 };
 
 template <int BN, bool PAIR, int H, bool SPLIT>
-__global__ void __launch_bounds__(64 + 128 * H)
+__global__ void __launch_bounds__(128 * (1 + H), 1)
 tc_conv_kernel(const __grid_constant__ TcParams p) {
   // SPLIT (YB_PREC_F16X3): every operand has a hi and a (2^11-scaled) lo fp16 plane; a k-block stages A_hi, A_lo, W_hi,
-  // W_lo and issues A_hi*W_hi into the tile's first accumulator and A_lo*W_hi + A_hi*W_lo into its second one (BN TMEM
-  // columns further); the epilogue combines acc_hi + 2^-11 * acc_lo (the lo*lo term is below fp32 resolution).
+  // W_lo (see mma_tile).
   constexpr int NPL = SPLIT ? 2 : 1;
-  constexpr int B_PLANE_BYTES = (PAIR ? BN / 2 : BN) * BLOCK_K * 2;   // a pair CTA stages half of the weight tile
+  constexpr int MH = 2 / H;
+  constexpr int NACC = BN / 2;
+  static_assert(MH * NPL * NACC <= 128, "accumulator tile exceeds the register budget");
+  constexpr int B_PLANE_BYTES = BN * BLOCK_K * 2;   // a pair CTA loads half of it and receives the peer's half
   constexpr int A_BYTES = NPL * A_STAGE_BYTES;
-  constexpr int B_STAGE_BYTES = NPL * B_PLANE_BYTES;
-  constexpr int STAGE_BYTES = A_BYTES + B_STAGE_BYTES;
+  constexpr int STAGE_BYTES = A_BYTES + NPL * B_PLANE_BYTES;
 
   extern __shared__ uint8_t smem_dyn[];
   __shared__ uint64_t full_bar[MAX_STAGES];
   __shared__ uint64_t empty_bar[MAX_STAGES];
-  __shared__ uint64_t tmem_full_bar[2];
-  __shared__ uint64_t tmem_empty_bar[2];
   __shared__ uint64_t res_full_bar[2];
-  __shared__ uint32_t s_tmem_base;
-  __shared__ __align__(16) float sbias[H * BN];   // one copy per epilogue group
 
   // 1024-byte alignment required by SWIZZLE_128B (host adds 1024 bytes of slack)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-  uint8_t* out_base = smem + p.out_off;   // epilogue staging tiles: [buffer][plane] x 16 KB
-  uint8_t* res_base = smem + p.res_off;   // residual tiles, same layout (only when residual && epi_tma)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int stages = p.stages;
   const int num_kb = p.ntaps * p.kchunks;
-  // work units of this CTA: unit0, unit0 + ustep, ... < num_units
   const int rank = PAIR ? (int)cluster_ctarank() : 0;
   const int unit0 = PAIR ? (int)cluster_id_x() : (int)blockIdx.x;
   const int ustep = PAIR ? (int)cluster_nclusters_x() : (int)gridDim.x;
   const int num_units = (PAIR ? (p.m_tiles + 1) / 2 : p.m_tiles) * p.n_tiles;
-  const int acc_stages = p.acc_stages;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], (PAIR ? 2 : 1) * H);   // one arrival per MMA warpgroup (of both CTAs of a pair)
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], (PAIR ? 2 : 1) * H);   // every epilogue group (of both CTAs of a pair) drains it
-      mbar_init(&res_full_bar[i], 1);
-    }
+    for (int i = 0; i < 2; ++i) mbar_init(&res_full_bar[i], 1);
     fence_barrier_init();
     tma_prefetch_desc(&p.tmB);
     tma_prefetch_desc(&p.tmA[0]);
     if (p.epi_tma) tma_prefetch_desc(&p.tmY);
   }
-  if (warp == 1) tmem_alloc_dyn(&s_tmem_base, (uint32_t)p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
   if (PAIR) cluster_sync_all();   // the peer's barriers are initialised before anything signals them
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem_base;
   // Programmatic dependent launch: everything above overlaps the tail of the previous kernel in the stream, and so do
   // the WEIGHT tiles of this CTA's first k-blocks (constants: they do not depend on the previous layer); the
   // activations are only touched after griddepcontrol.wait.  Dependents are released at once: they can become resident
@@ -409,13 +438,13 @@ tc_conv_kernel(const __grid_constant__ TcParams p) {
   uint32_t pre = 0;   // producer thread only: k-blocks whose weight tile is already in flight
   if (p.pdl) {
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    if (!PAIR && !SPLIT && !p.sk && warp == 0 && lane == 0 && unit0 < num_units) {   // (a stream-K walk starts mid-unit)
+    if (!PAIR && !SPLIT && !p.sk && threadIdx.x == 0 && unit0 < num_units) {   // (a stream-K walk starts mid-unit)
       const TileCoord t0 = decode_unit<PAIR>(p, unit0, rank, BN);
       const int npre = min(stages, num_kb);
       for (int kb = 0; kb < npre; ++kb) {
         const int tap = kb / p.kchunks;
         const int kc = kb - tap * p.kchunks;
-        mbar_expect_tx(&full_bar[kb], (uint32_t)p.a_box_bytes + (uint32_t)B_STAGE_BYTES);
+        mbar_expect_tx(&full_bar[kb], (uint32_t)p.a_box_bytes + (uint32_t)B_PLANE_BYTES);
         tma_load_3d(smem + (size_t)kb * STAGE_BYTES + A_BYTES, &p.tmB, &full_bar[kb], kc * BLOCK_K, t0.n0, tap);
       }
       pre = (uint32_t)npre;
@@ -423,12 +452,10 @@ tc_conv_kernel(const __grid_constant__ TcParams p) {
     asm volatile("griddepcontrol.wait;" ::: "memory");
   }
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      // a pair's leader expects the bytes of BOTH CTAs (each: its A tile + its half of the weight tile, per plane)
-      const uint32_t tx_bytes = ((uint32_t)p.a_box_bytes + (uint32_t)B_PLANE_BYTES) * (uint32_t)NPL * (PAIR ? 2u : 1u);
-      const uint32_t leader_full = PAIR ? mapa_u32(smem_u32(&full_bar[0]), 0) : 0u;
+  if (warp < 4) {
+    // ===================== TMA producer warpgroup (one thread issues) =====================
+    if (threadIdx.x == 0) {
+      const uint32_t tx_bytes = ((uint32_t)p.a_box_bytes + (uint32_t)B_PLANE_BYTES) * (uint32_t)NPL;
       uint32_t kbg = 0;
       WorkIter wi;
       wi.init(p.sk, num_kb, num_units, unit0, ustep);
@@ -446,12 +473,13 @@ tc_conv_kernel(const __grid_constant__ TcParams p) {
           const CUtensorMap* ma = &p.tmA[p.tap_map[tap]];
           const int ax = tc_.x0 + p.tap_dx[tap], ay = tc_.y0 + p.tap_dy[tap];
           if (PAIR) {
-            if (rank == 0) mbar_expect_tx(&full_bar[s], tx_bytes);
-            const uint32_t fb = leader_full + s * (uint32_t)sizeof(uint64_t);
+            // own A tile; own half of the weight tile, multicast into both CTAs (each barrier expects both halves)
+            mbar_expect_tx(&full_bar[s], tx_bytes);
 #pragma unroll
             for (int pl = 0; pl < NPL; ++pl) {
-              tma_load_4d_pair(sa + pl * A_STAGE_BYTES, ma, fb, kc * BLOCK_K + pl * p.cin, ax, ay, tc_.b);
-              tma_load_3d_pair(sb + pl * B_PLANE_BYTES, &p.tmB, fb, kc * BLOCK_K + pl * p.cin, tc_.n0 + rank * (BN / 2), tap);
+              tma_load_4d(sa + pl * A_STAGE_BYTES, ma, &full_bar[s], kc * BLOCK_K + pl * p.cin, ax, ay, tc_.b);
+              tma_load_3d_mc(sb + pl * B_PLANE_BYTES + rank * (B_PLANE_BYTES / 2), &p.tmB, &full_bar[s], (uint16_t)3,
+                             kc * BLOCK_K + pl * p.cin, tc_.n0 + rank * (BN / 2), tap);
             }
           } else if (!SPLIT && kbg < pre) {
             // PDL: this stage was armed and its weight tile requested before the dependency wait
@@ -467,386 +495,193 @@ tc_conv_kernel(const __grid_constant__ TcParams p) {
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (one thread) =====================
-    if (lane == 0 && rank == 0) {   // in a pair only the even CTA issues (for both)
-      uint32_t kbg = 0, t = 0;
-      WorkIter wi;
-      wi.init(p.sk, num_kb, num_units, unit0, ustep);
-      int u, k0, k1;
-      for (; wi.next(u, k0, k1); ++t) {
-        const uint32_t acc = t % (uint32_t)acc_stages;
-        const uint32_t use = t / (uint32_t)acc_stages;
-        mbar_wait(&tmem_empty_bar[acc], (use & 1u) ^ 1u);   // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * (uint32_t)(NPL * BN);
-        for (int kb = k0; kb < k1; ++kb, ++kbg) {
-          const uint32_t s = kbg % (uint32_t)stages;
-          const uint32_t it = kbg / (uint32_t)stages;
-          mbar_wait(&full_bar[s], it & 1u);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + (size_t)s * STAGE_BYTES);
-          const uint32_t sb = sa + A_BYTES;
-          const uint64_t da = make_sw128_desc(sa);
-          const uint64_t db = make_sw128_desc(sb);
-          auto mma = [&](uint64_t a, uint64_t b, uint32_t accum) {
-            if (PAIR) umma_f16_pair(tmem_d, a, b, p.idesc, accum); else umma_f16(tmem_d, a, b, p.idesc, accum);
-          };
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            // advance 16 fp16 = 32 bytes along K inside the 128-byte swizzle row: +2 in the >>4 field
-            mma(da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > k0 || k > 0) ? 1u : 0u);
-          }
-          if (SPLIT) {
-            const uint64_t dal = make_sw128_desc(sa + A_STAGE_BYTES);
-            const uint64_t dbl = make_sw128_desc(sb + B_PLANE_BYTES);
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k)   // A_lo * W_hi -> second accumulator
-              if (PAIR) umma_f16_pair(tmem_d + BN, dal + (uint64_t)(2 * k), db + (uint64_t)(2 * k), p.idesc, (kb > k0 || k > 0) ? 1u : 0u);
-              else umma_f16(tmem_d + BN, dal + (uint64_t)(2 * k), db + (uint64_t)(2 * k), p.idesc, (kb > k0 || k > 0) ? 1u : 0u);
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k)   // A_hi * W_lo -> second accumulator
-              if (PAIR) umma_f16_pair(tmem_d + BN, da + (uint64_t)(2 * k), dbl + (uint64_t)(2 * k), p.idesc, 1u);
-              else umma_f16(tmem_d + BN, da + (uint64_t)(2 * k), dbl + (uint64_t)(2 * k), p.idesc, 1u);
-          }
-          // frees this smem slot (in both CTAs of a pair) once the MMAs above have read it
-          if (PAIR) umma_commit_pair(&empty_bar[s]); else umma_commit(&empty_bar[s]);
-        }
-        // accumulator complete (both halves)
-        if (PAIR) umma_commit_pair(&tmem_full_bar[acc]); else umma_commit(&tmem_full_bar[acc]);
-      }
-    }
   } else {
-    // ===================== epilogue: H groups of 4 warps (TMEM lane quadrant = warp % 4) =====================
-    // H == 1: warps 2..5 process every 64-channel chunk of the tile, double-buffered staging tiles.
-    // H == 2: warps 2..5 take the even chunks and warps 6..9 the odd ones, one staging tile (and one
-    //         residual tile) per group: two chunks are in flight at once, which halves the epilogue a CTA
-    //         with a single tile cannot hide behind its main loop.
-    const int quad = warp & 3;
-    const int hgrp = (H == 2) ? ((warp - 2) >> 2) : 0;       // epilogue group of this warp
-    const int row = quad * 32 + lane;  // accumulator row == tile-local output pixel
-    const bool issuer = (warp == 2 + 4 * hgrp && lane == 0);
-    const bool has_res = (p.residual != nullptr) && !p.res_direct;   // residual staged by TMA (res_direct: read from global)
-    const uint32_t sw = (uint32_t)(row & 7);
-    float* my_bias = sbias + hgrp * BN;
-    constexpr int NBUF = (H == 2 || SPLIT) ? 1 : 2;           // staging / residual buffers per group (a buffer = NPL tiles)
-    constexpr int BUF_BYTES = NPL * A_STAGE_BYTES;
-    auto group_sync = [&]() {                                 // the 128 threads of this group
-      if (hgrp == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
-      else asm volatile("bar.sync 2, 128;" ::: "memory");
-    };
-
-    const uint32_t leader_tmem_empty = PAIR ? mapa_u32(smem_u32(&tmem_empty_bar[0]), 0) : 0u;
-    auto release_acc = [&](uint32_t acc) {   // this group's 128 threads have read the accumulator
-      if (PAIR && rank != 0)
-        mbar_arrive_cluster(leader_tmem_empty + acc * (uint32_t)sizeof(uint64_t));
-      else
-        mbar_arrive(&tmem_empty_bar[acc]);
-    };
-    // residual chunk stream (epi_tma only): this group's chunks, in order and across tiles; chunk number gq of
-    // the group lives in residual tile (H == 2 ? hgrp : gq & 1); the issuer keeps NBUF chunks in flight.
-    // (pf_tile, pf_c) = next chunk to fetch.
-    WorkIter pfi;                    // walks ahead over the segments that run the epilogue proper (k0 == 0)
-    pfi.init(p.sk, num_kb, num_units, unit0, ustep);
-    int pf_tile = -1, pf_c = hgrp;
-    auto pf_advance = [&]() {
-      int uu, a, b;
-      pf_tile = -1;
-      while (pfi.next(uu, a, b))
-        if (a == 0) {
-          pf_tile = uu;
-          break;
-        }
-    };
-    pf_advance();
-    uint32_t pf_g = 0;
-    auto prefetch_res = [&]() {
-      while (pf_tile >= 0) {
-        const TileCoord tcp = decode_unit<PAIR>(p, pf_tile, rank, BN);
-        const int nch = (min(BN, p.Cout - tcp.n0) + 63) >> 6;
-        if (pf_c >= nch) {            // this group has no (more) chunks in that tile
-          pf_c = hgrp;
-          pf_advance();
-          continue;
-        }
-        const uint32_t buf = (NBUF == 1) ? (uint32_t)hgrp : (pf_g & 1u);
-        mbar_expect_tx(&res_full_bar[buf], (uint32_t)p.a_box_bytes * (uint32_t)NPL);
-#pragma unroll
-        for (int pl = 0; pl < NPL; ++pl)
-          tma_load_4d(res_base + buf * BUF_BYTES + pl * A_STAGE_BYTES, &p.tmR, &res_full_bar[buf],
-                      tcp.n0 + pf_c * 64 + pl * p.Cout, tcp.x0, tcp.y0, tcp.b);
-        ++pf_g;
-        pf_c += H;
-        return;
-      }
-    };
-    if (p.epi_tma && has_res && issuer) {
-      for (int i = 0; i < NBUF; ++i) prefetch_res();
-    }
-
-    uint32_t t = 0, g = 0;  // local segment counter, staged-chunk counter of this group
+    // ===================== MMA warpgroups: main loop + epilogue =====================
+    const int cw = warp / 4 - 1;              // MMA warpgroup
+    const int ct = threadIdx.x - 128;         // 0 .. 128*H - 1
+    const int wq = warp & 3;
+    const bool signaller = (threadIdx.x & 127) == 0;
+    const bool has_res_tile = (p.residual != nullptr) && !p.res_direct && p.epi_tma;
+    const int nbuf = SPLIT ? 1 : 2;            // staging / residual buffers (a buffer = NPL tiles of 16 KB)
+    uint8_t* out_base = smem + p.out_off;
+    uint8_t* res_base = smem + p.res_off;
+    float acc[MH][NPL][NACC];
+    uint32_t kbg = 0, g = 0;
     WorkIter wi;
     wi.init(p.sk, num_kb, num_units, unit0, ustep);
     int u, k0, k1;
     // stream-K bookkeeping: this CTA's workspace slot, and (for the head of a split unit) the slots it collects
     const int sk_slot = PAIR ? 2 * unit0 + rank : unit0;
-    for (; wi.next(u, k0, k1); ++t) {
+    while (wi.next(u, k0, k1)) {
       const TileCoord tc_ = decode_unit<PAIR>(p, u, rank, BN);
       const bool sk_dump = (k0 > 0);                       // tail / middle of a unit: leave a partial tile
       const bool sk_head = (k0 == 0 && k1 < num_kb);       // head of a split unit: add the partials, then finish
+      const int x0 = tc_.x0, y0 = tc_.y0, b = tc_.b, n0 = tc_.n0;
+      const int nchunks = (min(BN, p.Cout - n0) + 63) >> 6;
+      if (has_res_tile && !sk_dump && ct == 0) {   // the residual of chunk 0 travels during the main loop
+        const uint32_t buf = (nbuf == 1) ? 0u : (g & 1u);
+        mbar_expect_tx(&res_full_bar[buf], (uint32_t)p.a_box_bytes * (uint32_t)NPL);
+#pragma unroll
+        for (int pl = 0; pl < NPL; ++pl)
+          tma_load_4d(res_base + buf * (NPL * A_STAGE_BYTES) + pl * A_STAGE_BYTES, &p.tmR, &res_full_bar[buf],
+                      n0 + pl * p.Cout, x0, y0, b);
+      }
+      mma_tile<BN, MH, H, SPLIT, PAIR>(acc, smem, full_bar, empty_bar, stages, STAGE_BYTES, A_BYTES, B_PLANE_BYTES, kbg,
+                                       k1 - k0, cw, signaller);
+      // stream-K partial tiles: slot-major, then accumulator register, then thread (coalesced)
+      const size_t ws_stride = (size_t)128 * H;
+      if (sk_dump) {
+        float* w = p.sk_ws + (size_t)sk_slot * BLOCK_M * BN + ct;
+#pragma unroll
+        for (int mh = 0; mh < MH; ++mh)
+#pragma unroll
+          for (int i = 0; i < NACC; ++i) __stcg(w + (mh * NACC + i) * ws_stride, acc[mh][0][i]);
+        __threadfence();     // the partial is visible device-wide before the flag
+        mma_bar_sync(128 * H);
+        if (ct == 0) asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p.sk_flags + 2 * sk_slot), "r"(1) : "memory");
+        continue;
+      }
       int sk_parts = 0;
-      if (sk_head) {
+      if (sk_head) {   // the partial tiles of this unit's other k ranges (the following CTAs / clusters left them first thing)
         const long long total = (long long)num_units * num_kb, unit_end = (long long)(u + 1) * num_kb;
         while (unit0 + 1 + sk_parts < ustep && WorkIter::share_lo(total, unit0 + 1 + sk_parts, ustep) < unit_end) ++sk_parts;
-      }
-      const int x0 = tc_.x0, y0 = tc_.y0, b = tc_.b, n0 = tc_.n0;
-      const uint32_t acc = t % (uint32_t)acc_stages;
-      const uint32_t use = t / (uint32_t)acc_stages;
-      const uint32_t tmem_acc = tmem_base + acc * (uint32_t)(NPL * BN) + ((uint32_t)(quad * 32) << 16);
-      // bias of this tile's BN output channels -> this group's copy in shared memory (broadcast float4 reads)
-      {
-        const int et = (threadIdx.x - 64) & 127;   // 0..127 within the group
-        for (int j = et; j < BN; j += 128) my_bias[j] = (p.bias && n0 + j < p.Cout) ? __ldg(p.bias + n0 + j) : 0.f;
-      }
-      mbar_wait(&tmem_full_bar[acc], use & 1u);
-      tc_fence_after();
-      group_sync();   // bias visible; the group's readers of the previous tile's bias are done
-
-      if (sk_dump) {
-        // ---- stream-K partial: the combined fp32 accumulator of this group's chunks goes to the CTA's workspace slot
-        const int nchunks = (min(BN, p.Cout - n0) + 63) >> 6;
-        float* wrow = p.sk_ws + ((size_t)sk_slot * BLOCK_M + (size_t)row) * BN;
-#pragma unroll 1
-        for (int c = hgrp; c < nchunks; c += H) {
-          uint32_t r0[32], r1[32];
-          tmem_ld32_nowait(tmem_acc + (uint32_t)(c * 64), r0);
-          tmem_ld32_nowait(tmem_acc + (uint32_t)(c * 64 + 32), r1);
-          if (SPLIT) {
-            uint32_t q[32];
-            tmem_ld32_nowait(tmem_acc + (uint32_t)(BN + c * 64), q);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) r0[j] = __float_as_uint(__fmaf_rn(__uint_as_float(q[j]), YB_LO_INV, __uint_as_float(r0[j])));
-            tmem_ld32_nowait(tmem_acc + (uint32_t)(BN + c * 64 + 32), q);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) r1[j] = __float_as_uint(__fmaf_rn(__uint_as_float(q[j]), YB_LO_INV, __uint_as_float(r1[j])));
+        if (ct == 0)
+          for (int j = 1; j <= sk_parts; ++j) {
+            const int* f = p.sk_flags + 2 * (PAIR ? 2 * (unit0 + j) + rank : unit0 + j);
+            int v;
+            do {
+              asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(f) : "memory");
+            } while (v == 0);
           }
-          tmem_ld_wait();
-          uint4* w4 = reinterpret_cast<uint4*>(wrow + c * 64);
+        mma_bar_sync(128 * H);
+        for (int j = 1; j <= sk_parts; ++j) {
+          const int slot = PAIR ? 2 * (unit0 + j) + rank : unit0 + j;
+          const float* w = p.sk_ws + (size_t)slot * BLOCK_M * BN + ct;
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            w4[j] = make_uint4(r0[4 * j], r0[4 * j + 1], r0[4 * j + 2], r0[4 * j + 3]);
-            w4[8 + j] = make_uint4(r1[4 * j], r1[4 * j + 1], r1[4 * j + 2], r1[4 * j + 3]);
-          }
+          for (int mh = 0; mh < MH; ++mh)
+#pragma unroll
+            for (int i = 0; i < NACC; ++i) acc[mh][0][i] += __ldcg(w + (mh * NACC + i) * ws_stride);
         }
-        tc_fence_before();
-        __threadfence();     // the partial is visible device-wide before the flag
-        group_sync();
-        if (issuer) {
-          release_acc(acc);
-          asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p.sk_flags + 2 * sk_slot + hgrp), "r"(1) : "memory");
-        }
-      } else if (p.epi_tma) {
-        // ---- staged epilogue: TMEM -> regs -> (+bias, +residual from smem, act) -> swizzled smem tile
-        //      -> one TMA store per 64-channel chunk (full 128-byte lines, OOB rows clipped by hardware)
-        const int nchunks = (min(BN, p.Cout - n0) + 63) >> 6;
-        if (sk_head) {   // the partial tiles of this unit's other k ranges (the following CTAs / clusters left them first thing)
-          if (issuer)
-            for (int j = 1; j <= sk_parts; ++j) {
-              const int* f = p.sk_flags + 2 * (PAIR ? 2 * (unit0 + j) + rank : unit0 + j) + hgrp;
-              int v;
-              do {
-                asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(f) : "memory");
-              } while (v == 0);
+      }
+      if (p.epi_tma) {
+        EpiArgs e;
+        e.tmY = &p.tmY;
+        e.tmR = &p.tmR;
+        e.res_full_bar = res_full_bar;
+        e.out_base = out_base;
+        e.res_base = res_base;
+        e.bias = p.bias;
+        // res_direct (flattened 1x1 layouts only): pixel = x0 + row, both planes of the pixel are contiguous
+        e.res_g = (p.res_direct && p.residual) ? p.residual + (size_t)x0 * (size_t)(NPL * p.Cout) + n0 : nullptr;
+        e.res_pix_stride = NPL * p.Cout;
+        e.res_tx = (uint32_t)p.a_box_bytes * (uint32_t)NPL;
+        e.Wo = p.Wo;
+        e.Cout = p.Cout;
+        e.n0 = n0;
+        e.x0 = x0;
+        e.y0 = y0;
+        e.b = b;
+        e.nchunks = nchunks;
+        e.nbuf = nbuf;
+        e.out_scale = p.out_scale;
+        epi_staged_act<SPLIT, BN, MH, H>(p.act, p.res_after_act, acc, e, has_res_tile, g, cw, ct, lane, wq);
+      } else {
+        // ---- direct epilogue (fp32 / unaligned outputs: the head tensors): each thread stores its fragment's
+        //      channel pairs of its rows
+        const int ncols = min(BN, p.Cout - n0);
+        const int raa = p.res_after_act;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          if (8 * j >= ncols) break;
+#pragma unroll
+          for (int e2 = 0; e2 < 2; ++e2) {
+            const int cl = 8 * j + 2 * (lane & 3) + e2;
+            if (cl >= ncols) continue;
+            const int n = n0 + cl;
+            const float bias_n = p.bias ? __ldg(p.bias + n) : 0.f;
+            int act = p.act;
+            // fused prediction head: this channel belongs to one of up to 3 output tensors
+            float* seg_base = nullptr;
+            long long seg_bs = 0;
+            int seg_ps = 0, seg_c = 0;
+            if (p.nseg > 0) {
+#pragma unroll
+              for (int sg = 0; sg < 3; ++sg)
+                if (sg < p.nseg && n >= p.seg_begin[sg] && n < p.seg_end[sg]) {
+                  seg_base = p.seg_y[sg];
+                  seg_bs = p.seg_bs[sg];
+                  seg_ps = p.seg_ps[sg];
+                  seg_c = n - p.seg_begin[sg];
+                  act = p.seg_act[sg];
+                }
             }
-          group_sync();
-        }
-        const int c_last = ((nchunks - 1 - hgrp) / H) * H + hgrp;   // this group's last chunk (< hgrp: none)
-        if (nchunks <= hgrp) {   // nothing to read for this group in this tile
-          tc_fence_before();
-          if (issuer) release_acc(acc);
-        }
-#pragma unroll 1
-        for (int c = hgrp; c < nchunks; c += H, ++g) {
-          const uint32_t buf = (NBUF == 1) ? (uint32_t)hgrp : (g & 1u);
-          uint8_t* out_tile = out_base + buf * BUF_BYTES;
-          uint8_t* res_tile = res_base + buf * BUF_BYTES;
-          if (g >= (uint32_t)NBUF) {
-            if (issuer) bulk_wait_read<NBUF - 1>();  // the store that last used this staging tile has read it
-            group_sync();
-          }
-          uint32_t r0[32], r1[32];
-          tmem_ld32_nowait(tmem_acc + (uint32_t)(c * 64), r0);
-          tmem_ld32_nowait(tmem_acc + (uint32_t)(c * 64 + 32), r1);
-          if (SPLIT) {   // + 2^-11 * (A_lo*W_hi + A_hi*W_lo), from the tile's second accumulator
-            uint32_t q[32];
-            tmem_ld32_nowait(tmem_acc + (uint32_t)(BN + c * 64), q);
-            tmem_ld_wait();
 #pragma unroll
-            for (int j = 0; j < 32; ++j) r0[j] = __float_as_uint(__fmaf_rn(__uint_as_float(q[j]), YB_LO_INV, __uint_as_float(r0[j])));
-            tmem_ld32_nowait(tmem_acc + (uint32_t)(BN + c * 64 + 32), q);
-            tmem_ld_wait();
+            for (int mh = 0; mh < MH; ++mh)
 #pragma unroll
-            for (int j = 0; j < 32; ++j) r1[j] = __float_as_uint(__fmaf_rn(__uint_as_float(q[j]), YB_LO_INV, __uint_as_float(r1[j])));
-          }
-          tmem_ld_wait();
-          if (sk_head) {
-            for (int j = 1; j <= sk_parts; ++j) {
-              const int slot = PAIR ? 2 * (unit0 + j) + rank : unit0 + j;
-              const float4* w4 = reinterpret_cast<const float4*>(p.sk_ws + ((size_t)slot * BLOCK_M + (size_t)row) * BN + c * 64);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 a = __ldcg(w4 + i), b = __ldcg(w4 + 8 + i);
-                r0[4 * i] = __float_as_uint(__uint_as_float(r0[4 * i]) + a.x);
-                r0[4 * i + 1] = __float_as_uint(__uint_as_float(r0[4 * i + 1]) + a.y);
-                r0[4 * i + 2] = __float_as_uint(__uint_as_float(r0[4 * i + 2]) + a.z);
-                r0[4 * i + 3] = __float_as_uint(__uint_as_float(r0[4 * i + 3]) + a.w);
-                r1[4 * i] = __float_as_uint(__uint_as_float(r1[4 * i]) + b.x);
-                r1[4 * i + 1] = __float_as_uint(__uint_as_float(r1[4 * i + 1]) + b.y);
-                r1[4 * i + 2] = __float_as_uint(__uint_as_float(r1[4 * i + 2]) + b.z);
-                r1[4 * i + 3] = __float_as_uint(__uint_as_float(r1[4 * i + 3]) + b.w);
+              for (int h = 0; h < 2; ++h) {
+                const int trow = (cw + mh * H) * 64 + wq * 16 + (lane >> 2) + 8 * h;
+                const int ty_ = trow / p.tw, tx_ = trow - ty_ * p.tw;
+                const int oy = y0 + ty_, ox = x0 + tx_;
+                if (trow >= p.tw * p.th || oy >= p.Ho || ox >= p.Wo || b >= p.nb) continue;
+                const long long pix = (long long)oy * p.Wo + ox;
+                const float a = acc[mh][0][j * 4 + 2 * h + e2];
+                float v = SPLIT ? __fmaf_rn(a, p.out_scale, bias_n) : a + bias_n;
+                float rsd = 0.f;
+                if (p.residual) {
+                  const __half* rp = p.residual + ((long long)b * p.res_batch_stride + pix * p.Cout) * NPL + n;
+                  rsd = __half2float(rp[0]);
+                  if (SPLIT) rsd += lo_to_f32(rp[p.Cout]);
+                }
+                if (!raa) v += rsd;
+                v = (act == ACT_RELU) ? fmaxf(v, 0.f) : (act == ACT_TANH) ? tanhf(v) : (act == ACT_LEAKY) ? (v > 0.f ? v : 0.1f * v) : v;
+                if (raa) v += rsd;
+                if (p.nseg > 0) {
+                  if (seg_base) seg_base[(long long)b * seg_bs + pix * seg_ps + seg_c] = v;
+                  continue;
+                }
+                const long long o = (long long)b * p.y_batch_stride + pix * p.y_pix_stride + n;
+                if (p.y_f32) {
+                  reinterpret_cast<float*>(p.y)[o] = v;
+                } else if (SPLIT) {   // y_pix_stride counts halfs and already includes both planes
+                  __half hi, lo;
+                  split_f32(v, hi, lo);
+                  reinterpret_cast<__half*>(p.y)[o] = hi;
+                  reinterpret_cast<__half*>(p.y)[o + p.Cout] = lo;
+                } else {
+                  reinterpret_cast<__half*>(p.y)[o] = from_f32<__half>(v);
+                }
               }
-            }
-          }
-          if (has_res) mbar_wait(&res_full_bar[buf], (NBUF == 1) ? (g & 1u) : ((g >> 1) & 1u));
-          const int nbase = n0 + c * 64;
-          const float* sb = my_bias + c * 64;
-          const uint8_t* rt = has_res ? res_tile : nullptr;
-          // res_direct (flattened 1x1 layouts only): pixel = x0 + row, both planes of the pixel are contiguous
-          const __half* rg = nullptr;
-          if (p.res_direct && x0 + row < p.Wo) rg = p.residual + (size_t)(x0 + row) * (size_t)(NPL * p.Cout) + nbase;
-          switch (p.act) {
-            case ACT_RELU: epi_chunk<ACT_RELU, false, SPLIT>(r0, r1, sb, rt, out_tile, (uint32_t)row, sw, p.out_scale, rg, p.Cout); break;
-            case ACT_LEAKY:
-              if (p.res_after_act)
-                epi_chunk<ACT_LEAKY, true, SPLIT>(r0, r1, sb, rt, out_tile, (uint32_t)row, sw, p.out_scale, rg, p.Cout);
-              else
-                epi_chunk<ACT_LEAKY, false, SPLIT>(r0, r1, sb, rt, out_tile, (uint32_t)row, sw, p.out_scale, rg, p.Cout);
-              break;
-            case ACT_TANH: epi_chunk<ACT_TANH, false, SPLIT>(r0, r1, sb, rt, out_tile, (uint32_t)row, sw, p.out_scale, rg, p.Cout); break;
-            default: epi_chunk<ACT_NONE, false, SPLIT>(r0, r1, sb, rt, out_tile, (uint32_t)row, sw, p.out_scale, rg, p.Cout); break;
-          }
-          fence_proxy_async();   // generic-proxy smem writes -> visible to the TMA (async proxy)
-          if (c == c_last) tc_fence_before();
-          group_sync();
-          if (issuer) {
-            if (c == c_last) release_acc(acc);  // all 128 threads of the group have read their rows
-            tma_store_4d(&p.tmY, out_tile, nbase, x0, y0, b);
-            if (SPLIT) tma_store_4d(&p.tmY, out_tile + A_STAGE_BYTES, nbase + p.Cout, x0, y0, b);
-            bulk_commit();
-            if (has_res) prefetch_res();   // the group is done reading res_tile[buf]: refill it
           }
         }
-        if (sk_head && issuer)   // every thread of the group has read the partials (barrier above): re-arm the flags
+      }
+      if (sk_head) {   // every thread has read the partials: re-arm the flags
+        mma_bar_sync(128 * H);
+        if (ct == 0)
           for (int j = 1; j <= sk_parts; ++j)
-            asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(p.sk_flags + 2 * (PAIR ? 2 * (unit0 + j) + rank : unit0 + j) + hgrp),
+            asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(p.sk_flags + 2 * (PAIR ? 2 * (unit0 + j) + rank : unit0 + j)),
                          "r"(0)
                          : "memory");
-      } else {
-        // ---- direct epilogue (fp32 / unaligned outputs: the head tensors): each warp transposes its
-        //      32 rows x 32 columns through shared memory so that a store instruction writes 32
-        //      consecutive channels of ONE pixel (coalesced), not one channel of 32 pixels.
-        float* tbuf = reinterpret_cast<float*>(out_base) + (hgrp * 4 + quad) * (32 * 33);
-        const int ncols = min(BN, p.Cout - n0);
-#pragma unroll 1
-        for (int c0 = hgrp * 32; c0 < ncols; c0 += 32 * H) {
-          uint32_t r[32];
-          tmem_ld32(tmem_acc + (uint32_t)c0, r);
-          if (SPLIT) {
-            uint32_t q[32];
-            tmem_ld32(tmem_acc + (uint32_t)(BN + c0), q);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__fmaf_rn(__uint_as_float(q[j]), YB_LO_INV, __uint_as_float(r[j])));
-          }
-          const int nbase = n0 + c0;
-          const int nvalid = min(32, p.Cout - nbase);
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) tbuf[lane * 33 + j] = __uint_as_float(r[j]);
-          __syncwarp();
-          const float bias_l = my_bias[c0 + lane];
-          int act = p.act;
-          const int raa = p.res_after_act;
-          // fused prediction head: this lane's channel belongs to one of up to 3 output tensors
-          float* seg_base = nullptr;
-          long long seg_bs = 0;
-          int seg_ps = 0, seg_c = 0;
-          if (p.nseg > 0) {
-            const int n = nbase + lane;
-#pragma unroll
-            for (int sg = 0; sg < 3; ++sg)
-              if (sg < p.nseg && n >= p.seg_begin[sg] && n < p.seg_end[sg]) {
-                seg_base = p.seg_y[sg];
-                seg_bs = p.seg_bs[sg];
-                seg_ps = p.seg_ps[sg];
-                seg_c = n - p.seg_begin[sg];
-                act = p.seg_act[sg];
-              }
-          }
-          for (int rr = 0; rr < 32; ++rr) {
-            const int trow = quad * 32 + rr;
-            const int ty_ = trow / p.tw, tx_ = trow - ty_ * p.tw;
-            const int oy = y0 + ty_, ox = x0 + tx_;
-            if (trow >= p.tw * p.th || oy >= p.Ho || ox >= p.Wo || b >= p.nb) continue;   // warp-uniform
-            if (lane >= nvalid) continue;
-            const long long pix = (long long)oy * p.Wo + ox;
-            float v = SPLIT ? __fmaf_rn(tbuf[rr * 33 + lane], p.out_scale, bias_l) : tbuf[rr * 33 + lane] + bias_l;
-            float rsd = 0.f;
-            if (has_res) {
-              const __half* rp = p.residual + ((long long)b * p.res_batch_stride + pix * p.Cout) * NPL + nbase + lane;
-              rsd = __half2float(rp[0]);
-              if (SPLIT) rsd += lo_to_f32(rp[p.Cout]);
-            }
-            if (!raa) v += rsd;
-            v = (act == ACT_RELU) ? fmaxf(v, 0.f) : (act == ACT_TANH) ? tanhf(v) : (act == ACT_LEAKY) ? (v > 0.f ? v : 0.1f * v) : v;
-            if (raa) v += rsd;
-            if (p.nseg > 0) {
-              if (seg_base) seg_base[(long long)b * seg_bs + pix * seg_ps + seg_c] = v;
-              continue;
-            }
-            const long long o = (long long)b * p.y_batch_stride + pix * p.y_pix_stride + nbase + lane;
-            if (p.y_f32) {
-              reinterpret_cast<float*>(p.y)[o] = v;
-            } else if (SPLIT) {   // y_pix_stride counts halfs and already includes both planes
-              __half hi, lo;
-              split_f32(v, hi, lo);
-              reinterpret_cast<__half*>(p.y)[o] = hi;
-              reinterpret_cast<__half*>(p.y)[o + p.Cout] = lo;
-            } else {
-              reinterpret_cast<__half*>(p.y)[o] = from_f32<__half>(v);
-            }
-          }
-        }
-        tc_fence_before();
-        group_sync();
-        if (issuer) release_acc(acc);
       }
     }
-    if (p.epi_tma && issuer) bulk_wait_read<0>();  // smem must outlive the bulk reads
+    if (p.epi_tma && ct == 0) bulk_wait_read<0>();  // smem must outlive the bulk reads
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (PAIR) cluster_sync_all();   // no CTA leaves while its peer's MMAs / signals may still touch it
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_dyn(tmem_base, (uint32_t)p.tmem_cols);
-  }
+  if (PAIR) cluster_sync_all();   // no CTA leaves while its peer may still multicast into it or signal its barriers
 }
 
 // ---------------------------------------------------------------------------------------------
 // chain kernel: a run of consecutive convolutions (the 1x1 -> 3x3 -> 1x1 (+residual) bottleneck blocks of one ResNet
 // stage, backbone.py:37-57) in ONE persistent launch
 // ---------------------------------------------------------------------------------------------
-// Every layer of the chain is an ordinary plan of the shape <BN = 128, single CTA, two epilogue groups, staged TMA
-// epilogue, residual read from global memory>; their parameter blocks (tensor maps included) sit in an array in global
+// Every layer of the chain is an ordinary plan of the shape <BN = 128 or 64, single CTA, two MMA warpgroups,
+// staged TMA epilogue, residual read from global memory>; their parameter blocks (tensor maps included) sit in an array in global
 // memory.  The work units of all layers form ONE list (layer-major, then M tile, then N tile) that is dealt round-robin
-// to the 148 CTAs, so a CTA moves from its last tile of layer L straight to its first tile of layer L + 1: no launch,
-// no prologue (barriers, TMEM allocation, descriptor fetch), no tail where most SMs idle -- the three pipelines of a
-// CTA (TMA ring, TMEM accumulators, staging tiles) simply keep running across the layer boundary.
-// Dependencies are tracked per M tile instead of by a grid-wide barrier: the epilogue groups bump done[layer][m tile]
-// once their stores of a tile have completed; before the first ACTIVATION load of a tile the producer warp waits until
+// to the CTAs (one per SM), so a CTA moves from its last tile of layer L straight to its first tile of layer L + 1: no launch,
+// no prologue (barriers, descriptor fetch), no tail where most SMs idle -- the TMA ring and the
+// staging tiles of a CTA simply keep running across the layer boundary.
+// Dependencies are tracked per M tile instead of by a grid-wide barrier: thread 0 of the MMA warpgroups bumps done[layer][m tile]
+// once the stores of a tile have completed; before the first ACTIVATION load of a tile the producer warp waits until
 // every tile of the layer that produces its input which overlaps the input rows the tile reads (its own rows mapped
 // through stride / padding / kernel height), and every tile of the layer that produces its residual which overlaps its
 // own rows, has been finished by all its N tiles (the weight tiles of the first k-blocks are requested before the
@@ -862,7 +697,7 @@ struct ChainLayer {
   int W, H, rows;          // OUTPUT image size; rows = B * H  (global row r = b * H + y, pixel = r * W + x)
   int tw, th, tiles_x, tiles_y;
   int done_off;            // this layer's counters: done[done_off + m_tile]
-  int target;              // a finished M tile: n_tiles * 2 (each epilogue group of each N tile adds 1)
+  int target;              // a finished M tile: n_tiles (each N tile adds 1 once its stores have completed)
   int dep_a;               // chain layer that writes this layer's input (-1: a tensor complete before the launch)
   int dep_r;               // chain layer that writes this layer's residual (-1: none / outside / implied by dep_a's own dependencies)
   int stride, pad, kh;     // output row y reads input rows [y * stride - pad, y * stride - pad + kh)
@@ -918,9 +753,9 @@ __device__ __forceinline__ void red_release_gpu_add(int* p, int v) {
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
 
-// H epilogue groups of 4 warps; each group owns an 8 KB (x 2 planes) staging buffer: H = 2 leaves room for three
-// split-precision stages, H = 4 for two
-__host__ __device__ constexpr int chain_stages(bool split, int h) { return split ? (h == 4 ? 2 : 3) : 6; }
+// pipeline stages of the chain kernel: the ring plus NPL x 16 KB staging tiles per buffer (two buffers in the fp16 mode,
+// one in the split mode) fill the 227 KB of an SM
+__host__ __device__ constexpr int chain_stages(bool split) { return split ? 3 : 6; }
 __device__ __forceinline__ bool mbar_test_wait(uint32_t addr, uint32_t parity) {   // non-blocking
   uint32_t ok;
   asm volatile(
@@ -941,35 +776,24 @@ __device__ __forceinline__ int chain_first_unit(int cta, int ubase, int G) {
   return r < 0 ? r + G : r;
 }
 
-template <bool SPLIT, int H>
-__global__ void __launch_bounds__(64 + 128 * H)
+template <bool SPLIT>
+__global__ void __launch_bounds__(384, 1)
 tc_chain_kernel(const TcParams* __restrict__ layers, const ChainLayer* __restrict__ info, int nl, int* __restrict__ done,
                 long long* __restrict__ stats) {
   // stats (diagnostics, YB_CHAIN_STATS=1; null otherwise): per CTA 8 counters of SM cycles spent waiting --
-  // [0] producer: dependency counters, [1] producer: free ring slot, [2] MMA issuer: operands, [3] MMA issuer: free
-  // accumulator, [4] epilogue group 0: accumulator, [5] epilogue group 0: store completion before a signal, [6] whole kernel
+  // [0] producer: dependency counters, [1] producer: free ring slot, [4] MMA warpgroups: store completion before a
+  // signal, [6] whole kernel (the others stay 0)
   const long long t_kernel0 = stats ? clock64() : 0;
   long long w0 = 0, w1 = 0;
-  constexpr int BN = 128;
   constexpr int NPL = SPLIT ? 2 : 1;
-  constexpr int B_PLANE_BYTES = BN * BLOCK_K * 2;
+  constexpr int B_PLANE_BYTES = 128 * BLOCK_K * 2;
   constexpr int A_BYTES = NPL * A_STAGE_BYTES;
   constexpr int STAGE_BYTES = A_BYTES + NPL * B_PLANE_BYTES;
-  constexpr int BUF_BYTES = NPL * CHUNK32_BYTES;
-  // the chain's own shared-memory layout (the plans' stage counts / offsets are not used): ring, then one staging
-  // buffer per epilogue group; two TMEM accumulator buffers.  The epilogue moves 32-channel chunks (8 KB tiles), which
-  // leaves room for a THIRD split-precision stage (3 x 64 KB + 32 KB).  Measured (profiles/r2_call14_summary.txt): the
-  // 105-layer trunk chain 2.14 -> 1.92 ms at batch 2, unchanged (3.59 ms) at batch 8, where the MMA issuer's operand
-  // waits are set by the L2 -> SM rate rather than by the bytes a CTA keeps in flight
-  constexpr int stages = chain_stages(SPLIT, H);
+  constexpr int stages = chain_stages(SPLIT);
 
   extern __shared__ uint8_t smem_dyn[];
   __shared__ uint64_t full_bar[MAX_STAGES];
   __shared__ uint64_t empty_bar[MAX_STAGES];
-  __shared__ uint64_t tmem_full_bar[2];
-  __shared__ uint64_t tmem_empty_bar[2];
-  __shared__ uint32_t s_tmem_base;
-  __shared__ __align__(16) float sbias[H * BN];
 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
   const int warp = threadIdx.x >> 5;
@@ -978,303 +802,193 @@ tc_chain_kernel(const TcParams* __restrict__ layers, const ChainLayer* __restric
   const int G = (int)gridDim.x;
   const int cta = (int)blockIdx.x;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], H);
+      mbar_init(&empty_bar[s], 2);
     }
     fence_barrier_init();
     tma_prefetch_desc(&layers[0].tmB);
     tma_prefetch_desc(&layers[0].tmA[0]);
-    tma_prefetch_desc(&layers[0].tmY32);
+    tma_prefetch_desc(&layers[0].tmY);
   }
-  if (warp == 1) tmem_alloc_dyn(&s_tmem_base, 512u);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem_base;
 
-  if (warp == 0) {
-    // ===================== TMA producer (lane 0 issues; the whole warp polls the dependency counters) =====================
-    uint32_t kbg = 0;
-    for (int L = 0; L < nl; ++L) {
-      const TcParams& p = layers[L];
-      const ChainLayer ci = info[L];
-      const int num_kb = p.ntaps * p.kchunks;
-      const int bn = p.bn;
-      const uint32_t tx_bytes = ((uint32_t)p.a_box_bytes + (uint32_t)(bn * BLOCK_K * 2)) * (uint32_t)NPL;
-      if (lane == 0 && L + 1 < nl) {   // the next layer's descriptors: fetched long before their first use
-        tma_prefetch_desc(&layers[L + 1].tmB);
-        tma_prefetch_desc(&layers[L + 1].tmA[0]);
-      }
-      const bool nodeps = (ci.dep_a < 0 && ci.dep_r < 0);
-      // the counters M tile m of this layer waits for: entry i of the list (input tiles first, then residual tiles);
-      // returns the length of the list
-      auto dep_of = [&](int m, int i, const int*& c, int& tgt) -> int {
-        int r0, r1;
-        chain_rows_of_tile(ci, m, r0, r1);
-        int ia = 0, ib = -1, ja = 0, jb = -1, ta = 0, tr = 0;
-        const int *ca = done, *cr = done;
-        if (ci.dep_a >= 0) {   // input rows, in the producer's row numbering (its image height differs under a stride)
-          const ChainLayer pa = info[ci.dep_a];
-          int ra, rb;
-          chain_input_rows(ci, pa, r0, r1, ra, rb);
-          chain_tiles_of_rows(pa, ra, rb, ia, ib);
-          ca = done + pa.done_off;
-          ta = pa.target;
-        }
-        if (ci.dep_r >= 0) {   // the residual has this layer's geometry
-          const ChainLayer pr = info[ci.dep_r];
-          chain_tiles_of_rows(pr, r0, r1, ja, jb);
-          cr = done + pr.done_off;
-          tr = pr.target;
-        }
-        const int na = ib - ia + 1, nr = jb - ja + 1;
-        if (i < na) {
-          c = ca + ia + i;
-          tgt = ta;
-        } else {
-          c = cr + ja + (i - na);
-          tgt = tr;
-        }
-        return na + nr;
-      };
-      // (Reading the NEXT tile's counters ahead of time, so that a satisfied check costs no L2 round trip in front of the
-      // tile, was tried: the producer's waiting share fell from 30 % to 18 %, the kernel time did not move -- 3.745 vs
-      // 3.740 ms, profiles/r2_call19_summary.txt: the MMA issuer waits for the operands themselves.  Removed.)
-      for (int u = chain_first_unit(cta, ci.ubase, G); u < ci.units; u += G) {
-        const TileCoord tc_ = decode_unit<false>(p, u, 0, bn);
-        bool ready = nodeps;
-        for (int kb = 0; kb < num_kb; ++kb, ++kbg) {
-          const uint32_t s = kbg % (uint32_t)stages;
-          const uint32_t it = kbg / (uint32_t)stages;
-          const int tap = kb / p.kchunks;
-          const int kc = kb - tap * p.kchunks;
-          uint8_t* sa = smem + (size_t)s * STAGE_BYTES;
-          uint8_t* sb = sa + A_BYTES;
-          if (lane == 0) {
-            const long long t0 = stats ? clock64() : 0;
-            mbar_wait(&empty_bar[s], (it & 1u) ^ 1u);
-            if (stats) w1 += clock64() - t0;
-            mbar_expect_tx(&full_bar[s], tx_bytes);
-#pragma unroll
-            for (int pl = 0; pl < NPL; ++pl)   // weights: constants, no dependency
-              tma_load_3d(sb + pl * B_PLANE_BYTES, &p.tmB, &full_bar[s], kc * BLOCK_K + pl * p.cin, tc_.n0, tap);
-          }
-          if (!ready) {
-            const long long tdep0 = stats ? clock64() : 0;
-            __syncwarp();
-            const int* c = done;
-            int tgt = 0;
-            const int n = dep_of(u / p.n_tiles, lane, c, tgt);
-            for (int i = lane; i < n; i += 32) {
-              if (i != lane) dep_of(u / p.n_tiles, i, c, tgt);
-#ifdef YB_WATCHDOG
-              const long long t0 = clock64();
-#endif
-              while (ld_acquire_gpu(c) < tgt) {
-#ifdef YB_WATCHDOG
-                if (clock64() - t0 > 4000000000ll) asm volatile("trap;");
-#endif
-              }
-            }
-            __syncwarp();
-            if (stats) w0 += clock64() - tdep0;
-            fence_proxy_async_all();   // the tiles were written through the async proxy (TMA stores) and are read through it
-            ready = true;
-          }
-          if (lane == 0) {
-            const CUtensorMap* ma = &p.tmA[p.tap_map[tap]];
-            const int ax = tc_.x0 + p.tap_dx[tap], ay = tc_.y0 + p.tap_dy[tap];
-#pragma unroll
-            for (int pl = 0; pl < NPL; ++pl)
-              tma_load_4d(sa + pl * A_STAGE_BYTES, ma, &full_bar[s], kc * BLOCK_K + pl * p.cin, ax, ay, tc_.b);
-          }
-        }
-      }
-    }
-    if (stats && lane == 0) {
-      stats[cta * 8 + 0] = w0;
-      stats[cta * 8 + 1] = w1;
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (one thread) =====================
-    if (lane == 0) {
-      uint32_t kbg = 0, t = 0;
+  if (warp < 4) {
+    // ===================== TMA producer (lane 0 of warp 0 issues; warp 0 polls the dependency counters) =====================
+    if (warp == 0) {
+      uint32_t kbg = 0;
       for (int L = 0; L < nl; ++L) {
         const TcParams& p = layers[L];
+        const ChainLayer ci = info[L];
         const int num_kb = p.ntaps * p.kchunks;
-        const uint32_t idesc = p.idesc;
-        const int ubase = info[L].ubase, units = info[L].units;
-        for (int u = chain_first_unit(cta, ubase, G); u < units; u += G, ++t) {
-          const uint32_t acc = t & 1u;
-          const uint32_t use = t >> 1;
-          long long t0 = stats ? clock64() : 0;
-          mbar_wait(&tmem_empty_bar[acc], (use & 1u) ^ 1u);
-          if (stats) w1 += clock64() - t0;
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + acc * (uint32_t)(NPL * BN);
+        const int bn = p.bn;
+        const uint32_t tx_bytes = ((uint32_t)p.a_box_bytes + (uint32_t)(bn * BLOCK_K * 2)) * (uint32_t)NPL;
+        if (lane == 0 && L + 1 < nl) {   // the next layer's descriptors: fetched long before their first use
+          tma_prefetch_desc(&layers[L + 1].tmB);
+          tma_prefetch_desc(&layers[L + 1].tmA[0]);
+        }
+        const bool nodeps = (ci.dep_a < 0 && ci.dep_r < 0);
+        // the counters M tile m of this layer waits for: entry i of the list (input tiles first, then residual tiles);
+        // returns the length of the list
+        auto dep_of = [&](int m, int i, const int*& c, int& tgt) -> int {
+          int r0, r1;
+          chain_rows_of_tile(ci, m, r0, r1);
+          int ia = 0, ib = -1, ja = 0, jb = -1, ta = 0, tr = 0;
+          const int *ca = done, *cr = done;
+          if (ci.dep_a >= 0) {   // input rows, in the producer's row numbering (its image height differs under a stride)
+            const ChainLayer pa = info[ci.dep_a];
+            int ra, rb;
+            chain_input_rows(ci, pa, r0, r1, ra, rb);
+            chain_tiles_of_rows(pa, ra, rb, ia, ib);
+            ca = done + pa.done_off;
+            ta = pa.target;
+          }
+          if (ci.dep_r >= 0) {   // the residual has this layer's geometry
+            const ChainLayer pr = info[ci.dep_r];
+            chain_tiles_of_rows(pr, r0, r1, ja, jb);
+            cr = done + pr.done_off;
+            tr = pr.target;
+          }
+          const int na = ib - ia + 1, nr = jb - ja + 1;
+          if (i < na) {
+            c = ca + ia + i;
+            tgt = ta;
+          } else {
+            c = cr + ja + (i - na);
+            tgt = tr;
+          }
+          return na + nr;
+        };
+        for (int u = chain_first_unit(cta, ci.ubase, G); u < ci.units; u += G) {
+          const TileCoord tc_ = decode_unit<false>(p, u, 0, bn);
+          bool ready = nodeps;
           for (int kb = 0; kb < num_kb; ++kb, ++kbg) {
             const uint32_t s = kbg % (uint32_t)stages;
             const uint32_t it = kbg / (uint32_t)stages;
-            t0 = stats ? clock64() : 0;
-            mbar_wait(&full_bar[s], it & 1u);
-            if (stats) w0 += clock64() - t0;
-            tc_fence_after();
-            const uint32_t sa = smem_u32(smem + (size_t)s * STAGE_BYTES);
-            const uint32_t sb = sa + A_BYTES;
-            const uint64_t da = make_sw128_desc(sa);
-            const uint64_t db = make_sw128_desc(sb);
+            const int tap = kb / p.kchunks;
+            const int kc = kb - tap * p.kchunks;
+            uint8_t* sa = smem + (size_t)s * STAGE_BYTES;
+            uint8_t* sb = sa + A_BYTES;
+            if (lane == 0) {
+              const long long t0 = stats ? clock64() : 0;
+              mbar_wait(&empty_bar[s], (it & 1u) ^ 1u);
+              if (stats) w1 += clock64() - t0;
+              mbar_expect_tx(&full_bar[s], tx_bytes);
 #pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-              umma_f16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-            if (SPLIT) {
-              const uint64_t dal = make_sw128_desc(sa + A_STAGE_BYTES);
-              const uint64_t dbl = make_sw128_desc(sb + B_PLANE_BYTES);
-#pragma unroll
-              for (int k = 0; k < BLOCK_K / UMMA_K; ++k)   // A_lo * W_hi -> second accumulator
-                umma_f16(tmem_d + BN, dal + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-#pragma unroll
-              for (int k = 0; k < BLOCK_K / UMMA_K; ++k)   // A_hi * W_lo -> second accumulator
-                umma_f16(tmem_d + BN, da + (uint64_t)(2 * k), dbl + (uint64_t)(2 * k), idesc, 1u);
+              for (int pl = 0; pl < NPL; ++pl)   // weights: constants, no dependency
+                tma_load_3d(sb + pl * B_PLANE_BYTES, &p.tmB, &full_bar[s], kc * BLOCK_K + pl * p.cin, tc_.n0, tap);
             }
-            umma_commit(&empty_bar[s]);
+            if (!ready) {
+              const long long tdep0 = stats ? clock64() : 0;
+              __syncwarp();
+              const int* c = done;
+              int tgt = 0;
+              const int n = dep_of(u / p.n_tiles, lane, c, tgt);
+              for (int i = lane; i < n; i += 32) {
+                if (i != lane) dep_of(u / p.n_tiles, i, c, tgt);
+#ifdef YB_WATCHDOG
+                const long long t0 = clock64();
+#endif
+                while (ld_acquire_gpu(c) < tgt) {
+#ifdef YB_WATCHDOG
+                  if (clock64() - t0 > 4000000000ll) asm volatile("trap;");
+#endif
+                }
+              }
+              __syncwarp();
+              if (stats) w0 += clock64() - tdep0;
+              fence_proxy_async_all();   // the tiles were written through the async proxy (TMA stores) and are read through it
+              ready = true;
+            }
+            if (lane == 0) {
+              const CUtensorMap* ma = &p.tmA[p.tap_map[tap]];
+              const int ax = tc_.x0 + p.tap_dx[tap], ay = tc_.y0 + p.tap_dy[tap];
+#pragma unroll
+              for (int pl = 0; pl < NPL; ++pl)
+                tma_load_4d(sa + pl * A_STAGE_BYTES, ma, &full_bar[s], kc * BLOCK_K + pl * p.cin, ax, ay, tc_.b);
+            }
           }
-          umma_commit(&tmem_full_bar[acc]);
         }
       }
-      if (stats) {
-        stats[cta * 8 + 2] = w0;
-        stats[cta * 8 + 3] = w1;
+      if (stats && lane == 0) {
+        stats[cta * 8 + 0] = w0;
+        stats[cta * 8 + 1] = w1;
       }
     }
   } else {
-    // ===================== epilogue: H groups of 4 warps, group g takes the 32-channel chunks g, g + H, ... =====================
-    const int quad = warp & 3;
-    const int hgrp = (warp - 2) >> 2;
-    const int row = quad * 32 + lane;
-    const bool issuer = (warp == 2 + 4 * hgrp && lane == 0);
-    float* my_bias = sbias + hgrp * BN;
-    uint8_t* out_tile = out_base + hgrp * BUF_BYTES;
-    auto group_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(hgrp + 1) : "memory"); };
-    // issuer only: counter to bump once this thread's outstanding stores (the previous tile's) have completed
+    // ===================== two MMA warpgroups: 64 rows of every tile each =====================
+    const int cw = warp / 4 - 1;
+    const int ct = threadIdx.x - 128;
+    const int wq = warp & 3;
+    const bool signaller = (threadIdx.x & 127) == 0;
+    float acc[1][NPL][64];
+    // thread 0 only: counter to bump once this thread's outstanding stores (the previous tile's) have completed
     int* pending = nullptr;
     auto flush_pending = [&]() {
       const long long t0 = stats ? clock64() : 0;
       bulk_wait_all();            // the stores have been performed, not just read out of shared memory
-      if (stats) w1 += clock64() - t0;
+      if (stats) w0 += clock64() - t0;
       fence_proxy_async_all();
       red_release_gpu_add(pending, 1);
       pending = nullptr;
     };
-    uint32_t t = 0, g = 0;
+    uint32_t kbg = 0, g = 0;
     for (int L = 0; L < nl; ++L) {
       const TcParams& p = layers[L];
       const int ubase = info[L].ubase, units = info[L].units, done_off = info[L].done_off;
-      const int act = p.act, raa = p.res_after_act, Cout = p.Cout, res_direct = p.res_direct, Wo = p.Wo;
-      const float out_scale = p.out_scale;
-      const float* bias = p.bias;
-      const __half* residual = p.residual;
+      const int num_kb = p.ntaps * p.kchunks;
       const int n_tiles = p.n_tiles;
       const int bn = p.bn;
-      for (int u = chain_first_unit(cta, ubase, G); u < units; u += G, ++t) {
+      for (int u = chain_first_unit(cta, ubase, G); u < units; u += G) {
         const TileCoord tc_ = decode_unit<false>(p, u, 0, bn);
-        const int x0 = tc_.x0, y0 = tc_.y0, b = tc_.b, n0 = tc_.n0;
-        const uint32_t acc = t & 1u;
-        const uint32_t use = t >> 1;
-        const uint32_t tmem_acc = tmem_base + acc * (uint32_t)(NPL * BN) + ((uint32_t)(quad * 32) << 16);
-        {
-          const int et = (threadIdx.x - 64) & 127;
-          for (int j = et; j < bn; j += 128) my_bias[j] = (bias && n0 + j < Cout) ? __ldg(bias + n0 + j) : 0.f;
-        }
-        // The previous tile's completion signal waits for its stores; that is free when this tile's accumulator is
-        // not ready yet (the group would idle anyway).  When it IS ready the signal is deferred until the first chunk
-        // of this tile has been computed (by then the stores have long landed) -- safe, because a ready accumulator
-        // means this tile depends on nothing that could be waiting for the deferred signal.
-        if (issuer && pending && !mbar_test_wait(smem_u32(&tmem_full_bar[acc]), use & 1u)) flush_pending();
-        const long long tacc0 = stats ? clock64() : 0;
-        mbar_wait(&tmem_full_bar[acc], use & 1u);
-        if (stats) w0 += clock64() - tacc0;
-        tc_fence_after();
-        group_sync();
-        const int nchunks = (min(bn, Cout - n0) + 31) >> 5;   // 32-channel chunks: 4, or 2 for a 64-wide N tile
-        const int c_last = ((nchunks - 1 - hgrp) / H) * H + hgrp;
-        if (nchunks <= hgrp) {   // nothing for this group, which only hands the accumulator back
-          tc_fence_before();
-          if (issuer) {
-            mbar_arrive(&tmem_empty_bar[acc]);
-            if (pending) flush_pending();
-          }
-        }
-#pragma unroll 1
-        for (int c = hgrp; c < nchunks; c += H, ++g) {
-          if (g >= 1u) {
-            if (issuer) bulk_wait_read<0>();   // the store that last used this group's staging tile has read it
-            group_sync();
-          }
-          uint32_t r[32];
-          tmem_ld32_nowait(tmem_acc + (uint32_t)(c * 32), r);
-          if (SPLIT) {
-            uint32_t q[32];
-            tmem_ld32_nowait(tmem_acc + (uint32_t)(BN + c * 32), q);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__fmaf_rn(__uint_as_float(q[j]), YB_LO_INV, __uint_as_float(r[j])));
-          } else {
-            tmem_ld_wait();
-          }
-          const int nbase = n0 + c * 32;
-          const float* sb = my_bias + c * 32;
-          const __half* rg = nullptr;
-          if (res_direct && x0 + row < Wo) rg = residual + (size_t)(x0 + row) * (size_t)(NPL * Cout) + nbase;
-          switch (act) {
-            case ACT_RELU: epi_chunk32<ACT_RELU, false, SPLIT>(r, sb, out_tile, (uint32_t)row, out_scale, rg, Cout); break;
-            case ACT_LEAKY:
-              if (raa)
-                epi_chunk32<ACT_LEAKY, true, SPLIT>(r, sb, out_tile, (uint32_t)row, out_scale, rg, Cout);
-              else
-                epi_chunk32<ACT_LEAKY, false, SPLIT>(r, sb, out_tile, (uint32_t)row, out_scale, rg, Cout);
-              break;
-            default: epi_chunk32<ACT_NONE, false, SPLIT>(r, sb, out_tile, (uint32_t)row, out_scale, rg, Cout); break;
-          }
-          fence_proxy_async();
-          if (issuer && pending) flush_pending();   // deferred signal of the previous tile
-          if (c == c_last) tc_fence_before();
-          group_sync();
-          if (issuer) {
-            if (c == c_last) mbar_arrive(&tmem_empty_bar[acc]);
-            tma_store_4d(&p.tmY32, out_tile, nbase, x0, y0, b);
-            if (SPLIT) tma_store_4d(&p.tmY32, out_tile + CHUNK32_BYTES, nbase + Cout, x0, y0, b);
-            bulk_commit();
-          }
-        }
-        if (issuer) {
-          if (nchunks > hgrp) pending = done + done_off + u / n_tiles;
-          else red_release_gpu_add(done + done_off + u / n_tiles, 1);   // nothing stored: counts at once
-        }
+        // The previous tile's completion signal waits for its stores; that is free when this tile's operands are not
+        // ready yet (the warpgroups would idle anyway).  When they ARE ready the signal is deferred until after the
+        // main loop -- safe, because ready operands mean this tile depends on nothing that could be waiting for it.
+        if (ct == 0 && pending &&
+            !mbar_test_wait(smem_u32(&full_bar[kbg % (uint32_t)stages]), (kbg / (uint32_t)stages) & 1u))
+          flush_pending();
+        if (bn == 128)
+          mma_tile<128, 1, 2, SPLIT, false>(acc, smem, full_bar, empty_bar, stages, STAGE_BYTES, A_BYTES, B_PLANE_BYTES, kbg,
+                                            num_kb, cw, signaller);
+        else
+          mma_tile<64, 1, 2, SPLIT, false>(acc, smem, full_bar, empty_bar, stages, STAGE_BYTES, A_BYTES, B_PLANE_BYTES, kbg,
+                                           num_kb, cw, signaller);
+        if (ct == 0 && pending) flush_pending();
+        EpiArgs e;
+        e.tmY = &p.tmY;
+        e.tmR = &p.tmR;
+        e.res_full_bar = nullptr;
+        e.out_base = out_base;
+        e.res_base = nullptr;
+        e.bias = p.bias;
+        e.res_g = p.residual ? p.residual + (size_t)tc_.x0 * (size_t)(NPL * p.Cout) + tc_.n0 : nullptr;   // flattened layouts only
+        e.res_pix_stride = NPL * p.Cout;
+        e.res_tx = 0;   // (no staged residual in a chain)
+        e.Wo = p.Wo;
+        e.Cout = p.Cout;
+        e.n0 = tc_.n0;
+        e.x0 = tc_.x0;
+        e.y0 = tc_.y0;
+        e.b = tc_.b;
+        e.nchunks = bn / 64;
+        e.nbuf = SPLIT ? 1 : 2;
+        e.out_scale = p.out_scale;
+        if (bn == 128) epi_staged_act<SPLIT, 128, 1, 2>(p.act, p.res_after_act, acc, e, false, g, cw, ct, lane, wq);
+        else epi_staged_act<SPLIT, 64, 1, 2>(p.act, p.res_after_act, acc, e, false, g, cw, ct, lane, wq);
+        if (ct == 0) pending = done + done_off + u / n_tiles;
       }
     }
-    if (issuer) {
+    if (ct == 0) {
       if (pending) flush_pending();
       bulk_wait_read<0>();
-      if (stats && hgrp == 0) {
+      if (stats) {
         stats[cta * 8 + 4] = w0;
-        stats[cta * 8 + 5] = w1;
         stats[cta * 8 + 6] = clock64() - t_kernel0;
       }
     }
   }
-
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_dyn(tmem_base, 512u);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1283,6 +997,20 @@ tc_chain_kernel(const TcParams* __restrict__ layers, const ChainLayer* __restric
 int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
 
 }  // namespace
+
+// SMs of the current device (132 on an H100 SXM): the persistent grids hold one CTA (or pair) per SM, and the stream-K
+// workspace one slot per CTA
+int device_sms() {
+  static std::atomic<int> cached[64] = {};
+  int dev = 0;
+  YB_CHECK_CUDA(cudaGetDevice(&dev));
+  int n = cached[dev & 63].load();
+  if (n <= 0) {
+    YB_CHECK_CUDA(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
+    cached[dev & 63].store(n);
+  }
+  return n;
+}
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
@@ -1336,7 +1064,7 @@ struct TcConvPlan {
   int sk = 0;           // stream-K requested (effective once a workspace is attached: prm.sk)
   int BN = 128;
   int pair = 0;
-  int epi_groups = 1;   // H: 4-warp epilogue groups per CTA
+  int epi_groups = 1;   // H: MMA warpgroups per CTA (each owns 2/H of the tile's 64-row halves)
   int pdl_friendly = 0; // sized so that two CTAs (this kernel's and the next layer's) fit on one SM
   int flat = 0;         // 1x1 / stride 1 / dense: all pixels of the batch on one axis
   int B = 0, Ho = 0, Wo = 0;   // the problem's output geometry (prm.Ho / prm.Wo are the flattened view's)
@@ -1475,6 +1203,7 @@ TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, in
   const int bn_min = q.epi_tma ? 64 : 32;
 
   // ---- N tile: minimise waves * (BN + fixed cost)
+  const int sms = device_sms();
   {
     const int cands[4] = {256, 128, 64, 32};
     double best = 1e30;
@@ -1484,7 +1213,7 @@ TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, in
       if (bn < bn_min) continue;
       if (bn > bn_min && bn >= 2 * p.Cout) continue;  // more than half the tile would be padding
       long long ctas = m_tiles * ceil_div(p.Cout, bn);
-      long long waves = (ctas + 147) / 148;
+      long long waves = (ctas + sms - 1) / sms;
       double cost = (double)waves * (bn + 64);
       if (cost < best - 1e-9) {
         best = cost;
@@ -1495,80 +1224,51 @@ TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, in
     if (bn_override == 32 || bn_override == 64 || bn_override == 128 || bn_override == 256)
       plan->BN = std::max(bn_override, bn_min);
   }
-  // ---- CTA pairs: two adjacent M tiles per (cluster of 2), each CTA stages half of the weight tile
+  // ---- CTA pairs: two adjacent M tiles per (cluster of 2), each CTA loads half of the weight tile for both
   const int pair = (pair_override > 0 && m_tiles >= 2 && plan->BN >= 64) ? 1 : 0;
-  int epi_req = (epi_override == 2 && plan->BN >= 64) ? 2 : 1;
-  if (split) {
-    // every stage and every epilogue buffer is twice as large: step down (second epilogue group first, then the
-    // N tile) until at least two pipeline stages fit
-    auto stages_for = [&](int bn, int hg) {
-      const int sb = 2 * (A_STAGE_BYTES + (pair ? bn / 2 : bn) * BLOCK_K * 2);
-      const int tiles = 2 * hg;
-      const int ob = std::max(tiles * A_STAGE_BYTES, hg == 2 ? 36 * 1024 : 2 * A_STAGE_BYTES);
-      // two groups on a flattened layout read the residual from global memory (no staging tiles), see res_direct
-      const int rb = (q.epi_tma && p.residual && !(hg == 2 && flat)) ? tiles * A_STAGE_BYTES : 0;
-      return (221 * 1024 - ob - rb) / sb;
-    };
-    while (stages_for(plan->BN, epi_req) < 2) {
-      if (epi_req == 2) epi_req = 1;
-      else if (plan->BN > std::max(bn_min, pair ? 64 : 32)) plan->BN /= 2;
-      else break;
-    }
-  }
+  // PDL-friendly plan: <= ~108 KB of shared memory and one MMA warpgroup, so that a CTA of the NEXT layer can become
+  // resident beside it and overlap its prologue + first weight tiles
+  const int pdlf = (pdl_override > 0 && !pair && !split) ? 1 : 0;
+  // ---- MMA warpgroups: the accumulators of a thread (npl * BN / H fp32 registers) must stay <= 128
+  int H = (epi_override == 2 && plan->BN >= 64 && !pdlf) ? 2 : 1;
+  if (npl * plan->BN > 128 && !pdlf) H = 2;
+  while (npl * plan->BN / H > 128 && plan->BN > std::max(bn_min, pair ? 64 : 32)) plan->BN /= 2;
+  YB_REQUIRE(npl * plan->BN / H <= 128, "tc_conv: accumulator tile exceeds the register budget");
+  plan->epi_groups = H;
+  plan->pdl_friendly = pdlf;
   const int BN = plan->BN;
   q.bn = BN;
   plan->pair = pair;
   q.pair = pair;
   q.nb = Bv;
-  const int stage_bytes = npl * (A_STAGE_BYTES + (pair ? BN / 2 : BN) * BLOCK_K * 2);
+  const int stage_bytes = npl * (A_STAGE_BYTES + BN * BLOCK_K * 2);   // a pair CTA receives the whole weight tile too
   // ---- persistent grid + shared-memory layout: [pipeline stages][2 x 16 KB out tiles][2 x 16 KB residual tiles]
   q.m_tiles = (int)m_tiles;
   q.n_tiles = ceil_div(p.Cout, BN);
   const int num_tiles = (pair ? (q.m_tiles + 1) / 2 : q.m_tiles) * q.n_tiles;   // work units (pairs of M tiles when paired)
-  int grid = std::min(num_tiles, grid_override > 0 ? (pair ? std::max(1, grid_override / 2) : grid_override) : (pair ? 74 : 148));
-  if (pair) grid = std::min(grid, 74);   // one cluster per TPC: 148 SMs = 74 CTA pairs, one CTA per SM
+  const int max_grid = pair ? sms / 2 : sms;
+  int grid = std::min(num_tiles, grid_override > 0 ? (pair ? std::max(1, grid_override / 2) : grid_override) : max_grid);
+  if (pair) grid = std::min(grid, max_grid);
   // stream-K: one share of the k-block iterations per SM (cluster), whatever the unit count -- worth it only when the
   // units do not fill whole waves; needs the staged (TMA) epilogue and co-resident CTAs (<= one per SM)
   const long long total_it = (long long)num_tiles * q.ntaps * q.kchunks;
   int sk = (sk_override > 0 && q.epi_tma && !(pdl_override > 0)) ? 1 : 0;
   if (sk) {
-    const int gsk = std::min<long long>(grid_override > 0 ? grid : (pair ? 74 : 148), total_it);
+    const int gsk = std::min<long long>(grid_override > 0 ? grid : max_grid, total_it);
     if (gsk <= 1 || num_tiles % gsk == 0) sk = 0;   // whole waves already: nothing to balance
     else grid = gsk;
   }
   plan->sk = sk;
-  q.acc_stages = (grid < num_tiles || sk) ? 2 : 1;
-  if (q.acc_stages * npl * BN > 512) q.acc_stages = 1;   // split: two accumulators per tile (2 * BN columns)
-  int tmem_cols = 32;
-  while (tmem_cols < q.acc_stages * npl * BN) tmem_cols *= 2;
-  // Pairs allocate all of TMEM (and > half of the shared memory, below): one CTA per SM, so both CTAs of a pair
-  // get the SAME accumulator address, which the single cta_group::2 MMA requires.
-  if (pair) tmem_cols = 512;
-  q.tmem_cols = tmem_cols;
   const int tiles_per_cta = sk ? 2 : ceil_div(num_tiles, grid);
-  // two epilogue groups (8 warps) work on two 64-channel chunks at once; pointless for a single-chunk tile
-  // PDL-friendly plan: <= ~108 KB of shared memory, one epilogue group (192 threads x 122 registers) and <= 256 TMEM
-  // columns, so a CTA of the NEXT layer can become resident beside it and overlap its prologue + first weight tiles
-  const int pdlf = (pdl_override > 0 && !pair && !split) ? 1 : 0;
-  plan->pdl_friendly = pdlf;
-  if (pdlf && q.acc_stages * BN > 256) q.acc_stages = 1;
-  if (pdlf) {   // (never a split plan)
-    int tc = 32;
-    while (tc < q.acc_stages * BN) tc *= 2;
-    q.tmem_cols = tc;
-  }
-  plan->epi_groups = (epi_req == 2 && !pdlf) ? 2 : 1;
-  // staging: 2 x 16 KB tiles (one per group when there are two); the direct (fp32) epilogue needs a padded
-  // 32x33 float transpose buffer per epilogue warp
-  // (split: one buffer of two tiles per group)
-  const int epi_tiles = split ? 2 * plan->epi_groups : 2;
-  const int out_bytes = std::max(epi_tiles * A_STAGE_BYTES, plan->epi_groups == 2 ? 36 * 1024 : 2 * A_STAGE_BYTES);
-  q.res_direct = ((split || chain_override > 0) && plan->epi_groups == 2 && p.residual && flat && q.epi_tma) ? 1 : 0;
-  const int res_bytes = (q.epi_tma && p.residual && !q.res_direct) ? epi_tiles * A_STAGE_BYTES : 0;
-  int stages = std::min(MAX_STAGES, ((pdlf ? 108 : (split ? 221 : 200)) * 1024 - out_bytes - res_bytes) / stage_bytes);
+  // staging: 2 x 16 KB (two fp16 buffers, or one buffer of a hi and a lo tile); the direct (fp32) epilogue stores
+  // straight from the accumulator registers
+  const int out_bytes = q.epi_tma ? 2 * A_STAGE_BYTES : 0;
+  q.res_direct = ((split || chain_override > 0) && H == 2 && p.residual && flat && q.epi_tma) ? 1 : 0;
+  const int res_bytes = (q.epi_tma && p.residual && !q.res_direct) ? 2 * A_STAGE_BYTES : 0;
+  int stages = std::min(MAX_STAGES, ((pdlf ? 108 : 225) * 1024 - out_bytes - res_bytes) / stage_bytes);
   if (stages < 1 && pdlf) {   // does not fit in half an SM: an ordinary plan
     plan->pdl_friendly = 0;
-    stages = std::min(MAX_STAGES, (200 * 1024 - out_bytes - res_bytes) / stage_bytes);
+    stages = std::min(MAX_STAGES, (225 * 1024 - out_bytes - res_bytes) / stage_bytes);
   }
   YB_REQUIRE(stages >= 1, "tc_conv: tile does not fit in shared memory");
   if (stages_override > 0) stages = std::min(stages, stages_override);
@@ -1579,12 +1279,7 @@ TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, in
   plan->smem_bytes = (size_t)q.res_off + res_bytes + 1024;
   if (plan->pdl_friendly && plan->smem_bytes > (size_t)112 * 1024) plan->pdl_friendly = 0;   // does not fit twice: plain plan
   q.pdl = plan->pdl_friendly;
-  if (pair) plan->smem_bytes = std::max(plan->smem_bytes, (size_t)120 * 1024);   // at most one pair CTA per SM
   plan->grid = dim3((unsigned)(pair ? 2 * grid : grid), 1, 1);
-
-  // ---- instruction descriptor (cute::UMMA::InstrDescriptor): D=f32, A=B=f16, K-major, N, M=128 (256 for a CTA pair)
-  q.idesc = (1u << 4) | (0u << 7) | (0u << 10) | (0u << 15) | (0u << 16) | ((uint32_t)(BN >> 3) << 17) |
-            ((uint32_t)((pair ? 2 * BLOCK_M : BLOCK_M) >> 4) << 24);
 
   // ---- A tensor maps
   const __half* x = reinterpret_cast<const __half*>(p.x);
@@ -1657,12 +1352,10 @@ TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, in
   if (q.epi_tma) {
     // output / residual tile maps: same geometry as the accumulator tile, 64-channel boxes
     uint32_t box[4] = {(uint32_t)BLOCK_K, (uint32_t)q.tw, (uint32_t)q.th, 1};
-    uint32_t box32[4] = {32u, (uint32_t)q.tw, (uint32_t)q.th, 1};
     if (flat) {
       uint64_t dims[4] = {CoutP, (uint64_t)Wov, 1, 1};
       uint64_t ystr[3] = {(uint64_t)p.y_pix_stride * 2, (uint64_t)Wov * p.y_pix_stride * 2, (uint64_t)Wov * p.y_pix_stride * 2};
       encode_map_f16(&q.tmY, p.y, 4, dims, ystr, box);
-      encode_map_f16(&q.tmY32, p.y, 4, dims, ystr, box32, 64);
       if (p.residual) {
         uint64_t rstr[3] = {CoutP * 2, (uint64_t)Wov * CoutP * 2, (uint64_t)Wov * CoutP * 2};
         encode_map_f16(&q.tmR, p.residual, 4, dims, rstr, box);
@@ -1671,7 +1364,6 @@ TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, in
       uint64_t dims[4] = {CoutP, (uint64_t)p.Wo, (uint64_t)p.Ho, (uint64_t)p.B};
       uint64_t ystr[3] = {(uint64_t)p.y_pix_stride * 2, (uint64_t)p.Wo * p.y_pix_stride * 2, (uint64_t)p.y_batch_stride * 2};
       encode_map_f16(&q.tmY, p.y, 4, dims, ystr, box);
-      encode_map_f16(&q.tmY32, p.y, 4, dims, ystr, box32, 64);
       if (p.residual) {
         uint64_t rstr[3] = {CoutP * 2, (uint64_t)p.Wo * CoutP * 2, (uint64_t)p.Ho * p.Wo * CoutP * 2};
         encode_map_f16(&q.tmR, p.residual, 4, dims, rstr, box);
@@ -1690,13 +1382,14 @@ int tc_conv_plan_pair(const TcConvPlan* plan) { return plan->pair; }
 int tc_conv_plan_epi_groups(const TcConvPlan* plan) { return plan->epi_groups; }
 int tc_conv_plan_pdl_friendly(const TcConvPlan* plan) { return plan->pdl_friendly; }
 int tc_conv_plan_sk(const TcConvPlan* plan) { return plan->sk; }
-size_t tc_conv_sk_workspace_bytes() { return (size_t)148 * BLOCK_M * 256 * sizeof(float) + 148 * 2 * sizeof(int); }
-// ws: tc_conv_sk_workspace_bytes() of device memory whose LAST 148 * 2 ints (the flags) are zero; kernels that share a
+// one slot per SM of the current device (a stream-K grid has at most one CTA per SM)
+size_t tc_conv_sk_workspace_bytes() { return (size_t)device_sms() * BLOCK_M * 256 * sizeof(float) + device_sms() * 2 * sizeof(int); }
+// ws: tc_conv_sk_workspace_bytes() of device memory whose LAST device_sms() * 2 ints (the flags) are zero; kernels that share a
 // workspace must be stream-ordered (each launch leaves the flags zero again)
 void tc_conv_plan_set_sk_workspace(TcConvPlan* plan, void* ws) {
   plan->prm.sk = (plan->sk && ws) ? 1 : 0;
   plan->prm.sk_ws = reinterpret_cast<float*>(ws);
-  plan->prm.sk_flags = reinterpret_cast<int*>(reinterpret_cast<char*>(ws) + (size_t)148 * BLOCK_M * 256 * sizeof(float));
+  plan->prm.sk_flags = reinterpret_cast<int*>(reinterpret_cast<char*>(ws) + (size_t)device_sms() * BLOCK_M * 256 * sizeof(float));
 }
 
 template <int BN, bool PAIR, int H, bool SPLIT>
@@ -1704,8 +1397,8 @@ static void launch_bn(const TcConvPlan* plan, cudaStream_t stream) {
   static PerDeviceOnce attr;
   if (attr.first())
     YB_CHECK_CUDA(cudaFuncSetAttribute(tc_conv_kernel<BN, PAIR, H, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)(224 * 1024)));
-  constexpr int THREADS = 64 + 128 * H;
+                                       (int)(226 * 1024)));
+  constexpr int THREADS = 128 * (1 + H);
   if (plan->prm.pdl || PAIR) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = plan->grid;
@@ -1733,12 +1426,17 @@ static void launch_bn(const TcConvPlan* plan, cudaStream_t stream) {
   }
 }
 
+// the (BN, warpgroups) combinations whose accumulators fit in 128 registers per thread (the plan never picks others)
 template <int BN, bool PAIR, bool SPLIT>
 static void launch_h(const TcConvPlan* plan, cudaStream_t stream) {
-  if (plan->epi_groups == 2)
-    launch_bn<BN, PAIR, (BN >= 64 ? 2 : 1), SPLIT>(plan, stream);
-  else
-    launch_bn<BN, PAIR, 1, SPLIT>(plan, stream);
+  constexpr int NPL = SPLIT ? 2 : 1;
+  if (plan->epi_groups == 2) {
+    if constexpr (NPL * BN / 2 <= 128) launch_bn<BN, PAIR, 2, SPLIT>(plan, stream);
+    else YB_REQUIRE(false, "tc_conv: N tile too wide for two MMA warpgroups");
+  } else {
+    if constexpr (NPL * BN <= 128) launch_bn<BN, PAIR, 1, SPLIT>(plan, stream);
+    else YB_REQUIRE(false, "tc_conv: N tile too wide for one MMA warpgroup");
+  }
 }
 
 template <bool SPLIT>
@@ -1766,7 +1464,6 @@ static void launch_s(const TcConvPlan* plan, cudaStream_t stream) {
 // ---------------------------------------------------------------------------------------------
 struct TcChain {
   int nl = 0, split = 0, grid = 0, n_done = 0;
-  int groups = 2;   // epilogue groups per CTA (2: three split stages, 4: two)
   size_t smem_bytes = 0;
   TcParams* d_layers = nullptr;
   ChainLayer* d_info = nullptr;
@@ -1774,8 +1471,8 @@ struct TcChain {
   long long* d_stats = nullptr;   // diagnostics (YB_CHAIN_STATS=1)
 };
 
-// a plan the chain kernel can run: its one tile shape (BN = 128, two epilogue groups, staged epilogue, two accumulator
-// buffers) and nothing the chain does not implement (pairs, stream-K, staged residual, partial N tiles)
+// a plan the chain kernel can run: its tile shape (BN = 128 or 64, two MMA warpgroups, staged epilogue) and nothing the
+// chain does not implement (pairs, stream-K, staged residual, partial N tiles)
 bool tc_conv_plan_chainable(const TcConvPlan* pl) {
   const TcParams& q = pl->prm;
   return (pl->BN == 128 || pl->BN == 64) && !pl->pair && pl->epi_groups == 2 && !pl->sk && !pl->pdl_friendly && q.epi_tma &&
@@ -1784,9 +1481,7 @@ bool tc_conv_plan_chainable(const TcConvPlan* pl) {
 
 // dep_a[i] / dep_r[i]: index (< i) of the plan that writes plan i's input / residual, -1 for a tensor that is complete
 // before the launch (or, for the residual, one whose completion the input dependency already implies)
-TcChain* tc_chain_create(const std::vector<const TcConvPlan*>& plans, const std::vector<int>& dep_a, const std::vector<int>& dep_r,
-                         int groups) {
-  YB_REQUIRE(groups == 2 || groups == 4, "tc_chain: 2 or 4 epilogue groups");
+TcChain* tc_chain_create(const std::vector<const TcConvPlan*>& plans, const std::vector<int>& dep_a, const std::vector<int>& dep_r) {
   YB_REQUIRE(!plans.empty() && plans.size() == dep_a.size() && plans.size() == dep_r.size(), "tc_chain: empty chain");
   const TcConvPlan* p0 = plans[0];
   std::vector<TcParams> lp;
@@ -1812,7 +1507,7 @@ TcChain* tc_chain_create(const std::vector<const TcConvPlan*>& plans, const std:
     c.tiles_x = pl->prm.tiles_x;
     c.tiles_y = pl->prm.tiles_y;
     c.done_off = done_off;
-    c.target = groups * pl->prm.n_tiles;
+    c.target = pl->prm.n_tiles;   // each (M tile, N tile) adds 1 once its stores have completed
     c.dep_a = dep_a[i];
     c.dep_r = dep_r[i];
     c.stride = pl->stride;
@@ -1826,16 +1521,13 @@ TcChain* tc_chain_create(const std::vector<const TcConvPlan*>& plans, const std:
   auto* ch = new TcChain();
   ch->nl = (int)plans.size();
   ch->split = p0->split;
-  ch->groups = groups;
   ch->n_done = done_off;
   {
     const int npl = p0->split ? 2 : 1;
-    ch->smem_bytes = (size_t)chain_stages(p0->split != 0, groups) * npl * (A_STAGE_BYTES + 128 * BLOCK_K * 2) +
-                     (size_t)groups * npl * CHUNK32_BYTES + 1024;
+    ch->smem_bytes = (size_t)chain_stages(p0->split != 0) * npl * (A_STAGE_BYTES + 128 * BLOCK_K * 2) +
+                     (size_t)(p0->split ? 1 : 2) * npl * A_STAGE_BYTES + 1024;
   }
-  int dev = 0, sms = 148;
-  YB_CHECK_CUDA(cudaGetDevice(&dev));
-  YB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int sms = device_sms();
   ch->grid = std::min(sms, ubase);   // one CTA per SM (the shared memory of a CTA sees to that): all co-resident
   try {
     YB_CHECK_CUDA(cudaMalloc(&ch->d_layers, lp.size() * sizeof(TcParams)));
@@ -1858,19 +1550,18 @@ void tc_chain_destroy(TcChain* ch) {
   delete ch;
 }
 int tc_chain_layers(const TcChain* ch) { return ch->nl; }
-int tc_chain_groups(const TcChain* ch) { return ch->groups; }
 
-template <bool SPLIT, int H>
+template <bool SPLIT>
 static void launch_chain_t(const TcChain* ch, cudaStream_t stream) {
   static PerDeviceOnce attr;
   if (attr.first())
-    YB_CHECK_CUDA(cudaFuncSetAttribute(tc_chain_kernel<SPLIT, H>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)ch->smem_bytes));   // (one size per <SPLIT, H>)
+    YB_CHECK_CUDA(cudaFuncSetAttribute(tc_chain_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)ch->smem_bytes));   // (one size per precision mode)
   // Cooperative launch: the grid starts only when ALL its CTAs can be resident at once.  The tile dependencies make CTAs
   // wait for each other, so a partially scheduled grid (two chains from different streams sharing the SMs) could deadlock.
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)ch->grid);
-  cfg.blockDim = dim3(64 + 128 * H);
+  cfg.blockDim = dim3(384);
   cfg.dynamicSmemBytes = ch->smem_bytes;
   cfg.stream = stream;
   cudaLaunchAttribute at[1];
@@ -1878,7 +1569,7 @@ static void launch_chain_t(const TcChain* ch, cudaStream_t stream) {
   at[0].val.cooperative = 1;
   cfg.attrs = at;
   cfg.numAttrs = 1;
-  YB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, tc_chain_kernel<SPLIT, H>, (const TcParams*)ch->d_layers, (const ChainLayer*)ch->d_info,
+  YB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, tc_chain_kernel<SPLIT>, (const TcParams*)ch->d_layers, (const ChainLayer*)ch->d_info,
                                    ch->nl, ch->d_done, ch->d_stats));
 }
 
@@ -1902,10 +1593,8 @@ void tc_chain_print_stats(TcChain* ch, const char* name) {
   const double tot = avg[6] > 0 ? avg[6] : 1.0;
   fprintf(stderr,
           "[yolact_b200] chain stats %s: kernel %.0f kcyc/CTA; share of it spent waiting (avg over CTAs / max): producer deps %.1f%% / %.1f%%, "
-          "producer ring slot %.1f%%, MMA operands %.1f%% / %.1f%%, MMA accumulator %.1f%%, epilogue accumulator %.1f%% / %.1f%%, epilogue store "
-          "completion %.1f%%\n",
-          name, tot / 1e3, 100 * avg[0] / tot, 100 * mx[0] / tot, 100 * avg[1] / tot, 100 * avg[2] / tot, 100 * mx[2] / tot, 100 * avg[3] / tot,
-          100 * avg[4] / tot, 100 * mx[4] / tot, 100 * avg[5] / tot);
+          "producer ring slot %.1f%%, store completion before a signal %.1f%% / %.1f%%\n",
+          name, tot / 1e3, 100 * avg[0] / tot, 100 * mx[0] / tot, 100 * avg[1] / tot, 100 * avg[4] / tot, 100 * mx[4] / tot);
 }
 
 // Can a chain launch be captured into a CUDA graph and replayed on this driver?  (One trial per process.)
@@ -1935,11 +1624,7 @@ bool tc_chain_graph_ok(const TcChain* ch) {
 }
 void launch_tc_chain(const TcChain* ch, cudaStream_t stream, LaunchCounter* lc) {
   YB_CHECK_CUDA(cudaMemsetAsync(ch->d_done, 0, (size_t)ch->n_done * sizeof(int), stream));   // (a memset node in the captured graph)
-  if (ch->split) {
-    if (ch->groups == 4) launch_chain_t<true, 4>(ch, stream); else launch_chain_t<true, 2>(ch, stream);
-  } else {
-    if (ch->groups == 4) launch_chain_t<false, 4>(ch, stream); else launch_chain_t<false, 2>(ch, stream);
-  }
+  if (ch->split) launch_chain_t<true>(ch, stream); else launch_chain_t<false>(ch, stream);
   YB_CHECK_LAUNCH();
   if (lc) lc->n++;
 }

@@ -36,7 +36,7 @@ def _handle(device, precision):
 
 def dcn_v2_conv(input, offset, mask, weight, bias, stride, padding, dilation, deformable_groups, precision="f32"):
     if not input.is_cuda:
-        raise _lib.YbError("yolact_b200.dcn_v2 runs on CUDA (B200) only (the reference's CPU path is an AT_ERROR stub too)")
+        raise _lib.YbError("yolact_b200.dcn_v2 runs on CUDA (H100) only (the reference's CPU path is an AT_ERROR stub too)")
     lib = _lib.load()
     sh, sw = _pair(stride)
     ph, pw = _pair(padding)

@@ -37,7 +37,7 @@ class Detect(object):
 
     def _handle(self, device):
         if device.type != "cuda":
-            raise _lib.YbError("yolact_b200.Detect runs on CUDA (B200) only; there is no CPU path.")
+            raise _lib.YbError("yolact_b200.Detect runs on CUDA (H100) only; there is no CPU path.")
         idx = device.index if device.index is not None else torch.cuda.current_device()
         key = (idx, self.top_k, self.conf_thresh, self.nms_thresh, self.max_num_detections, self.num_classes,
                self.mask_dim, self.max_size)

@@ -27,7 +27,7 @@ from .output_utils import _FORMATS, _ops_handle, postprocess
 
 def _require_cuda(t, what):
     if not t.is_cuda:
-        raise _lib.YbError("yolact_b200.%s runs on CUDA (B200) only; there is no CPU path." % what)
+        raise _lib.YbError("yolact_b200.%s runs on CUDA (H100) only; there is no CPU path." % what)
 
 
 def pack_masks(masks):

@@ -54,7 +54,7 @@ def assemble_masks(proto, coef, boxes, h, w, crop_masks=True, mask_format="f32",
     """Low-level: proto [ph,pw,k], coef [n,k], boxes [n,4] relative -> (masks, boxes_px int64 [n,4],
     proto_masks [n,ph,pw] or None).  No host sync."""
     if not proto.is_cuda:
-        raise _lib.YbError("yolact_b200.postprocess runs on CUDA (B200) only; there is no CPU path.")
+        raise _lib.YbError("yolact_b200.postprocess runs on CUDA (H100) only; there is no CPU path.")
     lib = _lib.load()
     dev = proto.device
     n = int(coef.shape[0])
@@ -85,7 +85,7 @@ def assemble_masks_batch(proto, coef, boxes, h, w, crop_masks=True, mask_format=
     """Whole batch in one launch: proto [B,ph,pw,k], coef [B,n,k], boxes [B,n,4] (padded rows, e.g.
     Yolact.infer_padded's outputs) -> (masks [B,n,...], boxes_px int64 [B,n,4]).  No host sync."""
     if not proto.is_cuda:
-        raise _lib.YbError("yolact_b200.postprocess runs on CUDA (B200) only; there is no CPU path.")
+        raise _lib.YbError("yolact_b200.postprocess runs on CUDA (H100) only; there is no CPU path.")
     lib = _lib.load()
     dev = proto.device
     B, ph, pw, k = (int(s) for s in proto.shape)

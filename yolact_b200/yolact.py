@@ -9,7 +9,7 @@ eval.py assigns (eval.py:871-872); `.maskiou_net` exists for YOLACT++ configs.
 
 Everything numerical happens in libyolact_b200.so through the C ABI (include/yolact_b200.h); the
 nn.Module tree below only HOLDS parameters under the reference's names -- its layers are never
-called.  There is no PyTorch/CPU fallback: without the CUDA library on a B200 forward() raises.
+called.  There is no PyTorch/CPU fallback: without the CUDA library on an H100 forward() raises.
 """
 import ctypes
 
@@ -186,9 +186,9 @@ def make_yb_config(c, precision):
 
 class Yolact(nn.Module):
     """See the module docstring.  `precision` (yb_precision in include/yolact_b200.h):
-      'f16x3' (default) split-precision tcgen05 -- fp16 hi+lo operand pairs, three MMA passes, fp32-equivalent results
+      'f16x3' (default) split-precision tensor-core -- fp16 hi+lo operand pairs, three MMA passes, fp32-equivalent results
               (boxes / scores / masks within 1e-3 of the fp32 reference, identical class ids);
-      'f16tc' single-pass fp16 tcgen05 -- ~2x faster conv stack, head tensors within ~2e-3 of range;
+      'f16tc' single-pass fp16 tensor-core -- faster conv stack, head tensors within ~2e-3 of range;
       'f32'   fp32 on CUDA cores (slow second opinion)."""
 
     def __init__(self, cfg=None, precision="f16x3"):
@@ -261,7 +261,7 @@ class Yolact(nn.Module):
 
     def _handle_for(self, device):
         if device.type != "cuda":
-            raise _lib.YbError("yolact_b200 runs on CUDA (B200) only; got a tensor on %s. There is no CPU path." % device)
+            raise _lib.YbError("yolact_b200 runs on CUDA (H100) only; got a tensor on %s. There is no CPU path." % device)
         idx = device.index if device.index is not None else torch.cuda.current_device()
         lib = _lib.load()
         if idx not in self._handles:
@@ -429,5 +429,5 @@ class Yolact(nn.Module):
         if x.dim() != 4 or x.shape[1] != 3:
             raise ValueError("Yolact.forward expects [B,3,H,W], got %s" % (tuple(x.shape),))
         if not x.is_cuda:
-            raise _lib.YbError("yolact_b200 runs on CUDA (B200) only; input is on %s. There is no CPU path." % x.device)
+            raise _lib.YbError("yolact_b200 runs on CUDA (H100) only; input is on %s. There is no CPU path." % x.device)
         return x.contiguous().float()
