@@ -31,10 +31,11 @@ def test_dcn_zero_offset_identity():
     assert (2 * y - x).abs().max() < 1e-6
 
 
+@pytest.mark.parametrize("Co", [96, 12, 4])
 @pytest.mark.parametrize("C,stride", [(64, 1), (128, 2), (32, 1)])
-def test_dcn_f16_paths_vs_oracle(C, stride):
+def test_dcn_f16_paths_vs_oracle(C, stride, Co):
     r = np.random.RandomState(C + stride)
-    B, H, W, Co = 2, 21, 19, 96
+    B, H, W = 2, 21, 19
     x = r.standard_normal((B, C, H, W)).astype(np.float32)
     w = (r.standard_normal((Co, C, 3, 3)) * (2.0 / (9 * C)) ** 0.5).astype(np.float32)
     bias = r.standard_normal(Co).astype(np.float32) * 0.1
@@ -44,15 +45,18 @@ def test_dcn_f16_paths_vs_oracle(C, stride):
     ref = O.dcn_v2_forward(x, off, msk, w, bias, stride, 1, 1)
     t = lambda a: torch.from_numpy(a).cuda()
     y = dcn_v2_conv(t(x), t(off), t(msk), t(w), t(bias), stride, 1, 1, 1, precision="f16tc").cpu().numpy()
-    # C % 64 == 0 -> gather + tensor-core contraction; else the fused SIMT fp16 kernel.  fp16 operands.
+    # C % 64 == 0 -> the fused tensor-core kernel (Co = 12 / 4 run with zero-padded output channels up to a multiple
+    # of 8); else the fused SIMT fp16 kernel.  fp16 operands.
     assert np.abs(y - ref).max() < 1e-2 * max(1.0, np.abs(ref).max())
 
 
+@pytest.mark.parametrize("Co", [96, 12, 4])
 @pytest.mark.parametrize("C,stride", [(64, 1), (128, 2)])
-def test_dcn_split_precision_vs_oracle(C, stride):
-    """YB_PREC_F16X3: gather of hi+lo samples -> split columns -> three-pass tensor-core contraction; fp32-equivalent."""
+def test_dcn_split_precision_vs_oracle(C, stride, Co):
+    """YB_PREC_F16X3: hi+lo samples gathered into the fused tensor-core kernel's split A stage -> three-pass contraction;
+    fp32-equivalent.  Co = 12 / 4 run with zero-padded output channels up to a multiple of 8."""
     r = np.random.RandomState(7 * C + stride)
-    B, H, W, Co = 2, 21, 19, 96
+    B, H, W = 2, 21, 19
     x = r.standard_normal((B, C, H, W)).astype(np.float32)
     w = (r.standard_normal((Co, C, 3, 3)) * (2.0 / (9 * C)) ** 0.5).astype(np.float32)
     bias = r.standard_normal(Co).astype(np.float32) * 0.1

@@ -52,7 +52,7 @@ __global__ void pack_w_simt_kernel(const float* __restrict__ w, T* __restrict__ 
     out[((int64_t)t * Ci + c) * Co + o] = from_f32<T>(w[i]);
   }
 }
-// OIHW fp32 (device) -> [Cout][tap*Cin + c] half (DCN contraction as a 1x1 conv over gathered columns)
+// OIHW fp32 (device) -> [Cout][tap*Cin + c] half (the fused DCN kernel's weights)
 __global__ void pack_w_dcn_tc_kernel(const float* __restrict__ w, __half* __restrict__ out, int Co, int Ci, int taps) {
   const int64_t total = (int64_t)Co * Ci * taps;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -182,20 +182,11 @@ int yb_create(const yb_config* cfg, int device, yb_handle** out) {
   h->device = device;
   h->ops_only = (cfg->backbone == YB_BACKBONE_NONE);
   // defaults: programmatic dependent launch in the single-pass fp16 mode, stream-K candidates in the split mode (whose
-  // plans fill the SM, so nothing can become resident early).  Not measured on the H100; YB_PDL / YB_SK switch them.
+  // plans fill the SM, so nothing can become resident early).  Not measured on the H100; YB_SK switches stream-K.
   h->pdl = (cfg->precision == YB_PREC_F16TC);
   h->sk_candidates = (cfg->precision == YB_PREC_F16X3);
-  if (const char* at = getenv("YB_AUTOTUNE")) h->autotune = (atoi(at) != 0);
-  if (const char* pc = getenv("YB_PAIR")) h->pair_candidates = (atoi(pc) != 0);
-  if (const char* ec = getenv("YB_EPI2")) h->epi2_candidates = (atoi(ec) != 0);
   if (const char* sk = getenv("YB_SK")) h->sk_candidates = (atoi(sk) != 0);
   if (const char* ch = getenv("YB_CHAIN")) h->chain_mode = std::min(2, std::max(0, atoi(ch)));
-  if (const char* sw = getenv("YB_STEM_WG")) h->stem_wg = (atoi(sw) == 2 || atoi(sw) == 4) ? atoi(sw) : 1;   // default 0: per precision mode
-  if (const char* st = getenv("YB_STEM_TC")) h->stem_on_tc = (atoi(st) != 0);
-  if (const char* df = getenv("YB_DCN_FUSED")) h->dcn_fused = (atoi(df) != 0);
-  if (const char* pd = getenv("YB_PDL")) h->pdl = (atoi(pd) != 0);
-  if (const char* fh = getenv("YB_FUSE_HEADS")) h->fuse_heads = (atoi(fh) != 0);
-  if (const char* br = getenv("YB_BRANCHES")) h->multi_stream = (atoi(br) != 0);
   if (!h->ops_only) {
     YB_REQUIRE(cfg->backbone == YB_BACKBONE_RESNET || cfg->backbone == YB_BACKBONE_DARKNET, "unknown backbone");
     YB_REQUIRE(cfg->num_stages >= 4 && cfg->num_stages <= 5, "num_stages must be 4 or 5");
@@ -581,12 +572,24 @@ int yb_dcn_forward(yb_handle* h, const float* d_input, const float* d_weight, co
                            &h->lc);
     launch_nhwc_to_nchw_f32<float>(y, d_output, B, Ho, Wo, Co, s, &h->lc);
   } else {
+    // the fused tensor-core kernel needs Cout % 8 == 0 and Cout >= 8: a narrower layer runs with zero weight rows and
+    // zero bias up to Cp output channels, of which the first Co are copied out
+    const int Cp = (C % 64 == 0) ? std::max(8, (Co + 7) / 8 * 8) : Co;
     __half* x = (__half*)tp.get((size_t)B * H * W * C * 2 * npl);
-    __half* y = (__half*)tp.get((size_t)B * Ho * Wo * Co * 2 * npl);
+    __half* y = (__half*)tp.get((size_t)B * Ho * Wo * Cp * 2 * npl);
     launch_nchw_f32_to_nhwc<__half>(d_input, x, B, C, H, W, s, &h->lc, sp);
     if (C % 64 == 0) {
-      __half* cols = (__half*)tp.get((size_t)B * Ho * Wo * 9 * C * 2 * npl);
-      __half* wk = (__half*)tp.get((size_t)wn * 2 * npl);
+      __half* wk = (__half*)tp.get((size_t)Cp * C * 9 * 2 * npl);
+      const float* bias = d_bias;
+      if (Cp > Co) {
+        YB_CHECK_CUDA(cudaMemsetAsync(wk, 0, (size_t)Cp * C * 9 * 2 * npl, s));
+        if (d_bias) {
+          float* bp = (float*)tp.get((size_t)Cp * 4);
+          YB_CHECK_CUDA(cudaMemsetAsync(bp, 0, (size_t)Cp * 4, s));
+          YB_CHECK_CUDA(cudaMemcpyAsync(bp, d_bias, (size_t)Co * 4, cudaMemcpyDeviceToDevice, s));
+          bias = bp;
+        }
+      }
       float out_scale = 1.f;
       if (sp) {
         // one power of two for the whole weight tensor: max |w| is read back (op-level hook, not the hot path)
@@ -604,44 +607,15 @@ int yb_dcn_forward(yb_handle* h, const float* d_input, const float* d_weight, co
         pack_w_dcn_tc_kernel<<<grid1d(wn), 256, 0, s>>>(d_weight, wk, Co, C, 9);
       }
       YB_CHECK_LAUNCH();
-      if (h->dcn_fused && dcn_tc_supported(C, Co)) {
-        DcnTcPlan* dp = dcn_tc_plan_create(x, om, wk, d_bias, y, B, H, W, C, Ho, Wo, Co, stride_h, pad_h, dilation_h,
-                                           ACT_NONE, 0, sp, out_scale);
-        try {
-          launch_dcn_tc(dp, s, &h->lc);
-        } catch (...) {
-          dcn_tc_plan_destroy(dp);
-          throw;
-        }
-        dcn_tc_plan_destroy(dp);
-        launch_nhwc_to_nchw_f32<__half>(y, d_output, B, Ho, Wo, Co, s, &h->lc, sp);
-        YB_CHECK_CUDA(cudaStreamSynchronize(s));
-        return YB_OK;
-      }
-      launch_dcn_gather_f16(x, om, cols, B, H, W, C, Ho, Wo, stride_h, pad_h, dilation_h, 0, s, &h->lc, sp);
-      ConvProblem p;
-      p.B = B;
-      p.H = Ho;
-      p.W = Wo;
-      p.Cin = 9 * C;
-      p.Ho = Ho;
-      p.Wo = Wo;
-      p.Cout = Co;
-      p.x = cols;
-      p.y = y;
-      p.split = sp;
-      p.out_scale = out_scale;
-      p.y_pix_stride = Co * npl;
-      p.y_batch_stride = (int64_t)Ho * Wo * p.y_pix_stride;
-      p.bias = d_bias;
-      TcConvPlan* plan = tc_conv_plan_create(p, wk);
+      DcnTcPlan* dp = dcn_tc_plan_create(x, om, wk, bias, y, B, H, W, C, Ho, Wo, Cp, stride_h, pad_h, dilation_h,
+                                         ACT_NONE, 0, sp, out_scale);
       try {
-        launch_tc_conv(plan, s, &h->lc);
+        launch_dcn_tc(dp, s, &h->lc);
       } catch (...) {
-        tc_conv_plan_destroy(plan);
+        dcn_tc_plan_destroy(dp);
         throw;
       }
-      tc_conv_plan_destroy(plan);
+      dcn_tc_plan_destroy(dp);
     } else {
       __half* wk = (__half*)tp.get((size_t)wn * 2);
       pack_w_simt_kernel<__half><<<grid1d(wn), 256, 0, s>>>(d_weight, wk, Co, C, 9);
@@ -649,7 +623,14 @@ int yb_dcn_forward(yb_handle* h, const float* d_input, const float* d_weight, co
       launch_dcn_simt<__half>(x, om, wk, d_bias, y, B, H, W, C, Ho, Wo, Co, stride_h, pad_h, dilation_h, ACT_NONE, 0,
                               s, &h->lc);
     }
-    launch_nhwc_to_nchw_f32<__half>(y, d_output, B, Ho, Wo, Co, s, &h->lc, sp);
+    if (Cp == Co) {
+      launch_nhwc_to_nchw_f32<__half>(y, d_output, B, Ho, Wo, Co, s, &h->lc, sp);
+    } else {
+      float* yp = (float*)tp.get((size_t)B * Cp * Ho * Wo * 4);
+      launch_nhwc_to_nchw_f32<__half>(y, yp, B, Ho, Wo, Cp, s, &h->lc, sp);
+      const size_t plane = (size_t)Ho * Wo * 4;   // bytes of one output channel
+      YB_CHECK_CUDA(cudaMemcpy2DAsync(d_output, Co * plane, yp, Cp * plane, Co * plane, B, cudaMemcpyDeviceToDevice, s));
+    }
   }
   YB_CHECK_CUDA(cudaStreamSynchronize(s));  // temporaries are freed on return
   YB_API_END
@@ -737,16 +718,20 @@ int yb_conv2d(yb_handle* h, const float* d_x, const float* h_w, const float* h_b
     __half* wd = (__half*)tp.get(pk.size() * 2);
     YB_CHECK_CUDA(cudaMemcpy(wd, pk.data(), pk.size() * 2, cudaMemcpyHostToDevice));
     {
-      const char* be = getenv("YB_CONV2D_BN");
-      const char* ge = getenv("YB_CONV2D_GRID");
-      const char* pe = getenv("YB_CONV2D_PAIR");
-      const char* ee = getenv("YB_CONV2D_EPI");
-      const char* de = getenv("YB_CONV2D_PDL");   // PDL-friendly plan + programmatic dependent launch
-      const char* ke = getenv("YB_CONV2D_SK");    // stream-K
-      plan = tc_conv_plan_create(p, wd, be ? atoi(be) : 0, 0, ge ? atoi(ge) : 0, pe ? atoi(pe) : 0, ee ? atoi(ee) : 0,
-                                 de ? atoi(de) : 0, ke ? atoi(ke) : 0);
-      if (de && atoi(de)) tc_conv_plan_set_pdl(plan, 1);
-      if (tc_conv_plan_sk(plan)) {
+      auto env = [](const char* name) {
+        const char* v = getenv(name);
+        return v ? atoi(v) : 0;
+      };
+      TcTiling want;
+      want.bn = env("YB_CONV2D_BN");
+      want.grid = env("YB_CONV2D_GRID");
+      want.pair = env("YB_CONV2D_PAIR");
+      want.mma_groups = env("YB_CONV2D_EPI");
+      want.pdl_friendly = env("YB_CONV2D_PDL");   // PDL-friendly plan + programmatic dependent launch
+      want.stream_k = env("YB_CONV2D_SK");
+      plan = tc_conv_plan_create(p, wd, want);
+      if (want.pdl_friendly) tc_conv_plan_set_pdl(plan, 1);
+      if (tc_conv_plan_tiling(plan).stream_k) {
         void* ws = tp.get(tc_conv_sk_workspace_bytes());
         YB_CHECK_CUDA(cudaMemsetAsync(ws, 0, tc_conv_sk_workspace_bytes(), s));
         tc_conv_plan_set_sk_workspace(plan, ws);

@@ -10,10 +10,6 @@
 // The reference materialises col as [B, C*9, Ho*Wo] fp32 in HBM and runs two batched SGEMMs.
 //  * launch_dcn_simt: fully fused gather + contraction on CUDA cores (fp32 parity mode, and the
 //    on-device second opinion for the tensor-core path).
-//  * launch_dcn_gather_f16: gather to fp16 NHWC columns [B,Ho,Wo,9*C] (2 B/element instead of
-//    4, channel-contiguous 16-byte stores) consumed by the tensor-core kernel as a 1x1 conv, K = 9*C.
-//    Kept behind YB_DCN_FUSED=0 as the A/B partner of the fused kernel (dcn_tc.cu), which is the default: one launch,
-//    no column buffer.
 #include <stdlib.h>
 #include <string>
 #include "kernels.cuh"
@@ -162,78 +158,6 @@ dcn_simt_kernel(const T* __restrict__ x, const float* __restrict__ om, const T* 
   }
 }
 
-// one thread = (pixel, tap, 8 channels).  split: x is [hi(C) | lo(C)] per pixel (sample = hi + lo) and the columns are
-// written as [hi(9C) | lo(9C)] per output pixel (YB_PREC_F16X3).
-__global__ void dcn_gather_f16_kernel(const __half* __restrict__ x, const float* __restrict__ om,
-                                      __half* __restrict__ cols, int B, int H, int W, int C, int Ho,
-                                      int Wo, int stride, int pad, int dil, int mask_logits, int split) {
-  const int CV = C / 8;
-  const int PS = split ? 2 * C : C;
-  const int64_t total = (int64_t)B * Ho * Wo * 9 * CV;
-  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total;
-       idx += (int64_t)gridDim.x * blockDim.x) {
-    const int cv = (int)(idx % CV);
-    int64_t t = idx / CV;
-    const int tap = (int)(t % 9);
-    const int64_t m = t / 9;
-    const int wo = (int)(m % Wo);
-    const int64_t t2 = m / Wo;
-    const int ho = (int)(t2 % Ho);
-    const int b = (int)(t2 / Ho);
-    const float* pom = om + m * 27;
-    const TapGeom g = tap_geometry(pom, tap, ho, wo, H, W, stride, pad, dil);
-    const float msk = tap_mask(pom, tap, mask_logits);
-    const __half* xb = x + (size_t)b * H * W * PS + cv * 8;
-    float acc[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-    auto corner = [&](int o, float wgt) {
-      if (o < 0) return;
-      uint4 raw = *reinterpret_cast<const uint4*>(xb + (size_t)o * PS);
-      const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
-      float f8[8];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float2 f = __half22float2(h2[j]);
-        f8[2 * j] = f.x;
-        f8[2 * j + 1] = f.y;
-      }
-      if (split) {
-        uint4 rawl = *reinterpret_cast<const uint4*>(xb + (size_t)o * PS + C);
-        const __half2* l2 = reinterpret_cast<const __half2*>(&rawl);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float2 f = lo2_to_f32(l2[j]);   // lo plane: residual * 2^11
-          f8[2 * j] += f.x;
-          f8[2 * j + 1] += f.y;
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < 8; ++j) acc[j] = fmaf(wgt, f8[j], acc[j]);
-    };
-    corner(g.o00, g.w00);
-    corner(g.o01, g.w01);
-    corner(g.o10, g.w10);
-    corner(g.o11, g.w11);
-    uint4 outv, outl;
-    __half2* o2 = reinterpret_cast<__half2*>(&outv);
-    __half2* ol2 = reinterpret_cast<__half2*>(&outl);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float v0 = acc[2 * j] * msk, v1 = acc[2 * j + 1] * msk;
-      o2[j] = __halves2half2(from_f32<__half>(v0), from_f32<__half>(v1));
-      if (split) {
-        const float2 hf = __half22float2(o2[j]);
-        ol2[j] = lo2_from_f32(fabsf(v0) > 65504.f ? 0.f : v0 - hf.x, fabsf(v1) > 65504.f ? 0.f : v1 - hf.y);   // lo' = residual * 2^11
-      }
-    }
-    __half* cp = cols + (size_t)m * 9 * PS + (size_t)tap * C + cv * 8;
-    *reinterpret_cast<uint4*>(cp) = outv;
-    if (split) *reinterpret_cast<uint4*>(cp + 9 * C) = outl;
-  }
-}
-
-
 }  // namespace
 
 template <typename T>
@@ -254,17 +178,5 @@ template void launch_dcn_simt<float>(const float*, const float*, const float*, c
 template void launch_dcn_simt<__half>(const __half*, const float*, const __half*, const float*,
                                       __half*, int, int, int, int, int, int, int, int, int, int, int, int,
                                       cudaStream_t, LaunchCounter*);
-
-void launch_dcn_gather_f16(const __half* x, const float* om, __half* cols, int B, int H, int W,
-                           int C, int Ho, int Wo, int stride, int pad, int dil, int mask_logits,
-                           cudaStream_t stream, LaunchCounter* lc, int split) {
-  YB_REQUIRE(C % 8 == 0, "dcn gather: C must be a multiple of 8");
-  const int64_t total = (int64_t)B * Ho * Wo * 9 * (C / 8);
-  int64_t g = (total + 255) / 256;
-  if (g > 132 * 32) g = 132 * 32;
-  dcn_gather_f16_kernel<<<(unsigned)g, 256, 0, stream>>>(x, om, cols, B, H, W, C, Ho, Wo, stride, pad, dil, mask_logits, split);
-  YB_CHECK_LAUNCH();
-  if (lc) lc->n++;
-}
 
 }  // namespace yb

@@ -4,8 +4,7 @@
 // Reference: DCN.forward (external/DCNv2/dcn_v2.py:118-128), modulated_deformable_im2col_gpu_kernel
 // (external/DCNv2/src/cuda/dcn_v2_im2col_cuda.cu:125-195, bilinear sampler :25-54) followed by the batched SGEMM + bias
 // of dcn_v2_cuda_forward (src/cuda/dcn_v2_cuda.cu:123-163).  The reference materialises the sampled columns
-// [B, 9*C, Ho*Wo] fp32 in HBM between the two (the YB_DCN_FUSED=0 path of dcn.cu writes them as fp16 and runs a 1x1
-// tensor-core conv over them).  Here they never leave the SM:
+// [B, 9*C, Ho*Wo] fp32 in HBM between the two.  Here they never leave the SM:
 //
 //   GEMM view   D[128 output pixels, BN couts] = sum over taps t (9) and 64-channel chunks kc of
 //               A_t,kc[128, 64] * W[BN, t*C + kc*64 .. +64]^T,
@@ -17,8 +16,8 @@
 //               every 64-channel chunk the geometry reaches the lanes that need it by WARP SHUFFLE (8 lanes share a
 //               row: one 16-byte vector of 8 channels each), the four corners are fetched with 16-byte loads, blended
 //               (fp32 in the split mode, packed half2 in the fp16 mode) and written as one swizzled 16-byte piece of the K-major SWIZZLE_128B A tile -- the layout
-//               wgmma consumes directly.  Geometry is computed once per (pixel, tap) instead of once per
-//               (pixel, tap, 8 channels) as in the per-thread gather.
+//               wgmma consumes directly.  Geometry is computed once per (pixel, tap), not once per
+//               (pixel, tap, 8 channels).
 //   epilogue    each warpgroup: accumulator registers -> (* out_scale) + bias -> ReLU -> its rows' channel pairs.
 //   SPLIT       (YB_PREC_F16X3) x and y are [hi(C) | lo(C)] pairs, the sample is hi + lo, the A stage holds a hi (fp16)
 //               and a lo (2^11-scaled fp16) tile, the weights [Cout][hi(9C) | lo(9C)], three MMA passes per k-block.

@@ -8,7 +8,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <array>
 #include <set>
 
 namespace yb {
@@ -221,14 +220,17 @@ struct NetBuilder {
     p.x = in.ptr;
     p.x_nchw_f32 = in_nchw ? 1 : 0;
     p.split = in.split ? 1 : 0;
+    // the half-precision modes run every conv on the tensor cores: the network's NCHW input through the stem kernel,
+    // the rest through the implicit-GEMM kernel
+    const bool stem_tc = f16 && in_nchw;
+    const bool tc = f16 && !in_nchw;
+    YB_REQUIRE(!stem_tc || (!ospec && !out_f32 && !residual && stem_tc_supported(k, stride, pad, in.C, h->peek_cout(key))),
+               ("conv " + key + ": stem shape not supported by the tensor-core stem").c_str());
     // in.C may be a zero-padded channel count (the tensor-core stem pads a 32-channel output to 64, see stem_tc)
-    const bool tc = f16 && !in_nchw && (in.C % 64 == 0) && !in.f32;
-    YB_REQUIRE(!split || tc || in_nchw, ("conv " + key + ": the split-precision mode has tensor-core kernels only").c_str());
-    const bool simt_half = f16 && !tc && !in.f32;
-    const bool stem_tc = f16 && in_nchw && !ospec && !out_f32 && !residual && h->stem_on_tc &&
-                         stem_tc_supported(k, stride, pad, in.C, h->peek_cout(key));
-    ConvW& w = stem_tc ? h->get_conv(key, bn, /*want_tc=*/true, false, false, /*pack=*/2)
-                       : h->get_conv(key, bn, /*want_tc=*/tc, /*want_f32=*/!tc && !simt_half, /*want_f16=*/simt_half, 0,
+    YB_REQUIRE(!tc || (in.C % 64 == 0 && !in.f32),
+               ("conv " + key + ": the half-precision modes need fp16 inputs with Cin % 64 == 0").c_str());
+    ConvW& w = stem_tc ? h->get_conv(key, bn, /*want_tc=*/true, false, /*pack=*/2)
+                       : h->get_conv(key, bn, /*want_tc=*/tc, /*want_f32=*/!tc, 0,
                                      /*cin_pad=*/tc ? in.C : 0,
                                      // a half-precision output narrower than 64 channels (Darknet's first block: 32)
                                      // is written as zero-padded 64-channel pixels for the tensor-core conv that follows
@@ -276,9 +278,8 @@ struct NetBuilder {
     if (stem_tc) {
       StemTcPlan* sp = stem_tc_plan_create((const float*)in.ptr, w.w_tc, w.bias, (__half*)out.ptr, in.B, in.H, in.W, k,
                                            stride, pad, w.Cout, act, split ? 1 : 0, w.out_scale, out.C);
-      stem_tc_plan_set_worker_groups(sp, h->stem_wg > 0 ? h->stem_wg : (split ? 2 : 1));
       ex->stem_plans.push_back(sp);
-      op.name += " stem wg=" + std::to_string(h->stem_wg > 0 ? h->stem_wg : (split ? 2 : 1));
+      op.name += " stem";
       op.fn = [sp, lc](cudaStream_t s) { launch_stem_tc(sp, s, lc); };
       push(op);
       return out;
@@ -287,25 +288,15 @@ struct NetBuilder {
       YB_REQUIRE(tc_conv_supported(p), ("conv " + key + ": not supported by the tensor-core kernel").c_str());
       TcConvPlan* plan = autotune_tc(p, w.w_tc);
       ex->plans.push_back(plan);
-      op.name += " tc BN=" + std::to_string(tc_conv_plan_bn(plan)) + " st=" + std::to_string(tc_conv_plan_stages(plan)) +
-                 " g=" + std::to_string(tc_conv_plan_grid(plan)) + (tc_conv_plan_pair(plan) ? " pair" : "") + (tc_conv_plan_epi_groups(plan) == 2 ? " epi2" : "") +
-              (tc_conv_plan_pdl_friendly(plan) ? " pdlf" : "") + (tc_conv_plan_sk(plan) ? " sk" : "");
+      op.name += " tc " + tc_tiling_str(tc_conv_plan_tiling(plan));
       tc_conv_plan_set_pdl(plan, h->pdl ? 1 : 0);
       op.fn = [plan, lc](cudaStream_t s) { launch_tc_conv(plan, s, lc); };
       op.has_prob = true;
       op.prob = p;
       op.w_tc = w.w_tc;
     } else {
-      int types;
-      if (!f16 || in.f32) {
-        // fp32 activations in; output fp32, or fp16 when this is the stem of the fp16 network
-        types = (f16 && !out.f32) ? SIMT_F32IN_F16OUT : SIMT_F32;
-      } else {
-        types = SIMT_F16;
-      }
-      const void* wp = (types == SIMT_F16) ? (const void*)w.w_f16 : (const void*)w.w_f32;
-      YB_REQUIRE(wp != nullptr, ("conv " + key + ": weights not packed for the SIMT kernel").c_str());
-      op.fn = [p, wp, types, lc](cudaStream_t s) { launch_simt_conv(p, wp, types, s, lc); };
+      const float* wp = w.w_f32;
+      op.fn = [p, wp, lc](cudaStream_t s) { launch_simt_conv(p, wp, SIMT_F32, s, lc); };
     }
     push(op);
     return out;
@@ -357,13 +348,14 @@ struct NetBuilder {
   Act dcn(const std::string& key, const std::string& bn, const Act& in, int stride) {
     // conv_offset_mask: 3x3, same stride/pad, bias, 27 channels, fp32 output (dcn_v2.py:106-124)
     Act om = conv(key + ".conv_offset_mask", "", in, 3, stride, 1, ACT_NONE, nullptr, /*out_f32=*/true);
-    const bool tc = f16;
-    ConvW& w = h->get_conv(key, bn, /*want_tc=*/tc, /*want_f32=*/!tc, /*want_f16=*/false, /*pack=*/1);
+    ConvW& w = h->get_conv(key, bn, /*want_tc=*/f16, /*want_f32=*/!f16, /*pack=*/1);
+    YB_REQUIRE(!f16 || dcn_tc_supported(in.C, w.Cout),
+               ("dcn " + key + ": the half-precision modes need C % 64 == 0 and Cout % 8 == 0 (tensor-core DCN)").c_str());
     const int Ho = om.H, Wo = om.W;
     Act out = alloc_act(in.B, Ho, Wo, w.Cout);
     if (dry) return out;
     LaunchCounter* lc = &h->lc;
-    if (!tc) {
+    if (!f16) {
       const float* wp = w.w_f32;
       const float* bias = w.bias;
       Op op;
@@ -374,7 +366,7 @@ struct NetBuilder {
                                in.C, out.H, out.W, Cout, stride, 1, 1, ACT_RELU, 1, s, lc);
       };
       push(op);
-    } else if (h->dcn_fused && dcn_tc_supported(in.C, w.Cout)) {
+    } else {
       // one kernel: warp-shuffled tap geometry -> bilinear samples straight into the swizzled A stage -> wgmma
       const int sp = in.split ? 1 : 0;
       DcnTcPlan* dp = dcn_tc_plan_create((const __half*)in.ptr, (const float*)om.ptr, w.w_tc, w.bias, (__half*)out.ptr, in.B,
@@ -385,44 +377,6 @@ struct NetBuilder {
       op.name = key + " dcn_fused " + std::to_string(in.C) + "->" + std::to_string(w.Cout) + " k3s" + std::to_string(stride) +
                 " " + std::to_string(Ho) + "x" + std::to_string(Wo);
       op.fn = [dp, lc](cudaStream_t s) { launch_dcn_tc(dp, s, lc); };
-      push(op);
-    } else {
-      // gather -> fp16 columns [B,Ho,Wo,9C]; contraction = 1x1 conv with K = 9C on the tensor cores
-      Act cols = alloc_act(in.B, Ho, Wo, 9 * in.C);
-      Op g;
-      g.is_conv = true;
-      g.name = key + " dcn_gather";
-      const int sp = in.split ? 1 : 0;
-      g.fn = [in, om, cols, stride, lc, sp](cudaStream_t s) {
-        launch_dcn_gather_f16((const __half*)in.ptr, (const float*)om.ptr, (__half*)cols.ptr, in.B, in.H, in.W, in.C,
-                              cols.H, cols.W, stride, 1, 1, 1, s, lc, sp);
-      };
-      push(g);
-      ConvProblem p;
-      p.B = in.B;
-      p.H = Ho;
-      p.W = Wo;
-      p.Cin = 9 * in.C;
-      p.Ho = Ho;
-      p.Wo = Wo;
-      p.Cout = w.Cout;
-      p.KH = p.KW = 1;
-      p.stride = 1;
-      p.pad = 0;
-      p.act = ACT_RELU;
-      p.x = cols.ptr;
-      p.y = out.ptr;
-      p.split = sp;
-      p.out_scale = w.out_scale;
-      p.y_pix_stride = sp ? 2 * w.Cout : w.Cout;
-      p.y_batch_stride = (int64_t)Ho * Wo * p.y_pix_stride;
-      p.bias = w.bias;
-      TcConvPlan* plan = autotune_tc(p, w.w_tc);
-      ex->plans.push_back(plan);
-      Op op;
-      op.is_conv = true;
-      op.name = key + " dcn_contract K=" + std::to_string(p.Cin);
-      op.fn = [plan, lc](cudaStream_t s) { launch_tc_conv(plan, s, lc); };
       push(op);
     }
     return out;
@@ -474,10 +428,7 @@ struct NetBuilder {
     Op op;
     op.is_conv = true;
     op.name = hn + ".bbox+conf+mask " + std::to_string(in.C) + "->" + std::to_string(w.Cout) + " k3s1 " +
-              std::to_string(in.H) + "x" + std::to_string(in.W) + " tc BN=" + std::to_string(tc_conv_plan_bn(plan)) +
-              " st=" + std::to_string(tc_conv_plan_stages(plan)) + " g=" + std::to_string(tc_conv_plan_grid(plan)) +
-              (tc_conv_plan_pair(plan) ? " pair" : "") + (tc_conv_plan_epi_groups(plan) == 2 ? " epi2" : "") +
-              (tc_conv_plan_pdl_friendly(plan) ? " pdlf" : "") + (tc_conv_plan_sk(plan) ? " sk" : "");
+              std::to_string(in.H) + "x" + std::to_string(in.W) + " tc " + tc_tiling_str(tc_conv_plan_tiling(plan));
     op.fn = [plan, lc](cudaStream_t s) { launch_tc_conv(plan, s, lc); };
     push(op);
   }
@@ -499,9 +450,14 @@ struct NetBuilder {
       if (!(q.KH == q.KW && (q.KH == 1 || q.KH == 3) && q.pad == q.KH / 2 && (q.stride == 1 || q.stride == 2) && q.Cout % 64 == 0 && !q.y_f32 &&
             q.nseg == 0 && q.y_pix_stride == (q.split ? 2 : 1) * q.Cout && q.y_batch_stride == (int64_t)q.Ho * q.Wo * q.y_pix_stride))
         return nullptr;
+      TcTiling t;
+      t.bn = (q.Cout % 128 == 0) ? 128 : 64;
+      t.stages = 2;
+      t.mma_groups = 2;
+      t.chain = 1;
       TcConvPlan* pl = nullptr;
       try {
-        pl = tc_conv_plan_create(q, op.w_tc, (q.Cout % 128 == 0) ? 128 : 64, 2, 0, 0, 2, 0, 0, /*chain=*/1);
+        pl = tc_conv_plan_create(q, op.w_tc, t);
       } catch (const Error&) {
         return nullptr;
       }
@@ -643,7 +599,6 @@ struct NetBuilder {
   // layer's real buffers (contents irrelevant) with CUDA events; the fastest plan is kept.  Small layers
   // are launch/wave-quantisation bound and large-K ones L2-bandwidth bound, so no single rule fits.
   TcConvPlan* autotune_tc(const ConvProblem& p, const __half* w) {
-    if (!h->autotune) return tc_conv_plan_create(p, w);
     // identical layer shapes (e.g. the 23 blocks of stage 3) share one decision
     const std::string tkey = std::to_string(p.B) + "," + std::to_string(p.H) + "," + std::to_string(p.W) + "," +
                              std::to_string(p.Cin) + "," + std::to_string(p.Cout) + "," + std::to_string(p.KH) + "," +
@@ -651,9 +606,8 @@ struct NetBuilder {
                              (p.y_f32 ? "f" : "h") + (p.split ? "s" : "") + std::to_string(p.nseg) + "," + std::to_string(p.y_pix_stride) + "," + std::to_string((long long)p.y_batch_stride);
     auto it = h->tune_cache.find(tkey);
     if (it != h->tune_cache.end()) {
-      TcConvPlan* pl = tc_conv_plan_create(p, w, it->second[0], it->second[1], it->second[2], it->second[3], it->second[4],
-                                           it->second[5], it->second[6]);
-      if (tc_conv_plan_sk(pl)) tc_conv_plan_set_sk_workspace(pl, sk_workspace());
+      TcConvPlan* pl = tc_conv_plan_create(p, w, it->second);
+      if (tc_conv_plan_tiling(pl).stream_k) tc_conv_plan_set_sk_workspace(pl, sk_workspace());
       return pl;
     }
     const int bns[4] = {256, 128, 64, 32};
@@ -665,10 +619,7 @@ struct NetBuilder {
     cudaEvent_t e0, e1;
     YB_CHECK_CUDA(cudaEventCreate(&e0));
     YB_CHECK_CUDA(cudaEventCreate(&e1));
-    // extra candidates: CTA pairs (clusters of two, persistent grid only) and two MMA warpgroups per CTA
-    const int npair = h->pair_candidates ? 2 : 1;
-    const int nepi = h->epi2_candidates ? 2 : 1;
-    // YB_PDL=1 (experimental): every single-CTA candidate is timed with programmatic dependent launch on a private
+    // in the fp16 mode (h->pdl) every single-CTA candidate is timed with programmatic dependent launch on a private
     // stream (consecutive launches of one kernel overlap like consecutive layers do), plus "PDL-friendly" plans that
     // leave room on the SM for the next layer's CTA
     const int npdl = h->pdl ? 2 : 1;
@@ -681,8 +632,8 @@ struct NetBuilder {
     const int nsk = h->sk_candidates ? 2 : 1;   // stream-K: persistent default grid only
     for (int ki = 0; ki < nsk; ++ki)
     for (int di = 0; di < npdl; ++di)
-    for (int ei = 0; ei < nepi; ++ei)
-    for (int pi = 0; pi < npair; ++pi)
+    for (int ei = 0; ei < 2; ++ei)     // two MMA warpgroups per CTA
+    for (int pi = 0; pi < 2; ++pi)     // CTA pairs (clusters of two, persistent grid only)
     for (int bi = 0; bi < 4; ++bi)
       for (int si = 0; si < 3; ++si)
         for (int gi = 0; gi < (pi ? 1 : 3); ++gi) {
@@ -691,24 +642,28 @@ struct NetBuilder {
           if (ei && (bns[bi] < 64 || gi == 1)) continue;   // 384-thread CTAs: one per SM
           if (di && (pi || ei || gi == 1)) continue;        // PDL-friendly: single CTAs, one MMA warpgroup, <= 1 CTA/SM of its own
           if (ki && (gi != 0 || di || h->pdl)) continue;    // stream-K: one CTA (cluster) per SM (TPC), no PDL
+          TcTiling want;
+          want.bn = bns[bi];
+          want.stages = sts[si];
+          want.grid = grids[gi];
+          want.pair = pi;
+          want.mma_groups = ei ? 2 : 1;
+          want.pdl_friendly = di;
+          want.stream_k = ki;
           TcConvPlan* cand = nullptr;
           try {
-            cand = tc_conv_plan_create(p, w, bns[bi], sts[si], grids[gi], pi, ei ? 2 : 1, di, ki);
+            cand = tc_conv_plan_create(p, w, want);
           } catch (const Error&) {
             continue;   // this tiling does not fit in shared memory (split precision doubles every stage)
           }
-          if ((pi && !tc_conv_plan_pair(cand)) || (ei && tc_conv_plan_epi_groups(cand) != 2) ||
-              (di && !tc_conv_plan_pdl_friendly(cand)) || (ki && !tc_conv_plan_sk(cand))) {
+          const TcTiling got = tc_conv_plan_tiling(cand);
+          if ((pi && !got.pair) || (ei && got.mma_groups != 2) || (di && !got.pdl_friendly) || (ki && !got.stream_k)) {
             tc_conv_plan_destroy(cand);
             continue;
           }
           if (ki) tc_conv_plan_set_sk_workspace(cand, sk_workspace());
           if (h->pdl) tc_conv_plan_set_pdl(cand, 1);
-          const std::string ck = std::to_string(tc_conv_plan_bn(cand)) + "/" + std::to_string(tc_conv_plan_stages(cand)) +
-                                 "/" + std::to_string(tc_conv_plan_grid(cand)) + "/" + std::to_string(tc_conv_plan_pair(cand)) + "/" +
-                                 std::to_string(tc_conv_plan_epi_groups(cand)) + "/" + std::to_string(tc_conv_plan_pdl_friendly(cand)) +
-                                 "/" + std::to_string(tc_conv_plan_sk(cand));
-          if (!seen.insert(ck).second) {  // overrides were clamped to an already-timed configuration
+          if (!seen.insert(tc_tiling_str(got)).second) {  // overrides were clamped to an already-timed configuration
             tc_conv_plan_destroy(cand);
             continue;
           }
@@ -738,8 +693,7 @@ struct NetBuilder {
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
     YB_REQUIRE(best != nullptr, "autotune: no candidate");
-    h->tune_cache[tkey] = {tc_conv_plan_bn(best), tc_conv_plan_stages(best), tc_conv_plan_grid(best), tc_conv_plan_pair(best),
-                           tc_conv_plan_epi_groups(best), tc_conv_plan_pdl_friendly(best), tc_conv_plan_sk(best)};
+    h->tune_cache[tkey] = tc_conv_plan_tiling(best);
     return best;
   }
 };
@@ -863,7 +817,7 @@ void build_network(yb_handle* h, Executor* ex, bool dry) {
     nb.lane = 1 + l;
     const std::string hn = "prediction_layers.0";
     Act u = nb.conv(hn + ".upfeature.0", "", Pl[l], 3, 1, 1, ACT_RELU);
-    if (nb.f16 && h->fuse_heads) {
+    if (nb.f16) {
       // bbox + conf + mask convs share their input: one tensor-core launch with Cout = A*(4+C+k), the epilogue
       // routes channel ranges to the three concatenated fp32 tensors (tanh on the mask coefficients)
       nb.fused_head(hn, u, ex->loc ? ex->loc + level_off[l] * 4 : nullptr, ex->conf ? ex->conf + level_off[l] * NC : nullptr,
@@ -968,7 +922,7 @@ static const HostTensor& need(yb_handle* h, const std::string& name) {
 }
 
 ConvW& yb_handle::get_conv(const std::string& conv_key, const std::string& bn_key, bool want_tc, bool want_f32,
-                           bool want_f16, int pack, int cin_pad, int cout_pad) {
+                           int pack, int cin_pad, int cout_pad) {
   ConvW& cw = convs[conv_key];
   const HostTensor& w = need(this, conv_key + ".weight");
   YB_REQUIRE(w.shape.size() == 4, ("weight " + conv_key + " is not 4-D").c_str());
@@ -988,8 +942,7 @@ ConvW& yb_handle::get_conv(const std::string& conv_key, const std::string& bn_ke
   const bool has_bn = !bn_key.empty();
   const bool need_f32 = want_f32 && !cw.w_f32;
   const bool need_tc = want_tc && !cw.w_tc;
-  const bool need_f16 = want_f16 && !cw.w_f16;
-  if (!need_f32 && !need_tc && !need_f16 && (cw.bias || (!has_bias && !has_bn))) return cw;
+  if (!need_f32 && !need_tc && (cw.bias || (!has_bias && !has_bn))) return cw;
 
   // fold BatchNorm (eval mode, eps = 1e-5): w' = w * g/sqrt(v+eps); b' = beta + (b - mean) * g/sqrt(v+eps)
   std::vector<float> scale(Co, 1.f), shift(Co, 0.f);
@@ -1021,15 +974,6 @@ ConvW& yb_handle::get_conv(const std::string& conv_key, const std::string& bn_ke
           pk[((size_t)t * Ci + c) * Co + o] = w.data[((size_t)o * Ci + c) * taps + t] * scale[o];
     cw.w_f32 = (float*)dmalloc(weight_allocs, pk.size() * 4);
     YB_CHECK_CUDA(cudaMemcpy(cw.w_f32, pk.data(), pk.size() * 4, cudaMemcpyHostToDevice));
-  }
-  if (need_f16) {
-    std::vector<__half> pk(K * Co);
-    for (int o = 0; o < Co; ++o)
-      for (int c = 0; c < Ci; ++c)
-        for (int t = 0; t < taps; ++t)
-          pk[((size_t)t * Ci + c) * Co + o] = __float2half_rn(w.data[((size_t)o * Ci + c) * taps + t] * scale[o]);
-    cw.w_f16 = (__half*)dmalloc(weight_allocs, pk.size() * 2);
-    YB_CHECK_CUDA(cudaMemcpy(cw.w_f16, pk.data(), pk.size() * 2, cudaMemcpyHostToDevice));
   }
   const bool split = (cfg.precision == YB_PREC_F16X3);
   if (need_tc && split) {
@@ -1072,7 +1016,7 @@ ConvW& yb_handle::get_conv(const std::string& conv_key, const std::string& bn_ke
           for (int t = 0; t < taps; ++t)
             pk[(size_t)o * kpad + (size_t)c * taps + t] = __float2half_rn(w.data[((size_t)o * Ci + c) * taps + t] * scale[o]);
     } else if (pack == 1) {
-      // [Cout][tap*Cin + c]: the contraction runs as a 1x1 conv over gathered columns
+      // DCN: [Cout][tap*Cin + c], the K order of the fused kernel's gathered A stage
       for (int o = 0; o < Co; ++o)
         for (int c = 0; c < Ci; ++c)
           for (int t = 0; t < taps; ++t)
@@ -1165,7 +1109,7 @@ void yb_handle::finalize() {
   build_network(this, &dry, /*dry=*/true);
   if (cfg.use_maskiou) {
     const char* idx[6] = {"0", "2", "4", "6", "8", "10"};
-    for (int i = 0; i < 6; ++i) get_conv(std::string("maskiou_net.maskiou_net.") + idx[i], "", false, true, false);
+    for (int i = 0; i < 6; ++i) get_conv(std::string("maskiou_net.maskiou_net.") + idx[i], "", false, true);
   }
   finalized = true;
 }
@@ -1270,7 +1214,7 @@ void yb_handle::forward(const float* d_x, int B, int H, int W, float* d_loc, flo
       cudaStream_t cs = capture_stream();
       YB_CHECK_CUDA(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
       try {
-        run_ops(this, ex, cs, multi_stream);
+        run_ops(this, ex, cs, true);
       } catch (...) {
         cudaStreamEndCapture(cs, &g);
         if (g) cudaGraphDestroy(g);
@@ -1341,7 +1285,7 @@ void yb_handle::infer(const float* d_x, int B, int H, int W, int cross_class, in
       cudaStream_t cs = capture_stream();
       YB_CHECK_CUDA(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
       try {
-        run_all(cs, multi_stream);
+        run_all(cs, true);
       } catch (...) {
         cudaStreamEndCapture(cs, &g);
         if (g) cudaGraphDestroy(g);

@@ -1,7 +1,6 @@
 // Host-side engine: weight store (reference state_dict names), BatchNorm folding + repacking,
 // per-input-shape executors (activation buffers, kernel plans, CUDA graph), Detect workspaces.
 #pragma once
-#include <array>
 #include <functional>
 #include <map>
 #include <memory>
@@ -31,7 +30,6 @@ struct ConvW {
   int cin_pad = 0;           // w_tc rows are padded with zeros to this many input channels (a multiple of 64) when the
                              // producer writes zero-padded pixels (Darknet: 32 -> 64); 0 = Cin
   float* w_f32 = nullptr;    // [KH*KW*Cin][Cout]           (SIMT fp32)
-  __half* w_f16 = nullptr;   // [KH*KW*Cin][Cout]           (SIMT fp16)
   __half* w_tc = nullptr;    // [KH*KW][Cout][Cin]          (tensor cores), or [1][Cout][9*Cin] for DCN
   float* bias = nullptr;     // [Cout] or null
   int pack = 0;              // 0 normal, 1 DCN ([Cout][9*Cin]), 2 stem ([Cout][Kpad], OIHW order)
@@ -112,21 +110,14 @@ struct yb_handle {
   bool finalized = false;
   bool use_graphs = true;
   bool profiling = false;
-  bool fuse_heads = true;   // YB_FUSE_HEADS=0: three separate head convs per level
-  bool pdl = false;         // programmatic dependent launch between consecutive tensor-core convs: on in the fp16 mode (YB_PDL=0/1)
-  bool stem_on_tc = true;   // YB_STEM_TC=0 falls back to the SIMT stem
-  bool dcn_fused = true;    // YB_DCN_FUSED=0: separate gather kernel + fp16 column buffer + 1x1 tensor-core contraction
-  int stem_wg = 0;          // YB_STEM_WG=1|2: worker threads per output pixel in the 7x7 stem; 0 = 1 in the fp16 mode, 2 in the split mode
-  bool autotune = true;     // YB_AUTOTUNE=0 disables plan-time autotuning of the tensor-core tiles
-  bool pair_candidates = true;    // YB_PAIR=0: the autotuner skips CTA-pair (cluster of two) plans
-  bool epi2_candidates = true;    // YB_EPI2=0: the autotuner skips plans with two MMA warpgroups (384 threads)
+  bool pdl = false;         // programmatic dependent launch between consecutive tensor-core convs: on in the fp16 mode
   float last_total_ms = 0.f, last_conv_ms = 0.f;
   yb::LaunchCounter lc;
   std::map<std::string, yb::HostTensor> host;
   std::map<std::string, yb::ConvW> convs;
   std::map<std::string, std::unique_ptr<yb::Executor>> execs;
   std::vector<void*> weight_allocs;
-  std::map<std::string, std::array<int, 7>> tune_cache;  // layer shape -> (BN, stages, grid, pair, MMA warpgroups, pdl-friendly, stream-K) from the autotuner
+  std::map<std::string, yb::TcTiling> tune_cache;  // layer shape -> the autotuner's tiling
   bool sk_candidates = true;      // the autotuner times stream-K plans: on in the split mode (YB_SK=0/1)
   int chain_mode = 1;             // runs of consecutive convs as one chain launch: 0 never, 1 when timed faster, 2 always (YB_CHAIN)
   cudaStream_t tune_stream = nullptr;   // private stream of the autotuner when PDL candidates are timed
@@ -139,7 +130,6 @@ struct yb_handle {
   cudaStream_t cap_stream = nullptr;  // private stream used only for CUDA-graph capture
   cudaStream_t lane_streams[8] = {};  // branch streams joined into the capture (parallel graph branches)
   cudaEvent_t ev_fork = nullptr, ev_join[8] = {};
-  bool multi_stream = true;           // YB_BRANCHES=0: capture a linear graph
   // call serialisation (capi.cu CallGuard): host-side mutex + device-side ordering across caller streams
   std::recursive_mutex mu;
   cudaEvent_t ev_last = nullptr;
@@ -150,7 +140,7 @@ struct yb_handle {
 
   // ---- weights
   yb::ConvW& get_conv(const std::string& conv_key, const std::string& bn_key, bool want_tc, bool want_f32,
-                      bool want_f16, int pack = 0, int cin_pad = 0, int cout_pad = 0);
+                      int pack = 0, int cin_pad = 0, int cout_pad = 0);
   int peek_cout(const std::string& conv_key) const;
   yb::ConvW& get_fused_head(const std::string& head_name);
   void finalize();

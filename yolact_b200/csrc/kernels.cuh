@@ -41,7 +41,6 @@ struct ConvProblem {
 
 enum SimtTypes : int {
   SIMT_F32 = 0,        // x float (NHWC or NCHW), w float, y float
-  SIMT_F32IN_F16OUT,   // x float (NCHW stem), w float, y half
   SIMT_F16,            // x half, w half, y half (or float when y_f32)
 };
 
@@ -52,26 +51,27 @@ void launch_simt_conv(const ConvProblem& p, const void* w, int types, cudaStream
 // ---- wgmma implicit-GEMM convolution (fp16 in, fp32 accumulate) ------------------------------
 struct TcConvPlan;  // opaque: tensor maps + tiling; built once per (layer, shape, pointers)
 int device_sms();   // SMs of the current device
+// The tiling of a tensor-core conv plan.  As a request to tc_conv_plan_create every field is an override, 0 = heuristic;
+// tc_conv_plan_tiling returns what a plan resolved to, which replayed as a request gives the same plan.
+struct TcTiling {
+  int bn = 0;             // N tile in {32, 64, 128, 256}
+  int stages = 0;         // caps the pipeline depth
+  int grid = 0;           // caps the number of (persistent) CTAs, counted as CTAs (a pair plan's grid is even);
+                          // default device_sms() = one per SM
+  int pair = 0;           // > 0: CTA pairs (cluster of 2; each CTA loads half the weight tile and multicasts it to both)
+  int mma_groups = 0;     // 2: two MMA warpgroups (384 threads)
+  int pdl_friendly = 0;   // > 0: plan sized for 2 CTAs/SM + programmatic dependent launch
+  int stream_k = 0;       // > 0: stream-K (needs tc_conv_plan_set_sk_workspace before launch)
+  int chain = 0;          // > 0: a chain-kernel plan (residual read from global memory in every mode)
+};
+// "BN=128 st=4 g=132 pair epi2 pdlf sk": names a tiling in op names, and keys the autotuner's dedupe set
+std::string tc_tiling_str(const TcTiling& t);
 // w_packed: device half [KH*KW][Cout][Cin] ([KH*KW][Cout][2*Cin] when p.split). Requires Cin % 64 == 0.
-// bn_override in {32,64,128,256} / stages_override > 0 pin the N tile / pipeline depth (autotuner); 0 = heuristic.
-// grid_override > 0 caps the number of (persistent) CTAs; default device_sms() = one per SM.
-// pair_override > 0: CTA pairs (cluster of 2; each CTA loads half the weight tile and multicasts it to both).
-TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, int bn_override = 0,
-                                int stages_override = 0, int grid_override = 0, int pair_override = 0,
-                                int epi_override = 0,    // epi_override == 2: two MMA warpgroups (384 threads)
-                                int pdl_override = 0,    // > 0: plan sized for 2 CTAs/SM + programmatic dependent launch
-                                int sk_override = 0,     // > 0: stream-K (needs tc_conv_plan_set_sk_workspace before launch)
-                                int chain_override = 0); // > 0: a chain-kernel plan (residual read from global memory in every mode)
-int tc_conv_plan_sk(const TcConvPlan* plan);
+TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, const TcTiling& want = {});
+TcTiling tc_conv_plan_tiling(const TcConvPlan* plan);
 size_t tc_conv_sk_workspace_bytes();
 void tc_conv_plan_set_sk_workspace(TcConvPlan* plan, void* ws);
-int tc_conv_plan_pdl_friendly(const TcConvPlan* plan);
-int tc_conv_plan_pair(const TcConvPlan* plan);
-int tc_conv_plan_epi_groups(const TcConvPlan* plan);
-int tc_conv_plan_grid(const TcConvPlan* plan);
 void tc_conv_plan_set_pdl(TcConvPlan* plan, int enable);   // programmatic dependent launch (prologue overlap)
-int tc_conv_plan_bn(const TcConvPlan* plan);
-int tc_conv_plan_stages(const TcConvPlan* plan);
 void tc_conv_plan_destroy(TcConvPlan* plan);
 bool tc_conv_supported(const ConvProblem& p);
 void launch_tc_conv(const TcConvPlan* plan, cudaStream_t stream, LaunchCounter* lc);
@@ -92,12 +92,12 @@ struct StemTcPlan;
 bool stem_tc_supported(int ks, int stride, int pad, int cin, int cout);
 int stem_tc_kpad(int ks);   // K = 3*ks*ks rounded up to 64
 // w_packed: device half [cout][kpad], k = c*ks*ks + r*ks + s (OIHW flattening), zero padded
-// split: w_packed is [cout][hi(kpad) | lo(kpad)] scaled by 1 / out_scale, y is [.., hi(cout) | lo(cout)]
+// split: w_packed is [cout][hi(kpad) | lo(kpad)] scaled by 1 / out_scale, y is [.., hi(cout) | lo(cout)]; the split 7x7
+// stem runs two worker threads per output pixel
 StemTcPlan* stem_tc_plan_create(const float* x_nchw, const __half* w_packed, const float* bias, __half* y, int B,
                                 int H, int W, int ks, int stride, int pad, int cout, int act, int split = 0,
                                 float out_scale = 1.f, int cpad = 0);   // cpad > cout: zero-padded output pixels
 void stem_tc_plan_destroy(StemTcPlan* plan);
-void stem_tc_plan_set_worker_groups(StemTcPlan* plan, int wg);   // 2 / 4: two / four threads per pixel (7x7 stem)
 void launch_stem_tc(const StemTcPlan* plan, cudaStream_t stream, LaunchCounter* lc);
 
 // ---- pointwise -------------------------------------------------------------------------------
@@ -192,11 +192,6 @@ template <typename T>
 void launch_dcn_simt(const T* x, const float* om, const T* w, const float* bias, T* y, int B, int H,
                      int W, int C, int Ho, int Wo, int Cout, int stride, int pad, int dil, int act,
                      int mask_logits, cudaStream_t stream, LaunchCounter* lc);
-// Deformable gather only: writes the modulated, bilinearly sampled columns as NHWC half
-// [B,Ho,Wo,9*C] (tap-major) so the tensor-core 1x1 contraction can consume them.
-void launch_dcn_gather_f16(const __half* x, const float* om, __half* cols, int B, int H, int W,
-                           int C, int Ho, int Wo, int stride, int pad, int dil, int mask_logits,
-                           cudaStream_t stream, LaunchCounter* lc, int split = 0);
 
 // ---- fused DCNv2 on the tensor cores (dcn_tc.cu): gather -> smem A stage -> MMA -> bias/act, no column buffer ----------------
 struct DcnTcPlan;

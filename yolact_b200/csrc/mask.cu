@@ -338,8 +338,8 @@ void launch_mask_assembly(const float* proto, int ph, int pw, int k, const float
     const int bands = ceil_div(out_h, band);
     // >= ~4 waves of 8 resident CTAs per SM: enough stores in flight to approach the HBM write rate and a short
     // tail (bands that cross many boxes take several times longer than empty ones); groups stay >= 8 detections
-    // so the band's prototype rows are reused from L1.  YB_MASK_CTAS_PER_SM overrides the target (tuning hook).
-    static const int ctas_per_sm = getenv("YB_MASK_CTAS_PER_SM") ? std::max(1, atoi(getenv("YB_MASK_CTAS_PER_SM"))) : 32;
+    // so the band's prototype rows are reused from L1.
+    const int ctas_per_sm = 32;
     int group = n;
     while (group > 8 && (int64_t)bands * ceil_div(n, group) * batch < (int64_t)ctas_per_sm * 132) group = (group + 1) / 2;
     dim3 grid(bands, ceil_div(n, group), batch);

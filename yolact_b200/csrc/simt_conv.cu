@@ -1,8 +1,7 @@
 // Generic implicit-GEMM convolution on CUDA cores (fp32 FMA, fp32 accumulation).
 //
-// Role in the design (DESIGN.md): (1) the whole network in YB_PREC_F32 parity mode, (2) the layers
-// the tensor-core kernel does not take in YB_PREC_F16TC mode (7x7 stem with Cin=3, FastMaskIoUNet),
-// (3) on-device second opinion for the tensor-core kernel in tests.
+// Role in the design (DESIGN.md): (1) the whole network in YB_PREC_F32 parity mode, (2) FastMaskIoUNet
+// in every mode, (3) on-device second opinion for the tensor-core kernel in tests.
 //
 // Reference semantics: nn.Conv2d (cross-correlation, zero padding) + folded BatchNorm2d bias
 // (backbone.py:37-57) + optional residual add + activation.
@@ -153,10 +152,6 @@ void launch_simt_conv(const ConvProblem& p, const void* w, int types, cudaStream
   switch (types) {
     case SIMT_F32:
       launch_t<float, float, float>(p, w, stream);
-      break;
-    case SIMT_F32IN_F16OUT:
-      YB_REQUIRE(!p.residual, "simt_conv: residual must match input dtype");
-      launch_t<float, float, __half>(p, w, stream);
       break;
     case SIMT_F16:
       YB_REQUIRE(!p.x_nchw_f32, "simt_conv: NCHW input is fp32 only");

@@ -5,8 +5,8 @@
 // Cin = 3 is useless for TMA (6 bytes per pixel) so the A operand is built by the CUDA cores:
 // each of the 128 worker threads owns one output pixel, gathers its KxKx3 patch straight from the
 // fp32 NCHW frame (zero padding by predication, layout conversion and fp32->fp16 cast fused in),
-// (with WG = 2 / 4 worker warpgroups, two / four threads share a pixel: alternate 16-byte k-groups of the patch --
-// more warps in flight for the latency-bound gather)
+// (with WG = 2 worker warpgroups, as in the split-precision 7x7 stem, two threads share a pixel: alternate 16-byte
+// k-groups of the patch -- more warps in flight for the latency-bound gather)
 // and writes it as one K-major SWIZZLE_128B row of the wgmma A tile in shared memory
 // (k = c*K*K + r*K + s, the OIHW flattening, so the weights need no permutation).  Thread 0 TMA-loads the
 // [Cout][Kpad] weight tile meanwhile; then warpgroup w runs ceil(K/16) wgmmas (M = 64, N = Cout) for the 64-row
@@ -198,7 +198,6 @@ void launch_variant(const StemParams& prm, cudaStream_t stream) {
 struct StemTcPlan {
   StemParams prm;
   int ks, stride, pad, cout;
-  int wg = 1;   // worker groups (7x7 stem only)
   int split = 0;
 };
 
@@ -242,27 +241,17 @@ StemTcPlan* stem_tc_plan_create(const float* x_nchw, const __half* w_packed, con
 }
 
 void stem_tc_plan_destroy(StemTcPlan* plan) { delete plan; }
-void stem_tc_plan_set_worker_groups(StemTcPlan* plan, int wg) {
-  plan->wg = ((wg == 2 || wg == 4) && plan->ks == 7) ? wg : 1;
-}
 
 void launch_stem_tc(const StemTcPlan* plan, cudaStream_t stream, LaunchCounter* lc) {
   if (plan->split) {
     // the split stem holds 144 KB of operand tiles (one CTA per SM): two worker threads per pixel double the warps
-    // that hide the gather's latency (YB_STEM_WG=1 selects one)
-    if (plan->ks == 7 && plan->wg == 4)
-      launch_variant<7, 2, 3, 64, 4, true>(plan->prm, stream);   // 512 workers: 4 threads per pixel
-    else if (plan->ks == 7 && plan->wg == 2)
+    // that hide the gather's latency
+    if (plan->ks == 7)
       launch_variant<7, 2, 3, 64, 2, true>(plan->prm, stream);
-    else if (plan->ks == 7)
-      launch_variant<7, 2, 3, 64, 1, true>(plan->prm, stream);
     else
       launch_variant<3, 1, 1, 32, 1, true>(plan->prm, stream);
   } else if (plan->ks == 7) {
-    if (plan->wg == 2)
-      launch_variant<7, 2, 3, 64, 2, false>(plan->prm, stream);
-    else
-      launch_variant<7, 2, 3, 64, 1, false>(plan->prm, stream);
+    launch_variant<7, 2, 3, 64, 1, false>(plan->prm, stream);
   } else {
     launch_variant<3, 1, 1, 32, 1, false>(plan->prm, stream);
   }

@@ -1066,6 +1066,7 @@ struct TcConvPlan {
   int pair = 0;
   int epi_groups = 1;   // H: MMA warpgroups per CTA (each owns 2/H of the tile's 64-row halves)
   int pdl_friendly = 0; // sized so that two CTAs (this kernel's and the next layer's) fit on one SM
+  int chain = 0;        // planned for the chain kernel
   int flat = 0;         // 1x1 / stride 1 / dense: all pixels of the batch on one axis
   int B = 0, Ho = 0, Wo = 0;   // the problem's output geometry (prm.Ho / prm.Wo are the flattened view's)
   int Hi = 0, Wi = 0, stride = 1, pad = 0, KH = 1;
@@ -1138,9 +1139,7 @@ void tc_chain_debug_deps(int B, int Hin, int Win, int k, int stride, int pad, in
   for (int i = 0; i < 14; ++i) out[i] = v[i];
 }
 
-TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, int bn_override, int stages_override,
-                                int grid_override, int pair_override, int epi_override, int pdl_override, int sk_override,
-                                int chain_override) {
+TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, const TcTiling& want) {
   YB_REQUIRE(tc_conv_supported(p), "tc_conv: unsupported problem");
   YB_REQUIRE(p.Ho == (p.H + 2 * p.pad - p.KH) / p.stride + 1, "tc_conv: bad Ho");
   YB_REQUIRE(p.Wo == (p.W + 2 * p.pad - p.KW) / p.stride + 1, "tc_conv: bad Wo");
@@ -1221,16 +1220,16 @@ TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, in
       }
     }
     plan->BN = bn_best;
-    if (bn_override == 32 || bn_override == 64 || bn_override == 128 || bn_override == 256)
-      plan->BN = std::max(bn_override, bn_min);
+    if (want.bn == 32 || want.bn == 64 || want.bn == 128 || want.bn == 256)
+      plan->BN = std::max(want.bn, bn_min);
   }
   // ---- CTA pairs: two adjacent M tiles per (cluster of 2), each CTA loads half of the weight tile for both
-  const int pair = (pair_override > 0 && m_tiles >= 2 && plan->BN >= 64) ? 1 : 0;
+  const int pair = (want.pair > 0 && m_tiles >= 2 && plan->BN >= 64) ? 1 : 0;
   // PDL-friendly plan: <= ~108 KB of shared memory and one MMA warpgroup, so that a CTA of the NEXT layer can become
   // resident beside it and overlap its prologue + first weight tiles
-  const int pdlf = (pdl_override > 0 && !pair && !split) ? 1 : 0;
+  const int pdlf = (want.pdl_friendly > 0 && !pair && !split) ? 1 : 0;
   // ---- MMA warpgroups: the accumulators of a thread (npl * BN / H fp32 registers) must stay <= 128
-  int H = (epi_override == 2 && plan->BN >= 64 && !pdlf) ? 2 : 1;
+  int H = (want.mma_groups == 2 && plan->BN >= 64 && !pdlf) ? 2 : 1;
   if (npl * plan->BN > 128 && !pdlf) H = 2;
   while (npl * plan->BN / H > 128 && plan->BN > std::max(bn_min, pair ? 64 : 32)) plan->BN /= 2;
   YB_REQUIRE(npl * plan->BN / H <= 128, "tc_conv: accumulator tile exceeds the register budget");
@@ -1247,14 +1246,14 @@ TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, in
   q.n_tiles = ceil_div(p.Cout, BN);
   const int num_tiles = (pair ? (q.m_tiles + 1) / 2 : q.m_tiles) * q.n_tiles;   // work units (pairs of M tiles when paired)
   const int max_grid = pair ? sms / 2 : sms;
-  int grid = std::min(num_tiles, grid_override > 0 ? (pair ? std::max(1, grid_override / 2) : grid_override) : max_grid);
+  int grid = std::min(num_tiles, want.grid > 0 ? (pair ? std::max(1, want.grid / 2) : want.grid) : max_grid);
   if (pair) grid = std::min(grid, max_grid);
   // stream-K: one share of the k-block iterations per SM (cluster), whatever the unit count -- worth it only when the
   // units do not fill whole waves; needs the staged (TMA) epilogue and co-resident CTAs (<= one per SM)
   const long long total_it = (long long)num_tiles * q.ntaps * q.kchunks;
-  int sk = (sk_override > 0 && q.epi_tma && !(pdl_override > 0)) ? 1 : 0;
+  int sk = (want.stream_k > 0 && q.epi_tma && !(want.pdl_friendly > 0)) ? 1 : 0;
   if (sk) {
-    const int gsk = std::min<long long>(grid_override > 0 ? grid : max_grid, total_it);
+    const int gsk = std::min<long long>(want.grid > 0 ? grid : max_grid, total_it);
     if (gsk <= 1 || num_tiles % gsk == 0) sk = 0;   // whole waves already: nothing to balance
     else grid = gsk;
   }
@@ -1263,7 +1262,8 @@ TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, in
   // staging: 2 x 16 KB (two fp16 buffers, or one buffer of a hi and a lo tile); the direct (fp32) epilogue stores
   // straight from the accumulator registers
   const int out_bytes = q.epi_tma ? 2 * A_STAGE_BYTES : 0;
-  q.res_direct = ((split || chain_override > 0) && H == 2 && p.residual && flat && q.epi_tma) ? 1 : 0;
+  plan->chain = want.chain > 0 ? 1 : 0;
+  q.res_direct = ((split || plan->chain) && H == 2 && p.residual && flat && q.epi_tma) ? 1 : 0;
   const int res_bytes = (q.epi_tma && p.residual && !q.res_direct) ? 2 * A_STAGE_BYTES : 0;
   int stages = std::min(MAX_STAGES, ((pdlf ? 108 : 225) * 1024 - out_bytes - res_bytes) / stage_bytes);
   if (stages < 1 && pdlf) {   // does not fit in half an SM: an ordinary plan
@@ -1271,7 +1271,7 @@ TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, in
     stages = std::min(MAX_STAGES, (225 * 1024 - out_bytes - res_bytes) / stage_bytes);
   }
   YB_REQUIRE(stages >= 1, "tc_conv: tile does not fit in shared memory");
-  if (stages_override > 0) stages = std::min(stages, stages_override);
+  if (want.stages > 0) stages = std::min(stages, want.stages);
   stages = std::max(1, std::min(stages, q.ntaps * q.kchunks * tiles_per_cta));
   q.stages = stages;
   q.out_off = stages * stage_bytes;
@@ -1375,13 +1375,23 @@ TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, in
 
 void tc_conv_plan_destroy(TcConvPlan* plan) { delete plan; }
 void tc_conv_plan_set_pdl(TcConvPlan* plan, int enable) { plan->prm.pdl = (enable && !plan->pair) ? 1 : 0; }
-int tc_conv_plan_bn(const TcConvPlan* plan) { return plan->BN; }
-int tc_conv_plan_stages(const TcConvPlan* plan) { return plan->prm.stages; }
-int tc_conv_plan_grid(const TcConvPlan* plan) { return (int)plan->grid.x; }
-int tc_conv_plan_pair(const TcConvPlan* plan) { return plan->pair; }
-int tc_conv_plan_epi_groups(const TcConvPlan* plan) { return plan->epi_groups; }
-int tc_conv_plan_pdl_friendly(const TcConvPlan* plan) { return plan->pdl_friendly; }
-int tc_conv_plan_sk(const TcConvPlan* plan) { return plan->sk; }
+TcTiling tc_conv_plan_tiling(const TcConvPlan* plan) {
+  TcTiling t;
+  t.bn = plan->BN;
+  t.stages = plan->prm.stages;
+  t.grid = (int)plan->grid.x;
+  t.pair = plan->pair;
+  t.mma_groups = plan->epi_groups;
+  t.pdl_friendly = plan->pdl_friendly;
+  t.stream_k = plan->sk;
+  t.chain = plan->chain;
+  return t;
+}
+std::string tc_tiling_str(const TcTiling& t) {
+  return "BN=" + std::to_string(t.bn) + " st=" + std::to_string(t.stages) + " g=" + std::to_string(t.grid) +
+         (t.pair ? " pair" : "") + (t.mma_groups == 2 ? " epi2" : "") + (t.pdl_friendly ? " pdlf" : "") +
+         (t.stream_k ? " sk" : "") + (t.chain ? " chain" : "");
+}
 // one slot per SM of the current device (a stream-K grid has at most one CTA per SM)
 size_t tc_conv_sk_workspace_bytes() { return (size_t)device_sms() * BLOCK_M * 256 * sizeof(float) + device_sms() * 2 * sizeof(int); }
 // ws: tc_conv_sk_workspace_bytes() of device memory whose LAST device_sms() * 2 ints (the flags) are zero; kernels that share a
