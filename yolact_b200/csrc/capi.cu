@@ -40,45 +40,6 @@ struct DeviceGuard {
   }
 };
 
-// OIHW fp32 (device) -> [K][Cout] (T), K = (r*KW+s)*Cin + c
-template <typename T>
-__global__ void pack_w_simt_kernel(const float* __restrict__ w, T* __restrict__ out, int Co, int Ci, int taps) {
-  const int64_t total = (int64_t)Co * Ci * taps;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    int t = (int)(i % taps);
-    int64_t r = i / taps;
-    int c = (int)(r % Ci);
-    int o = (int)(r / Ci);
-    out[((int64_t)t * Ci + c) * Co + o] = from_f32<T>(w[i]);
-  }
-}
-// OIHW fp32 (device) -> [Cout][tap*Cin + c] half (the fused DCN kernel's weights)
-__global__ void pack_w_dcn_tc_kernel(const float* __restrict__ w, __half* __restrict__ out, int Co, int Ci, int taps) {
-  const int64_t total = (int64_t)Co * Ci * taps;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    int t = (int)(i % taps);
-    int64_t r = i / taps;
-    int c = (int)(r % Ci);
-    int o = (int)(r / Ci);
-    out[(int64_t)o * taps * Ci + (int64_t)t * Ci + c] = from_f32<__half>(w[i]);
-  }
-}
-// split-precision variant: [Cout][hi(9*Cin) | lo(9*Cin)] of w * up (up = a power of two)
-__global__ void pack_w_dcn_tc_split_kernel(const float* __restrict__ w, __half* __restrict__ out, int Co, int Ci, int taps,
-                                           float up) {
-  const int64_t total = (int64_t)Co * Ci * taps;
-  const int64_t K = (int64_t)taps * Ci;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    int t = (int)(i % taps);
-    int64_t r = i / taps;
-    int c = (int)(r % Ci);
-    int o = (int)(r / Ci);
-    __half hi, lo;
-    split_f32(w[i] * up, hi, lo);   // same pair format as the activations
-    out[(int64_t)o * 2 * K + (int64_t)t * Ci + c] = hi;
-    out[(int64_t)o * 2 * K + K + (int64_t)t * Ci + c] = lo;
-  }
-}
 // offset [B,18,HW] + mask [B,9,HW] (NCHW fp32) -> om [B,HW,27]
 __global__ void pack_om_kernel(const float* __restrict__ off, const float* __restrict__ msk, float* __restrict__ om,
                                int B, int HW) {
@@ -138,6 +99,12 @@ struct TempPool {  // RAII device temporaries for the op-level hooks
     void* p = nullptr;
     YB_CHECK_CUDA(cudaMalloc(&p, std::max<size_t>(bytes, 256)));
     v.push_back(p);
+    return p;
+  }
+  void* put(const PackedWeights& pw) {   // a device copy of packed weights, in whichever element format they hold
+    const size_t bytes = pw.f.size() * 4 + pw.h.size() * 2;
+    void* p = get(bytes);
+    YB_CHECK_CUDA(cudaMemcpy(p, pw.f.empty() ? (const void*)pw.h.data() : pw.f.data(), bytes, cudaMemcpyHostToDevice));
     return p;
   }
   ~TempPool() {
@@ -556,18 +523,19 @@ int yb_dcn_forward(yb_handle* h, const float* d_input, const float* d_weight, co
   float* om = (float*)tp.get((size_t)B * Ho * Wo * 27 * 4);
   pack_om_kernel<<<grid1d((int64_t)B * Ho * Wo * 27), 256, 0, s>>>(d_offset, d_mask, om, B, Ho * Wo);
   YB_CHECK_LAUNCH();
-  const int64_t wn = (int64_t)Co * C * 9;
   const bool f16 = (h->cfg.precision != YB_PREC_F32);
   const int sp = (h->cfg.precision == YB_PREC_F16X3) ? 1 : 0;
   YB_REQUIRE(!sp || C % 64 == 0, "yb_dcn_forward: the split-precision mode needs C % 64 == 0");
   const int npl = sp ? 2 : 1;
+  // the weights are packed on the host (op-level hook, not the hot path)
+  std::vector<float> hw((size_t)Co * C * 9);
+  YB_CHECK_CUDA(cudaMemcpyAsync(hw.data(), d_weight, hw.size() * 4, cudaMemcpyDeviceToHost, s));
+  YB_CHECK_CUDA(cudaStreamSynchronize(s));
   if (!f16) {
     float* x = (float*)tp.get((size_t)B * H * W * C * 4);
     float* y = (float*)tp.get((size_t)B * Ho * Wo * Co * 4);
-    float* wk = (float*)tp.get((size_t)wn * 4);
+    const float* wk = (const float*)tp.put(pack_weights(hw.data(), Co, C, 3, 3, nullptr, WLayout::Simt, WFormat::F32));
     launch_nchw_f32_to_nhwc<float>(d_input, x, B, C, H, W, s, &h->lc);
-    pack_w_simt_kernel<float><<<grid1d(wn), 256, 0, s>>>(d_weight, wk, Co, C, 9);
-    YB_CHECK_LAUNCH();
     launch_dcn_simt<float>(x, om, wk, d_bias, y, B, H, W, C, Ho, Wo, Co, stride_h, pad_h, dilation_h, ACT_NONE, 0, s,
                            &h->lc);
     launch_nhwc_to_nchw_f32<float>(y, d_output, B, Ho, Wo, Co, s, &h->lc);
@@ -579,36 +547,18 @@ int yb_dcn_forward(yb_handle* h, const float* d_input, const float* d_weight, co
     __half* y = (__half*)tp.get((size_t)B * Ho * Wo * Cp * 2 * npl);
     launch_nchw_f32_to_nhwc<__half>(d_input, x, B, C, H, W, s, &h->lc, sp);
     if (C % 64 == 0) {
-      __half* wk = (__half*)tp.get((size_t)Cp * C * 9 * 2 * npl);
+      const PackedWeights pw =
+          pack_weights(hw.data(), Co, C, 3, 3, nullptr, WLayout::Dcn, sp ? WFormat::Split : WFormat::F16, 0, Cp);
+      const __half* wk = (const __half*)tp.put(pw);
       const float* bias = d_bias;
-      if (Cp > Co) {
-        YB_CHECK_CUDA(cudaMemsetAsync(wk, 0, (size_t)Cp * C * 9 * 2 * npl, s));
-        if (d_bias) {
-          float* bp = (float*)tp.get((size_t)Cp * 4);
-          YB_CHECK_CUDA(cudaMemsetAsync(bp, 0, (size_t)Cp * 4, s));
-          YB_CHECK_CUDA(cudaMemcpyAsync(bp, d_bias, (size_t)Co * 4, cudaMemcpyDeviceToDevice, s));
-          bias = bp;
-        }
+      if (Cp > Co && d_bias) {
+        float* bp = (float*)tp.get((size_t)Cp * 4);
+        YB_CHECK_CUDA(cudaMemsetAsync(bp, 0, (size_t)Cp * 4, s));
+        YB_CHECK_CUDA(cudaMemcpyAsync(bp, d_bias, (size_t)Co * 4, cudaMemcpyDeviceToDevice, s));
+        bias = bp;
       }
-      float out_scale = 1.f;
-      if (sp) {
-        // one power of two for the whole weight tensor: max |w| is read back (op-level hook, not the hot path)
-        std::vector<float> hw((size_t)wn);
-        YB_CHECK_CUDA(cudaMemcpyAsync(hw.data(), d_weight, (size_t)wn * 4, cudaMemcpyDeviceToHost, s));
-        YB_CHECK_CUDA(cudaStreamSynchronize(s));
-        float mx = 0.f;
-        for (float v : hw) mx = std::max(mx, fabsf(v));
-        int ex = 0;
-        if (mx > 0.f) frexpf(mx, &ex);
-        const int e = mx > 0.f ? std::max(-24, std::min(40, 14 - ex)) : 0;
-        out_scale = ldexpf(1.f, -e);
-        pack_w_dcn_tc_split_kernel<<<grid1d(wn), 256, 0, s>>>(d_weight, wk, Co, C, 9, ldexpf(1.f, e));
-      } else {
-        pack_w_dcn_tc_kernel<<<grid1d(wn), 256, 0, s>>>(d_weight, wk, Co, C, 9);
-      }
-      YB_CHECK_LAUNCH();
       DcnTcPlan* dp = dcn_tc_plan_create(x, om, wk, bias, y, B, H, W, C, Ho, Wo, Cp, stride_h, pad_h, dilation_h,
-                                         ACT_NONE, 0, sp, out_scale);
+                                         ACT_NONE, 0, sp, pw.out_scale);
       try {
         launch_dcn_tc(dp, s, &h->lc);
       } catch (...) {
@@ -617,9 +567,7 @@ int yb_dcn_forward(yb_handle* h, const float* d_input, const float* d_weight, co
       }
       dcn_tc_plan_destroy(dp);
     } else {
-      __half* wk = (__half*)tp.get((size_t)wn * 2);
-      pack_w_simt_kernel<__half><<<grid1d(wn), 256, 0, s>>>(d_weight, wk, Co, C, 9);
-      YB_CHECK_LAUNCH();
+      const __half* wk = (const __half*)tp.put(pack_weights(hw.data(), Co, C, 3, 3, nullptr, WLayout::Simt, WFormat::F16));
       launch_dcn_simt<__half>(x, om, wk, d_bias, y, B, H, W, C, Ho, Wo, Co, stride_h, pad_h, dilation_h, ACT_NONE, 0,
                               s, &h->lc);
     }
@@ -649,8 +597,6 @@ int yb_conv2d(yb_handle* h, const float* d_x, const float* h_w, const float* h_b
   const int Ho = (H + 2 * pad - kh) / stride + 1, Wo = (W + 2 * pad - kw) / stride + 1;
   YB_REQUIRE(Ho >= 1 && Wo >= 1, "yb_conv2d: empty output");
   TempPool tp;
-  const int taps = kh * kw;
-  const size_t K = (size_t)taps * Ci;
   const bool f16 = precision != 0;
   const size_t es = (f16 && !sp) ? 2 : 4;   // split: two halfs per element
   void* x = tp.get((size_t)B * H * W * Ci * es);
@@ -690,33 +636,13 @@ int yb_conv2d(yb_handle* h, const float* d_x, const float* h_w, const float* h_b
   }
   std::function<void()> run;
   TcConvPlan* plan = nullptr;
-  if (precision == 1 || precision == 3) {
-    YB_REQUIRE(tc_conv_supported(p), "yb_conv2d: shape not supported by the tensor-core kernel (Cin % 64, taps <= 9)");
-    std::vector<__half> pk(K * Co * (sp ? 2 : 1));
-    if (sp) {
-      float mx = 0.f;
-      for (size_t i = 0; i < K * Co; ++i) mx = std::max(mx, fabsf(h_w[i]));
-      int ex = 0;
-      if (mx > 0.f) frexpf(mx, &ex);
-      const int e = mx > 0.f ? std::max(-24, std::min(40, 14 - ex)) : 0;
-      const float up = ldexpf(1.f, e);
-      p.out_scale = ldexpf(1.f, -e);
-      for (int o = 0; o < Co; ++o)
-        for (int c = 0; c < Ci; ++c)
-          for (int t = 0; t < taps; ++t) {
-            const float vs = h_w[((size_t)o * Ci + c) * taps + t] * up;
-            const __half hi = __float2half_rn(vs);
-            const size_t idx = ((size_t)t * Co + o) * 2 * Ci + c;
-            pk[idx] = hi;
-            pk[idx + Ci] = __float2half_rn((vs - __half2float(hi)) * 2048.f);   // lo' = residual * 2^11 (common.cuh)
-          }
-    } else
-    for (int o = 0; o < Co; ++o)
-      for (int c = 0; c < Ci; ++c)
-        for (int t = 0; t < taps; ++t)
-          pk[((size_t)t * Co + o) * Ci + c] = __float2half_rn(h_w[((size_t)o * Ci + c) * taps + t]);
-    __half* wd = (__half*)tp.get(pk.size() * 2);
-    YB_CHECK_CUDA(cudaMemcpy(wd, pk.data(), pk.size() * 2, cudaMemcpyHostToDevice));
+  const bool tc = precision == 1 || precision == 3;
+  YB_REQUIRE(!tc || tc_conv_supported(p), "yb_conv2d: shape not supported by the tensor-core kernel (Cin % 64, taps <= 9)");
+  static const WFormat kFormat[4] = {WFormat::F32, WFormat::F16, WFormat::F16, WFormat::Split};
+  const PackedWeights pw = pack_weights(h_w, Co, Ci, kh, kw, nullptr, tc ? WLayout::Conv : WLayout::Simt, kFormat[precision]);
+  const void* wd = tp.put(pw);
+  p.out_scale = pw.out_scale;
+  if (tc) {
     {
       auto env = [](const char* name) {
         const char* v = getenv(name);
@@ -729,7 +655,7 @@ int yb_conv2d(yb_handle* h, const float* d_x, const float* h_w, const float* h_b
       want.mma_groups = env("YB_CONV2D_EPI");
       want.pdl_friendly = env("YB_CONV2D_PDL");   // PDL-friendly plan + programmatic dependent launch
       want.stream_k = env("YB_CONV2D_SK");
-      plan = tc_conv_plan_create(p, wd, want);
+      plan = tc_conv_plan_create(p, (const __half*)wd, want);
       if (want.pdl_friendly) tc_conv_plan_set_pdl(plan, 1);
       if (tc_conv_plan_tiling(plan).stream_k) {
         void* ws = tp.get(tc_conv_sk_workspace_bytes());
@@ -738,23 +664,8 @@ int yb_conv2d(yb_handle* h, const float* d_x, const float* h_w, const float* h_b
       }
     }
     run = [&]() { launch_tc_conv(plan, s, &h->lc); };
-  } else if (precision == 2) {
-    std::vector<__half> pk(K * Co);
-    for (int o = 0; o < Co; ++o)
-      for (int c = 0; c < Ci; ++c)
-        for (int t = 0; t < taps; ++t)
-          pk[((size_t)t * Ci + c) * Co + o] = __float2half_rn(h_w[((size_t)o * Ci + c) * taps + t]);
-    __half* wd = (__half*)tp.get(pk.size() * 2);
-    YB_CHECK_CUDA(cudaMemcpy(wd, pk.data(), pk.size() * 2, cudaMemcpyHostToDevice));
-    run = [&, wd]() { launch_simt_conv(p, wd, SIMT_F16, s, &h->lc); };
   } else {
-    std::vector<float> pk(K * Co);
-    for (int o = 0; o < Co; ++o)
-      for (int c = 0; c < Ci; ++c)
-        for (int t = 0; t < taps; ++t) pk[((size_t)t * Ci + c) * Co + o] = h_w[((size_t)o * Ci + c) * taps + t];
-    float* wd = (float*)tp.get(pk.size() * 4);
-    YB_CHECK_CUDA(cudaMemcpy(wd, pk.data(), pk.size() * 4, cudaMemcpyHostToDevice));
-    run = [&, wd]() { launch_simt_conv(p, wd, SIMT_F32, s, &h->lc); };
+    run = [&]() { launch_simt_conv(p, wd, precision == 2 ? SIMT_F16 : SIMT_F32, s, &h->lc); };
   }
   try {
     run();  // warm-up + result

@@ -56,14 +56,15 @@ struct DType<__half> {
 
 __device__ __forceinline__ float to_f32(float v) { return v; }
 __device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+// from_f32, lo_from_f32 and split_f32 are also the host weight packer's encoders (engine.cu pack_weights)
 template <typename T>
-__device__ __forceinline__ T from_f32(float v);
+__host__ __device__ __forceinline__ T from_f32(float v);
 template <>
-__device__ __forceinline__ float from_f32<float>(float v) {
+__host__ __device__ __forceinline__ float from_f32<float>(float v) {
   return v;
 }
 template <>
-__device__ __forceinline__ __half from_f32<__half>(float v) {
+__host__ __device__ __forceinline__ __half from_f32<__half>(float v) {
   // saturate instead of producing inf: fp16 max is 65504
   v = fminf(fmaxf(v, -65504.f), 65504.f);
   return __float2half_rn(v);
@@ -80,7 +81,7 @@ __device__ __forceinline__ __half from_f32<__half>(float v) {
 // fp16 exponent range.  A pixel of a split NHWC tensor is [hi(C) | lo'(C)], i.e. 2*C halfs.
 #define YB_LO_SCALE 2048.f
 #define YB_LO_INV 4.8828125e-4f   /* 2^-11 */
-__device__ __forceinline__ __half lo_from_f32(float r) { return __float2half_rn(r * YB_LO_SCALE); }
+__host__ __device__ __forceinline__ __half lo_from_f32(float r) { return __float2half_rn(r * YB_LO_SCALE); }
 __device__ __forceinline__ float lo_to_f32(__half h) { return __half2float(h) * YB_LO_INV; }
 __device__ __forceinline__ __half2 lo2_from_f32(float r0, float r1) {
   return __floats2half2_rn(r0 * YB_LO_SCALE, r1 * YB_LO_SCALE);
@@ -90,7 +91,7 @@ __device__ __forceinline__ float2 lo2_to_f32(__half2 h) {
   return make_float2(f.x * YB_LO_INV, f.y * YB_LO_INV);
 }
 // (hi saturates at +-65504; the residual of a saturated value is dropped)
-__device__ __forceinline__ void split_f32(float v, __half& hi, __half& lo) {
+__host__ __device__ __forceinline__ void split_f32(float v, __half& hi, __half& lo) {
   const float c = fminf(fmaxf(v, -65504.f), 65504.f);
   hi = __float2half_rn(c);
   lo = lo_from_f32(c - __half2float(hi));

@@ -229,8 +229,8 @@ struct NetBuilder {
     // in.C may be a zero-padded channel count (the tensor-core stem pads a 32-channel output to 64, see stem_tc)
     YB_REQUIRE(!tc || (in.C % 64 == 0 && !in.f32),
                ("conv " + key + ": the half-precision modes need fp16 inputs with Cin % 64 == 0").c_str());
-    ConvW& w = stem_tc ? h->get_conv(key, bn, /*want_tc=*/true, false, /*pack=*/2)
-                       : h->get_conv(key, bn, /*want_tc=*/tc, /*want_f32=*/!tc, 0,
+    ConvW& w = stem_tc ? h->get_conv(key, bn, /*want_tc=*/true, false, WLayout::Stem)
+                       : h->get_conv(key, bn, /*want_tc=*/tc, /*want_f32=*/!tc, WLayout::Conv,
                                      /*cin_pad=*/tc ? in.C : 0,
                                      // a half-precision output narrower than 64 channels (Darknet's first block: 32)
                                      // is written as zero-padded 64-channel pixels for the tensor-core conv that follows
@@ -348,7 +348,7 @@ struct NetBuilder {
   Act dcn(const std::string& key, const std::string& bn, const Act& in, int stride) {
     // conv_offset_mask: 3x3, same stride/pad, bias, 27 channels, fp32 output (dcn_v2.py:106-124)
     Act om = conv(key + ".conv_offset_mask", "", in, 3, stride, 1, ACT_NONE, nullptr, /*out_f32=*/true);
-    ConvW& w = h->get_conv(key, bn, /*want_tc=*/f16, /*want_f32=*/!f16, /*pack=*/1);
+    ConvW& w = h->get_conv(key, bn, /*want_tc=*/f16, /*want_f32=*/!f16, WLayout::Dcn);
     YB_REQUIRE(!f16 || dcn_tc_supported(in.C, w.Cout),
                ("dcn " + key + ": the half-precision modes need C % 64 == 0 and Cout % 8 == 0 (tensor-core DCN)").c_str());
     const int Ho = om.H, Wo = om.W;
@@ -898,21 +898,75 @@ int yb_handle::peek_cout(const std::string& conv_key) const {
   return (it == host.end() || it->second.shape.empty()) ? 0 : (int)it->second.shape[0];
 }
 
-// ---- split-precision weight packing (YB_PREC_F16X3) -----------------------------------------------------------------
-// w * 2^e = hi + lo with hi = rn_fp16(w * 2^e), lo = rn_fp16(w * 2^e - hi).  e puts the largest |w| of the layer
-// just below 2^14, so that hi never overflows and lo (<= 2^-11 |hi|) is a normal fp16 number for every weight larger
-// than 2^-17 of the layer's maximum; the kernels multiply the fp32 accumulator by 2^-e (exact).
+// ---- weight packing (engine.cuh pack_weights) -----------------------------------------------------------------------
+// Split precision: w * 2^e = hi + lo with hi = rn_fp16(w * 2^e), lo = rn_fp16(w * 2^e - hi).  e puts the largest |w|
+// of the tensor just below 2^14, so that hi never overflows and lo (<= 2^-11 |hi|) is a normal fp16 number for every
+// weight larger than 2^-17 of the tensor's maximum; the kernels multiply the fp32 accumulator by 2^-e (exact).
 static int split_exponent(float max_abs) {
   if (!(max_abs > 0.f) || !std::isfinite(max_abs)) return 0;
   int ex = 0;
   frexpf(max_abs, &ex);          // max_abs = m * 2^ex, m in [0.5, 1)
   return std::max(-24, std::min(40, 14 - ex));
 }
-static inline void split_pack(float v, float scale, __half* hi, __half* lo) {
-  const float vs = v * scale;
-  const __half h = __float2half_rn(vs);
-  *hi = h;
-  *lo = __float2half_rn((vs - __half2float(h)) * 2048.f);   // lo' = residual * 2^11 (common.cuh)
+
+PackedWeights yb::pack_weights(const float* w, int Co, int Ci, int KH, int KW, const float* co_scale, WLayout layout,
+                           WFormat fmt, int cin_pad, int cout_pad) {
+  const bool simt = layout == WLayout::Simt, split = fmt == WFormat::Split;
+  YB_REQUIRE(simt ? !split : fmt != WFormat::F32, "pack_weights: no kernel reads this layout in this format");
+  const int CiP = std::max(Ci, cin_pad), CoP = std::max(Co, cout_pad);
+  YB_REQUIRE(CiP == Ci || layout == WLayout::Conv, "pack_weights: only the conv layout pads input channels");
+  YB_REQUIRE(CoP == Co || layout == WLayout::Conv || layout == WLayout::Dcn,
+             "pack_weights: only the conv and DCN layouts pad output channels");
+  const int taps = KH * KW;
+  const size_t K = (size_t)taps * Ci;
+  auto value = [&](int o, size_t i) { return co_scale ? w[o * K + i] * co_scale[o] : w[o * K + i]; };   // i = c*taps + t
+  PackedWeights pw;
+  if (simt) {   // [tap*Cin + c][Cout]
+    if (fmt == WFormat::F32) pw.f.resize(K * Co);
+    else pw.h.resize(K * Co);
+    for (int o = 0; o < Co; ++o)
+      for (int c = 0; c < Ci; ++c)
+        for (int t = 0; t < taps; ++t) {
+          const size_t d = ((size_t)t * Ci + c) * Co + o;
+          const float v = value(o, (size_t)c * taps + t);
+          if (fmt == WFormat::F32) pw.f[d] = v;
+          else pw.h[d] = from_f32<__half>(v);
+        }
+    return pw;
+  }
+  float up = 1.f;
+  if (split) {   // one power of two for the whole tensor
+    float mx = 0.f;
+    for (int o = 0; o < Co; ++o)
+      for (size_t i = 0; i < K; ++i) mx = std::max(mx, fabsf(value(o, i)));
+    const int e = split_exponent(mx);
+    up = ldexpf(1.f, e);
+    pw.out_scale = ldexpf(1.f, -e);
+  }
+  // tensor-core layouts: rows of L halfs (split: of 2*L halfs, [hi(L) | lo(L)])
+  const size_t L = layout == WLayout::Conv ? (size_t)CiP : layout == WLayout::Dcn ? K : (size_t)stem_tc_kpad(KH);
+  const size_t rows = layout == WLayout::Conv ? (size_t)taps * CoP : layout == WLayout::Dcn ? (size_t)CoP : (size_t)Co;
+  YB_REQUIRE(layout != WLayout::Stem || K <= L, "pack_weights: too many stem input channels");
+  const size_t row_len = split ? 2 * L : L;
+  pw.h.assign(rows * row_len, __float2half_rn(0.f));
+  for (int o = 0; o < Co; ++o)
+    for (int c = 0; c < Ci; ++c)
+      for (int t = 0; t < taps; ++t) {
+        __half* d = layout == WLayout::Conv ? &pw.h[((size_t)t * CoP + o) * row_len + c]
+                    : layout == WLayout::Dcn ? &pw.h[o * row_len + (size_t)t * Ci + c]
+                                             : &pw.h[o * row_len + (size_t)c * taps + t];
+        const float v = value(o, (size_t)c * taps + t);
+        if (split) split_f32(v * up, d[0], d[L]);
+        else d[0] = from_f32<__half>(v);
+      }
+  return pw;
+}
+
+template <typename T>
+static T* upload(std::vector<void*>& pool, const std::vector<T>& v) {
+  T* d = (T*)dmalloc(pool, v.size() * sizeof(T));
+  YB_CHECK_CUDA(cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+  return d;
 }
 
 static const HostTensor& need(yb_handle* h, const std::string& name) {
@@ -922,13 +976,14 @@ static const HostTensor& need(yb_handle* h, const std::string& name) {
 }
 
 ConvW& yb_handle::get_conv(const std::string& conv_key, const std::string& bn_key, bool want_tc, bool want_f32,
-                           int pack, int cin_pad, int cout_pad) {
+                           WLayout tc_layout, int cin_pad, int cout_pad) {
   ConvW& cw = convs[conv_key];
   const HostTensor& w = need(this, conv_key + ".weight");
   YB_REQUIRE(w.shape.size() == 4, ("weight " + conv_key + " is not 4-D").c_str());
   const int Co = (int)w.shape[0], Ci = (int)w.shape[1], KH = (int)w.shape[2], KW = (int)w.shape[3];
-  const int CiP = (want_tc && pack == 0 && cin_pad > Ci) ? cin_pad : Ci;   // row length of the tensor-core packing
-  const int CoP = (want_tc && pack == 0 && cout_pad > Co) ? cout_pad : Co;  // rows of the tensor-core packing (zeros beyond Co)
+  const bool pad = want_tc && tc_layout == WLayout::Conv;
+  const int CiP = (pad && cin_pad > Ci) ? cin_pad : Ci;   // row length of the tensor-core packing
+  const int CoP = (pad && cout_pad > Co) ? cout_pad : Co;  // rows of the tensor-core packing (zeros beyond Co)
   if (cw.Cout == 0) {
     cw.cout_pad = CoP;
     cw.cin_pad = CiP;
@@ -936,7 +991,6 @@ ConvW& yb_handle::get_conv(const std::string& conv_key, const std::string& bn_ke
     cw.Cout = Co;
     cw.KH = KH;
     cw.KW = KW;
-    cw.pack = pack;
   }
   const bool has_bias = host.count(conv_key + ".bias") > 0;
   const bool has_bn = !bn_key.empty();
@@ -964,76 +1018,17 @@ ConvW& yb_handle::get_conv(const std::string& conv_key, const std::string& bn_ke
       shift[o] = be.data[o] + (shift[o] - mu.data[o]) * s;
     }
   }
-  const int taps = KH * KW;
-  const size_t K = (size_t)taps * Ci;
-  if (need_f32) {
-    std::vector<float> pk(K * Co);
-    for (int o = 0; o < Co; ++o)
-      for (int c = 0; c < Ci; ++c)
-        for (int t = 0; t < taps; ++t)
-          pk[((size_t)t * Ci + c) * Co + o] = w.data[((size_t)o * Ci + c) * taps + t] * scale[o];
-    cw.w_f32 = (float*)dmalloc(weight_allocs, pk.size() * 4);
-    YB_CHECK_CUDA(cudaMemcpy(cw.w_f32, pk.data(), pk.size() * 4, cudaMemcpyHostToDevice));
-  }
-  const bool split = (cfg.precision == YB_PREC_F16X3);
-  if (need_tc && split) {
-    float mx = 0.f;
-    for (int o = 0; o < Co; ++o)
-      for (size_t i = 0; i < (size_t)Ci * taps; ++i) mx = std::max(mx, fabsf(w.data[(size_t)o * Ci * taps + i] * scale[o]));
-    const int e = split_exponent(mx);
-    const float up = ldexpf(1.f, e);
-    cw.out_scale = ldexpf(1.f, -e);
-    const size_t kpad = (pack == 2) ? (size_t)stem_tc_kpad(KH) : (size_t)taps * CiP;   // plane length along K
-    std::vector<__half> pk(2 * kpad * CoP, __float2half_rn(0.f));
-    for (int o = 0; o < Co; ++o)
-      for (int c = 0; c < Ci; ++c)
-        for (int t = 0; t < taps; ++t) {
-          const float v = w.data[((size_t)o * Ci + c) * taps + t] * scale[o];
-          size_t hi;   // index of the hi half; lo lives one plane further
-          size_t plane;
-          if (pack == 2) {          // stem: [Cout][hi(Kpad) | lo(Kpad)], k = c*taps + t
-            hi = (size_t)o * 2 * kpad + (size_t)c * taps + t;
-            plane = kpad;
-          } else if (pack == 1) {   // DCN: [Cout][hi(9*Cin) | lo(9*Cin)], k = t*Cin + c
-            hi = (size_t)o * 2 * K + (size_t)t * Ci + c;
-            plane = K;
-          } else {                  // [tap][Cout][hi(CinP) | lo(CinP)]
-            hi = ((size_t)t * CoP + o) * 2 * CiP + c;
-            plane = (size_t)CiP;
-          }
-          split_pack(v, up, &pk[hi], &pk[hi + plane]);
-        }
-    cw.w_tc = (__half*)dmalloc(weight_allocs, pk.size() * 2);
-    YB_CHECK_CUDA(cudaMemcpy(cw.w_tc, pk.data(), pk.size() * 2, cudaMemcpyHostToDevice));
-  } else if (need_tc) {
-    std::vector<__half> pk((size_t)taps * CiP * CoP, __float2half_rn(0.f));
-    if (pack == 2) {
-      // stem: [Cout][Kpad], k = c*taps + t (the OIHW flattening), zero padded to a multiple of 64
-      const size_t kpad = (size_t)stem_tc_kpad(KH);
-      pk.assign(kpad * Co, __float2half_rn(0.f));
-      for (int o = 0; o < Co; ++o)
-        for (int c = 0; c < Ci; ++c)
-          for (int t = 0; t < taps; ++t)
-            pk[(size_t)o * kpad + (size_t)c * taps + t] = __float2half_rn(w.data[((size_t)o * Ci + c) * taps + t] * scale[o]);
-    } else if (pack == 1) {
-      // DCN: [Cout][tap*Cin + c], the K order of the fused kernel's gathered A stage
-      for (int o = 0; o < Co; ++o)
-        for (int c = 0; c < Ci; ++c)
-          for (int t = 0; t < taps; ++t)
-            pk[(size_t)o * K + (size_t)t * Ci + c] = __float2half_rn(w.data[((size_t)o * Ci + c) * taps + t] * scale[o]);
-    } else {
-      for (int o = 0; o < Co; ++o)
-        for (int c = 0; c < Ci; ++c)
-          for (int t = 0; t < taps; ++t)
-            pk[((size_t)t * CoP + o) * CiP + c] = __float2half_rn(w.data[((size_t)o * Ci + c) * taps + t] * scale[o]);
-    }
-    cw.w_tc = (__half*)dmalloc(weight_allocs, pk.size() * 2);
-    YB_CHECK_CUDA(cudaMemcpy(cw.w_tc, pk.data(), pk.size() * 2, cudaMemcpyHostToDevice));
+  if (need_f32)
+    cw.w_f32 = upload(weight_allocs, pack_weights(w.data.data(), Co, Ci, KH, KW, scale.data(), WLayout::Simt, WFormat::F32).f);
+  if (need_tc) {
+    const WFormat fmt = cfg.precision == YB_PREC_F16X3 ? WFormat::Split : WFormat::F16;
+    PackedWeights pw = pack_weights(w.data.data(), Co, Ci, KH, KW, scale.data(), tc_layout, fmt, CiP, CoP);
+    cw.w_tc = upload(weight_allocs, pw.h);
+    cw.out_scale = pw.out_scale;
   }
   if (!cw.bias && (has_bias || has_bn)) {
     shift.resize((size_t)std::max(Co, cw.cout_pad), 0.f);   // zero bias for the padding channels
-    cw.bias = (float*)dmalloc(weight_allocs, shift.size() * 4);
-    YB_CHECK_CUDA(cudaMemcpy(cw.bias, shift.data(), shift.size() * 4, cudaMemcpyHostToDevice));
+    cw.bias = upload(weight_allocs, shift);
   }
   return cw;
 }
@@ -1050,46 +1045,25 @@ ConvW& yb_handle::get_fused_head(const std::string& hn) {
     Ci = (int)w.shape[1];
     Co += (int)w.shape[0];
   }
-  const bool split = (cfg.precision == YB_PREC_F16X3);
-  const int npl = split ? 2 : 1;
-  std::vector<__half> pk((size_t)9 * Co * Ci * npl);
+  // the three heads' OIHW weights as one conv: one power-of-two scale for all of them (they share the accumulator tile)
+  std::vector<float> oihw;
   std::vector<float> bias(Co, 0.f);
-  float up = 1.f;
-  if (split) {   // one power-of-two scale for the three fused convs (they share the accumulator tile)
-    float mx = 0.f;
-    for (int i = 0; i < 3; ++i)
-      for (float v : need(this, hn + parts[i] + ".weight").data) mx = std::max(mx, fabsf(v));
-    const int e = split_exponent(mx);
-    up = ldexpf(1.f, e);
-    cw.out_scale = ldexpf(1.f, -e);
-  }
   int o0 = 0;
   for (int i = 0; i < 3; ++i) {
     const HostTensor& w = need(this, hn + parts[i] + ".weight");
-    const int co = (int)w.shape[0];
-    for (int o = 0; o < co; ++o)
-      for (int c = 0; c < Ci; ++c)
-        for (int t = 0; t < 9; ++t) {
-          const float v = w.data[((size_t)o * Ci + c) * 9 + t];
-          if (split) {
-            const size_t hi = ((size_t)t * Co + o0 + o) * 2 * Ci + c;
-            split_pack(v, up, &pk[hi], &pk[hi + Ci]);
-          } else {
-            pk[((size_t)t * Co + o0 + o) * Ci + c] = __float2half_rn(v);
-          }
-        }
+    oihw.insert(oihw.end(), w.data.begin(), w.data.end());
     auto it = host.find(hn + parts[i] + ".bias");
-    if (it != host.end())
-      for (int o = 0; o < co; ++o) bias[o0 + o] = it->second.data[o];
-    o0 += co;
+    if (it != host.end()) std::copy_n(it->second.data.begin(), w.shape[0], bias.begin() + o0);
+    o0 += (int)w.shape[0];
   }
+  const WFormat fmt = cfg.precision == YB_PREC_F16X3 ? WFormat::Split : WFormat::F16;
+  PackedWeights pw = pack_weights(oihw.data(), Co, Ci, 3, 3, nullptr, WLayout::Conv, fmt);
   cw.Cin = Ci;
   cw.Cout = Co;
   cw.KH = cw.KW = 3;
-  cw.w_tc = (__half*)dmalloc(weight_allocs, pk.size() * 2);
-  YB_CHECK_CUDA(cudaMemcpy(cw.w_tc, pk.data(), pk.size() * 2, cudaMemcpyHostToDevice));
-  cw.bias = (float*)dmalloc(weight_allocs, (size_t)Co * 4);
-  YB_CHECK_CUDA(cudaMemcpy(cw.bias, bias.data(), (size_t)Co * 4, cudaMemcpyHostToDevice));
+  cw.out_scale = pw.out_scale;
+  cw.w_tc = upload(weight_allocs, pw.h);
+  cw.bias = upload(weight_allocs, bias);
   return cw;
 }
 

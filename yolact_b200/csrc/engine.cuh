@@ -29,14 +29,32 @@ struct ConvW {
                              // then writes 64-channel pixels the next tensor-core conv can consume; 0 = Cout
   int cin_pad = 0;           // w_tc rows are padded with zeros to this many input channels (a multiple of 64) when the
                              // producer writes zero-padded pixels (Darknet: 32 -> 64); 0 = Cin
-  float* w_f32 = nullptr;    // [KH*KW*Cin][Cout]           (SIMT fp32)
-  __half* w_tc = nullptr;    // [KH*KW][Cout][Cin]          (tensor cores), or [1][Cout][9*Cin] for DCN
+  float* w_f32 = nullptr;    // WLayout::Simt, fp32
+  __half* w_tc = nullptr;    // WLayout::Conv, Dcn or Stem (tensor cores), fp16 or split pairs
   float* bias = nullptr;     // [Cout] or null
-  int pack = 0;              // 0 normal, 1 DCN ([Cout][9*Cin]), 2 stem ([Cout][Kpad], OIHW order)
-  // YB_PREC_F16X3: w_tc holds [..][hi(K) | lo(K)] fp16 pairs of w * 2^e (e chosen so that max |w| * 2^e < 2^15:
+  // YB_PREC_F16X3: w_tc holds [..][hi(K) | lo(K)] fp16 pairs of w * 2^e (e chosen so that max |w| * 2^e < 2^14:
   // the lo parts stay normal fp16 numbers); out_scale = 2^-e is applied to the fp32 accumulator
   float out_scale = 1.f;
 };
+
+// Weight packing: OIHW fp32 -> the layout and element format a kernel reads (K = taps*Cin, k = tap*Cin + c):
+//   Conv  [tap][CoutP][CinP]                                  (implicit-GEMM and chain kernels)
+//   Dcn   [CoutP][K], row index k                             (fused tensor-core DCN)
+//   Stem  [Cout][Kpad], row index c*taps + tap (OIHW order), Kpad = stem_tc_kpad(KH)   (tensor-core stem)
+//   Simt  [K][Cout], row k                                    (CUDA-core conv and DCN)
+// Conv, Dcn and Stem take F16 or Split, where each row of n values becomes [hi(n) | lo(n)]; Simt takes F32 or F16.
+// Other combinations are rejected.  CinP = max(Cin, cin_pad), CoutP = max(Cout, cout_pad); all padding is zeros.
+// co_scale (null = 1) multiplies output channel o first (folded BatchNorm).  Split: the pairs encode w * 2^e with one
+// exponent e over the whole tensor (engine.cu split_exponent), and out_scale = 2^-e.  Makes no CUDA calls.
+enum class WLayout { Conv, Dcn, Stem, Simt };
+enum class WFormat { F32, F16, Split };
+struct PackedWeights {
+  std::vector<__half> h;     // F16, Split
+  std::vector<float> f;      // F32
+  float out_scale = 1.f;
+};
+PackedWeights pack_weights(const float* oihw, int Co, int Ci, int KH, int KW, const float* co_scale, WLayout layout,
+                           WFormat fmt, int cin_pad = 0, int cout_pad = 0);
 
 // NHWC activation (element type float in YB_PREC_F32, __half in YB_PREC_F16TC unless f32 is set;
 // YB_PREC_F16X3: `split` -- every pixel is [hi(C) | lo(C)] halfs, value = hi + lo)
@@ -140,7 +158,7 @@ struct yb_handle {
 
   // ---- weights
   yb::ConvW& get_conv(const std::string& conv_key, const std::string& bn_key, bool want_tc, bool want_f32,
-                      int pack = 0, int cin_pad = 0, int cout_pad = 0);
+                      yb::WLayout tc_layout = yb::WLayout::Conv, int cin_pad = 0, int cout_pad = 0);
   int peek_cout(const std::string& conv_key) const;
   yb::ConvW& get_fused_head(const std::string& head_name);
   void finalize();
