@@ -79,29 +79,58 @@ __host__ __device__ __forceinline__ __half from_f32<__half>(float v) {
 // acc_hi + 2^-11 * acc_lo  in the epilogue.
 // Weights are additionally multiplied by a per-layer power of two (engine.cu split_exponent) so that hi uses the upper
 // fp16 exponent range.  A pixel of a split NHWC tensor is [hi(C) | lo'(C)], i.e. 2*C halfs.
+// The pair is encoded (split_f32, split2_from_f32) and decoded (split_to_f32, split2_to_f32) only here; the three MMA
+// passes and the accumulator combine are tc_common.cuh mma_passes and split_combine.
 #define YB_LO_SCALE 2048.f
 #define YB_LO_INV 4.8828125e-4f   /* 2^-11 */
 __host__ __device__ __forceinline__ __half lo_from_f32(float r) { return __float2half_rn(r * YB_LO_SCALE); }
-__device__ __forceinline__ float lo_to_f32(__half h) { return __half2float(h) * YB_LO_INV; }
-__device__ __forceinline__ __half2 lo2_from_f32(float r0, float r1) {
+__host__ __device__ __forceinline__ float lo_to_f32(__half h) { return __half2float(h) * YB_LO_INV; }
+__host__ __device__ __forceinline__ __half2 lo2_from_f32(float r0, float r1) {
   return __floats2half2_rn(r0 * YB_LO_SCALE, r1 * YB_LO_SCALE);
 }
-__device__ __forceinline__ float2 lo2_to_f32(__half2 h) {
+__host__ __device__ __forceinline__ float2 lo2_to_f32(__half2 h) {
   const float2 f = __half22float2(h);
   return make_float2(f.x * YB_LO_INV, f.y * YB_LO_INV);
 }
-// (hi saturates at +-65504; the residual of a saturated value is dropped)
+// saturating fp16 pair: +-65504 instead of inf
+__host__ __device__ __forceinline__ __half2 f16x2_from_f32(float a, float b) {
+  a = fminf(fmaxf(a, -65504.f), 65504.f);
+  b = fminf(fmaxf(b, -65504.f), 65504.f);
+  return __floats2half2_rn(a, b);
+}
+// (hi saturates at +-65504; the residual is taken against the clamped value, so a saturated element gets lo = 0 and
+// hi + lo stays finite)
 __host__ __device__ __forceinline__ void split_f32(float v, __half& hi, __half& lo) {
   const float c = fminf(fmaxf(v, -65504.f), 65504.f);
   hi = __float2half_rn(c);
   lo = lo_from_f32(c - __half2float(hi));
 }
+// split_f32 of two lanes
+__host__ __device__ __forceinline__ void split2_from_f32(float v0, float v1, __half2& hi, __half2& lo) {
+  hi = f16x2_from_f32(v0, v1);
+  const float2 hf = __half22float2(hi);
+  const float c0 = fminf(fmaxf(v0, -65504.f), 65504.f), c1 = fminf(fmaxf(v1, -65504.f), 65504.f);
+  lo = lo2_from_f32(c0 - hf.x, c1 - hf.y);
+}
+__host__ __device__ __forceinline__ float split_to_f32(__half hi, __half lo) { return __half2float(hi) + lo_to_f32(lo); }
+__host__ __device__ __forceinline__ float2 split2_to_f32(__half2 hi, __half2 lo) {
+  const float2 h = __half22float2(hi), l = lo2_to_f32(lo);
+  return make_float2(h.x + l.x, h.y + l.y);
+}
 
+// activation with a compile-time selector: the epilogue loops use it directly, a runtime selector goes through apply_act
+template <int ACT>
+__device__ __forceinline__ float act_t(float v) {
+  if (ACT == ACT_RELU) return fmaxf(v, 0.f);
+  if (ACT == ACT_LEAKY) return v > 0.f ? v : 0.1f * v;
+  if (ACT == ACT_TANH) return tanhf(v);
+  return v;
+}
 __device__ __forceinline__ float apply_act(float v, int act) {
   switch (act) {
-    case ACT_RELU: return fmaxf(v, 0.f);
-    case ACT_TANH: return tanhf(v);
-    case ACT_LEAKY: return v > 0.f ? v : 0.1f * v;
+    case ACT_RELU: return act_t<ACT_RELU>(v);
+    case ACT_TANH: return act_t<ACT_TANH>(v);
+    case ACT_LEAKY: return act_t<ACT_LEAKY>(v);
     default: return v;
   }
 }

@@ -50,15 +50,6 @@ struct alignas(64) DcnParams {
   float out_scale;
 };
 
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ uint4 ldg_nc16(const void* p) {
-  uint4 r;
-  asm volatile("ld.global.nc.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
-  return r;
-}
-
 template <int BN, bool SPLIT>
 __global__ void __launch_bounds__(DTHREADS)
 dcn_tc_kernel(const __grid_constant__ DcnParams p) {
@@ -213,9 +204,7 @@ dcn_tc_kernel(const __grid_constant__ DcnParams p) {
 #pragma unroll
             for (int j = 0; j < 4; ++j) o2[j] = (c == 0) ? __hmul2(w2, v2[j]) : __hfma2(w2, v2[j], o2[j]);
           }
-          const int row = gw * 16 + 4 * i + src_sub;
-          const uint32_t off = (uint32_t)row * 128u + (((uint32_t)piece ^ ((uint32_t)row & 7u)) << 4);
-          *reinterpret_cast<uint4*>(sa + off) = oh;
+          *reinterpret_cast<uint4*>(sa + sw128_off(gw * 16 + 4 * i + src_sub, piece)) = oh;
         }
       } else {
 #pragma unroll
@@ -235,17 +224,17 @@ dcn_tc_kernel(const __grid_constant__ DcnParams p) {
             float r0 = 0.f, r1 = 0.f;
 #pragma unroll
             for (int c = 0; c < 4; ++c) {
-              const float2 fh = __half22float2(reinterpret_cast<const __half2*>(&rh[c])[j]);
-              const float2 fl = lo2_to_f32(reinterpret_cast<const __half2*>(&rl[c])[j]);
-              r0 = __fmaf_rn(aw[i][c], fh.x + fl.x, r0);
-              r1 = __fmaf_rn(aw[i][c], fh.y + fl.y, r1);
+              const float2 f = split2_to_f32(reinterpret_cast<const __half2*>(&rh[c])[j], reinterpret_cast<const __half2*>(&rl[c])[j]);
+              r0 = __fmaf_rn(aw[i][c], f.x, r0);
+              r1 = __fmaf_rn(aw[i][c], f.y, r1);
             }
-            oh2[j] = __floats2half2_rn(r0, r1);   // |sample| <= max |x|: no saturation needed
+            // split2_from_f32 without its clamp (two min/max per element in an issue-bound gather): with sigmoid masks,
+            // as in the network, |sample| <= max |x| <= 65504
+            oh2[j] = __floats2half2_rn(r0, r1);
             const float2 hf = __half22float2(oh2[j]);
             ol2[j] = lo2_from_f32(r0 - hf.x, r1 - hf.y);
           }
-          const int row = gw * 16 + 4 * i + src_sub;
-          const uint32_t off = (uint32_t)row * 128u + (((uint32_t)piece ^ ((uint32_t)row & 7u)) << 4);
+          const uint32_t off = sw128_off(gw * 16 + 4 * i + src_sub, piece);
           *reinterpret_cast<uint4*>(sa + off) = oh;
           *reinterpret_cast<uint4*>(sa + A_TILE + off) = ol;
         }
@@ -256,19 +245,11 @@ dcn_tc_kernel(const __grid_constant__ DcnParams p) {
       {
         const uint32_t sa32 = smem_u32(sa) + (uint32_t)wgi * (64u * 128u);
         const uint32_t sb32 = smem_u32(sa) + (uint32_t)(NPL * A_TILE);
-        const uint64_t da = make_sw128_desc(sa32), db = make_sw128_desc(sb32);
         wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < DK / 16; ++k) Wgmma<BN>::mma(acc[0], da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1u);
-        if (SPLIT) {
-          const uint64_t dal = make_sw128_desc(sa32 + A_TILE), dbl = make_sw128_desc(sb32 + B_PLANE);
-#pragma unroll
-          for (int k = 0; k < DK / 16; ++k)   // A_lo * W_hi -> second accumulator
-            Wgmma<BN>::mma(acc[NPL - 1], dal + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1u);
-#pragma unroll
-          for (int k = 0; k < DK / 16; ++k)   // A_hi * W_lo -> second accumulator
-            Wgmma<BN>::mma(acc[NPL - 1], da + (uint64_t)(2 * k), dbl + (uint64_t)(2 * k), 1u);
-        }
+        mma_passes<BN, DK / 16, SPLIT>(
+            acc[0], acc[NPL - 1],
+            [&](int pl, int k) { return make_sw128_desc(sa32 + (uint32_t)(pl * A_TILE)) + (uint64_t)(2 * k); },
+            [&](int pl, int k) { return make_sw128_desc(sb32 + (uint32_t)(pl * B_PLANE)) + (uint64_t)(2 * k); });
         wgmma_commit();
       }
       if (kb > 0) {   // k-block kb - 1 has been read: its weight tile can be refilled
@@ -294,20 +275,15 @@ dcn_tc_kernel(const __grid_constant__ DcnParams p) {
         const int col = 8 * j + 2 * (lane & 3);
         const int ch = n0 + col;
         const int i = 4 * j + 2 * hh;
-        float v0 = acc[0][i], v1 = acc[0][i + 1];
-        if (SPLIT) {
-          v0 = __fmaf_rn(acc[NPL - 1][i], YB_LO_INV, v0) * p.out_scale;
-          v1 = __fmaf_rn(acc[NPL - 1][i + 1], YB_LO_INV, v1) * p.out_scale;
-        }
-        v0 = apply_act(v0 + (p.bias ? __ldg(p.bias + ch) : 0.f), p.act);
-        v1 = apply_act(v1 + (p.bias ? __ldg(p.bias + ch + 1) : 0.f), p.act);
-        const float c0 = fminf(fmaxf(v0, -65504.f), 65504.f), c1 = fminf(fmaxf(v1, -65504.f), 65504.f);
-        const __half2 o = __floats2half2_rn(c0, c1);
-        *reinterpret_cast<__half2*>(yrow + col) = o;
-        if (SPLIT) {
-          const float2 hf = __half22float2(o);
-          *reinterpret_cast<__half2*>(yrow + p.Cout + col) = lo2_from_f32(c0 - hf.x, c1 - hf.y);
-        }
+        const float a0 = SPLIT ? split_combine(acc[0][i], acc[NPL - 1][i]) : acc[0][i];
+        const float a1 = SPLIT ? split_combine(acc[0][i + 1], acc[NPL - 1][i + 1]) : acc[0][i + 1];
+        const float v0 = apply_act(scale_bias<SPLIT>(a0, p.out_scale, p.bias ? __ldg(p.bias + ch) : 0.f), p.act);
+        const float v1 = apply_act(scale_bias<SPLIT>(a1, p.out_scale, p.bias ? __ldg(p.bias + ch + 1) : 0.f), p.act);
+        __half2 hi, lo;
+        if (SPLIT) split2_from_f32(v0, v1, hi, lo);
+        else hi = f16x2_from_f32(v0, v1);
+        *reinterpret_cast<__half2*>(yrow + col) = hi;
+        if (SPLIT) *reinterpret_cast<__half2*>(yrow + p.Cout + col) = lo;
       }
     }
   }

@@ -46,53 +46,41 @@ __device__ __forceinline__ uint4 pack<__half>(const float* f) {
   return r;
 }
 
-// lo-plane element access for the scalar layout kernels (split tensors exist for T = __half only)
-__device__ __forceinline__ float lo_of(float) { return 0.f; }
-__device__ __forceinline__ float lo_of(__half h) { return lo_to_f32(h); }
-template <typename T>
-__device__ __forceinline__ T lo_make(float r);
-template <>
-__device__ __forceinline__ float lo_make<float>(float r) {
-  return r;
-}
-template <>
-__device__ __forceinline__ __half lo_make<__half>(float r) {
-  return lo_from_f32(r);
-}
-
 // One 16-byte channel vector of a pixel -> floats.  `px` points at the pixel's first element; split (fp16 only):
 // the pixel is [hi(C) | lo(C)] and the value is hi + lo (YB_PREC_F16X3).
 template <typename T>
 __device__ __forceinline__ void load_vec(const T* px, int C, int cv, int split, float* f) {
   constexpr int V = DType<T>::kVec;
-  unpack<T>(*reinterpret_cast<const uint4*>(px + cv * V), f);
-  if (sizeof(T) == 2 && split) {   // lo plane: residual * 2^11
-    const uint4 rl = *reinterpret_cast<const uint4*>(px + C + cv * V);
-    const __half2* l2 = reinterpret_cast<const __half2*>(&rl);
+  const uint4 rh = *reinterpret_cast<const uint4*>(px + cv * V);
+  if constexpr (sizeof(T) == 2) {
+    if (split) {
+      const uint4 rl = *reinterpret_cast<const uint4*>(px + C + cv * V);
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 t = lo2_to_f32(l2[j]);
-      f[(2 * j) % V] += t.x;
-      f[(2 * j + 1) % V] += t.y;
+      for (int j = 0; j < 4; ++j) {
+        const float2 t = split2_to_f32(reinterpret_cast<const __half2*>(&rh)[j], reinterpret_cast<const __half2*>(&rl)[j]);
+        f[2 * j] = t.x;
+        f[2 * j + 1] = t.y;
+      }
+      return;
     }
   }
+  unpack<T>(rh, f);
 }
 template <typename T>
 __device__ __forceinline__ void store_vec(T* px, int C, int cv, int split, const float* f) {
   constexpr int V = DType<T>::kVec;
-  const uint4 hi = pack<T>(f);
-  *reinterpret_cast<uint4*>(px + cv * V) = hi;
-  if (sizeof(T) == 2 && split) {
-    float h[V], l[8];
-    unpack<T>(hi, h);
+  if constexpr (sizeof(T) == 2) {
+    if (split) {
+      uint4 hi, lo;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) l[j] = fabsf(f[j % V]) > 65504.f ? 0.f : f[j % V] - h[j % V];
-    uint4 lo;
-    __half2* l2 = reinterpret_cast<__half2*>(&lo);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) l2[j] = lo2_from_f32(l[2 * j], l[2 * j + 1]);
-    *reinterpret_cast<uint4*>(px + C + cv * V) = lo;
+      for (int j = 0; j < 4; ++j)
+        split2_from_f32(f[2 * j], f[2 * j + 1], reinterpret_cast<__half2*>(&hi)[j], reinterpret_cast<__half2*>(&lo)[j]);
+      *reinterpret_cast<uint4*>(px + cv * V) = hi;
+      *reinterpret_cast<uint4*>(px + C + cv * V) = lo;
+      return;
+    }
   }
+  *reinterpret_cast<uint4*>(px + cv * V) = pack<T>(f);
 }
 
 // ---- 3x3/s2/p1 max pool (backbone.py:80).  Padding acts as -inf (PyTorch semantics). ----------
@@ -194,8 +182,11 @@ __global__ void nhwc_to_nchw_kernel(const T* __restrict__ x, float* __restrict__
     int p = p0 + i, c = c0 + threadIdx.x;
     float v = 0.f;
     if (p < HW && c < C) {
-      v = to_f32(xb[(int64_t)p * PS + c]);
-      if (split) v += lo_of(xb[(int64_t)p * PS + C + c]);
+      const T* px = xb + (int64_t)p * PS;
+      v = to_f32(px[c]);
+      if constexpr (sizeof(T) == 2) {   // split pairs are fp16 only
+        if (split) v = split_to_f32(px[c], px[C + c]);
+      }
     }
     tile[i][threadIdx.x] = v;
   }
@@ -223,9 +214,13 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, T* __restrict__
     int p = p0 + i, c = c0 + threadIdx.x;
     if (c < C && p < HW) {
       const float v = tile[threadIdx.x][i];
-      const T hi = from_f32<T>(v);
-      yb_[(int64_t)p * PS + c] = hi;
-      if (split) yb_[(int64_t)p * PS + C + c] = lo_make<T>(fabsf(v) > 65504.f ? 0.f : v - to_f32(hi));
+      T* px = yb_ + (int64_t)p * PS;
+      if constexpr (sizeof(T) == 2) {   // split pairs are fp16 only
+        if (split) split_f32(v, px[c], px[C + c]);
+        else px[c] = from_f32<T>(v);
+      } else {
+        px[c] = v;
+      }
     }
   }
 }

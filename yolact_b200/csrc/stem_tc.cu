@@ -84,7 +84,6 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
     }
     const size_t plane = (size_t)p.H * p.W;
     const float* xb = p.x + (size_t)b * 3 * plane + (long long)hb * p.W + wb;  // may point before the frame: guarded
-    const uint32_t sw = (uint32_t)(row & 7);
 #pragma unroll
     for (int kg = 0; kg < ATOMS * 8; ++kg) {
       if (WG > 1 && (kg % WG) != wg) continue;   // warp-uniform
@@ -104,14 +103,11 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
           }
           v[e] = val;
         }
-        h2[j2] = __halves2half2(from_f32<__half>(v[0]), from_f32<__half>(v[1]));
-        if (SPLIT) {
-          const float2 hf = __half22float2(h2[j2]);
-          l2[j2] = lo2_from_f32(fabsf(v[0]) > 65504.f ? 0.f : v[0] - hf.x, fabsf(v[1]) > 65504.f ? 0.f : v[1] - hf.y);   // lo' = residual * 2^11
-        }
+        if (SPLIT) split2_from_f32(v[0], v[1], h2[j2], l2[j2]);
+        else h2[j2] = __halves2half2(from_f32<__half>(v[0]), from_f32<__half>(v[1]));
       }
       const int atom = kg >> 3;
-      const uint32_t aoff = row * 128 + ((((uint32_t)kg & 7u) ^ sw) << 4);
+      const uint32_t aoff = sw128_off(row, kg & 7);
       *reinterpret_cast<uint4*>(sA + atom * A_ATOM_BYTES + aoff) = pk;
       if (SPLIT) *reinterpret_cast<uint4*>(sA + (ATOMS + atom) * A_ATOM_BYTES + aoff) = pkl;
     }
@@ -135,18 +131,14 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
 #pragma unroll
       for (int i = 0; i < COUT / 2; ++i) acc[pl][i] = 0.f;
     wgmma_fence();
-#pragma unroll
-    for (int pass = 0; pass < (SPLIT ? 3 : 1); ++pass) {
-      const int pa = (pass == 1) ? 1 : 0, pb = (pass == 2) ? 1 : 0;   // hi*hi, lo*hi, hi*lo
-#pragma unroll
-      for (int j = 0; j < KSTEPS; ++j) {
-        const int atom = j >> 2, kk = j & 3;
-        const uint64_t da = make_sw128_desc(smem_u32(sA + (pa * ATOMS + atom) * A_ATOM_BYTES + h * 64 * 128)) + (uint64_t)(2 * kk);
-        const uint64_t db = make_sw128_desc(smem_u32(sB + (pb * ATOMS + atom) * B_ATOM_BYTES)) + (uint64_t)(2 * kk);
-        // hi*hi -> accumulator 0; lo*hi and hi*lo -> accumulator 1, see common.cuh
-        Wgmma<COUT>::mma(acc[pass > 0 ? NPL - 1 : 0], da, db, 1u);
-      }
-    }
+    mma_passes<COUT, KSTEPS, SPLIT>(
+        acc[0], acc[NPL - 1],
+        [&](int pl, int j) {
+          return make_sw128_desc(smem_u32(sA + (pl * ATOMS + (j >> 2)) * A_ATOM_BYTES + h * 64 * 128)) + (uint64_t)(2 * (j & 3));
+        },
+        [&](int pl, int j) {
+          return make_sw128_desc(smem_u32(sB + (pl * ATOMS + (j >> 2)) * B_ATOM_BYTES)) + (uint64_t)(2 * (j & 3));
+        });
     wgmma_commit();
     wgmma_wait<0>();
 #pragma unroll
@@ -161,20 +153,15 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
       for (int j = 0; j < COUT / 8; ++j) {
         const int col = 8 * j + 2 * (lane & 3);
         const int i = 4 * j + 2 * hh;
-        float v0 = acc[0][i], v1 = acc[0][i + 1];
-        if (SPLIT) {
-          v0 = __fmaf_rn(acc[NPL - 1][i], YB_LO_INV, v0) * p.out_scale;
-          v1 = __fmaf_rn(acc[NPL - 1][i + 1], YB_LO_INV, v1) * p.out_scale;
-        }
-        v0 = apply_act(v0 + (p.bias ? __ldg(p.bias + col) : 0.f), p.act);
-        v1 = apply_act(v1 + (p.bias ? __ldg(p.bias + col + 1) : 0.f), p.act);
-        const __half2 o = __halves2half2(from_f32<__half>(v0), from_f32<__half>(v1));
-        *reinterpret_cast<__half2*>(yrow + col) = o;
-        if (SPLIT) {
-          const float2 hf = __half22float2(o);
-          *reinterpret_cast<__half2*>(yrow + p.cpad + col) =
-              lo2_from_f32(fabsf(v0) > 65504.f ? 0.f : v0 - hf.x, fabsf(v1) > 65504.f ? 0.f : v1 - hf.y);   // lo' = residual * 2^11
-        }
+        const float a0 = SPLIT ? split_combine(acc[0][i], acc[NPL - 1][i]) : acc[0][i];
+        const float a1 = SPLIT ? split_combine(acc[0][i + 1], acc[NPL - 1][i + 1]) : acc[0][i + 1];
+        const float v0 = apply_act(scale_bias<SPLIT>(a0, p.out_scale, p.bias ? __ldg(p.bias + col) : 0.f), p.act);
+        const float v1 = apply_act(scale_bias<SPLIT>(a1, p.out_scale, p.bias ? __ldg(p.bias + col + 1) : 0.f), p.act);
+        __half2 hi, lo;
+        if (SPLIT) split2_from_f32(v0, v1, hi, lo);
+        else hi = __halves2half2(from_f32<__half>(v0), from_f32<__half>(v1));
+        *reinterpret_cast<__half2*>(yrow + col) = hi;
+        if (SPLIT) *reinterpret_cast<__half2*>(yrow + p.cpad + col) = lo;
       }
     }
   }

@@ -33,6 +33,22 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t addr, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
+__device__ __forceinline__ bool mbar_test_wait(uint32_t addr, uint32_t parity) {   // non-blocking
+  uint32_t ok;
+  asm volatile(
+      "{\n\t"
+      ".reg .pred P1;\n\t"
+      "mbarrier.test_wait.parity.shared::cta.b64 P1, [%1], %2;\n\t"
+      "selp.u32 %0, 1, 0, P1;\n\t"
+      "}"
+      : "=r"(ok)
+      : "r"(addr), "r"(parity)
+      : "memory");
+  return ok != 0;
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 // Blocking wait.  Build with -DYB_WATCHDOG during kernel development: a protocol bug then surfaces as a
 // launch failure (trap after ~2 s) instead of a hung GPU.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
@@ -81,7 +97,30 @@ template <int N>
 __device__ __forceinline__ void bulk_wait_read() {
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
+// ---- global-memory flags and counters shared between CTAs (stream-K partials, chain dependencies)
+__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
+  int v;
+  asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release_gpu(int* p, int v) {
+  asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ void st_relaxed_gpu(int* p, int v) {
+  asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ void red_release_gpu_add(int* p, int v) {
+  asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+// 16-byte read-only load through the non-coherent path
+__device__ __forceinline__ uint4 ldg_nc16(const void* p) {
+  uint4 r;
+  asm volatile("ld.global.nc.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
+  return r;
+}
 // ---- clusters: a CTA pair (cluster of two) shares one weight tile, each CTA loading half of it with a multicast TMA
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
@@ -252,6 +291,36 @@ __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
   d |= (uint64_t)(1024 >> 4) << 32;
   d |= (uint64_t)1 << 62;
   return d;
+}
+// byte offset of 16-byte chunk `chunk` (0..7) of row `row` in such a tile (128-byte rows, 128B swizzle)
+__device__ __forceinline__ uint32_t sw128_off(uint32_t row, uint32_t chunk) {
+  return row * 128u + ((chunk ^ (row & 7u)) << 4);
+}
+
+// The MMA passes of KSTEPS k16 steps, pass-major: A_hi*W_hi into acc_hi; SPLIT (YB_PREC_F16X3, common.cuh) then adds
+// A_lo*W_hi and A_hi*W_lo into acc_lo (the lo*lo term is below fp32 resolution).  da(plane, step) and db(plane, step)
+// return the operand descriptors of a step.
+template <int N, int KSTEPS, bool SPLIT, typename DescA, typename DescB>
+__device__ __forceinline__ void mma_passes(float* acc_hi, float* acc_lo, DescA da, DescB db) {
+  auto pass = [&](float* acc, int pa, int pb) {
+#pragma unroll
+    for (int k = 0; k < KSTEPS; ++k) {
+      const uint64_t a = da(pa, k);   // (A before B: a fixed evaluation order keeps the instruction schedule stable)
+      Wgmma<N>::mma(acc, a, db(pb, k), 1u);
+    }
+  };
+  pass(acc_hi, 0, 0);
+  if (SPLIT) {
+    pass(acc_lo, 1, 0);
+    pass(acc_lo, 0, 1);
+  }
+}
+// the two accumulators of a split result: acc_hi + 2^-11 * acc_lo
+__device__ __forceinline__ float split_combine(float acc_hi, float acc_lo) { return __fmaf_rn(acc_lo, YB_LO_INV, acc_hi); }
+// accumulator -> pre-activation value: SPLIT weights are scaled by 1 / out_scale, which the accumulator undoes
+template <bool SPLIT>
+__device__ __forceinline__ float scale_bias(float acc, float out_scale, float bias) {
+  return SPLIT ? __fmaf_rn(acc, out_scale, bias) : acc + bias;
 }
 
 

@@ -98,30 +98,11 @@ struct alignas(64) TcParams {
 // Warpgroup 0 is the TMA producer (one thread issues), warpgroups 1..H are the MMA warpgroups: each owns 2/H of the
 // tile's two 64-row halves, accumulates them with wgmma in registers and runs the epilogue of its rows.  The producer
 // runs up to `stages` k-blocks ahead across tile boundaries, so the loads of tile i+1 overlap the epilogue of tile i.
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
 __device__ __forceinline__ void mma_bar_sync(int nthreads) { asm volatile("bar.sync 1, %0;" ::"r"(nthreads) : "memory"); }
 
-// activation with a compile-time selector (the generic apply_act() is a runtime switch: far too
-// expensive inside the epilogue loops)
-template <int ACT>
-__device__ __forceinline__ float act_t(float v) {
-  if (ACT == ACT_RELU) return fmaxf(v, 0.f);
-  if (ACT == ACT_LEAKY) return v > 0.f ? v : 0.1f * v;
-  if (ACT == ACT_TANH) return tanhf(v);
-  return v;
-}
-__device__ __forceinline__ __half2 pack_sat(float a, float b) {
-  // saturate to the fp16 range instead of producing inf
-  a = fminf(fmaxf(a, -65504.f), 65504.f);
-  b = fminf(fmaxf(b, -65504.f), 65504.f);
-  return __floats2half2_rn(a, b);
-}
-
-// The k-blocks [k0, k1) of one tile: acc[mh][plane] of 64-row half (cw + mh * H) of the tile.  SPLIT: A_hi*W_hi into
-// plane 0, A_lo*W_hi + A_hi*W_lo into plane 1 (combined as acc0 + 2^-11 * acc1 by the caller; the lo*lo term is below
-// fp32 resolution).  Each stage is handed back to the producer(s) once the wgmmas that read it have completed.
+// The k-blocks [k0, k1) of one tile: acc[mh][plane] of 64-row half (cw + mh * H) of the tile (mma_passes; SPLIT: the
+// planes are combined into plane 0 at the end).  Each stage is handed back to the producer(s) once the wgmmas that
+// read it have completed.
 template <int BN, int MH, int H, bool SPLIT, bool PAIR, int NACC>
 __device__ __forceinline__ void mma_tile(float (&acc)[MH][SPLIT ? 2 : 1][NACC], uint8_t* smem, uint64_t* full_bar,
                                          uint64_t* empty_bar, int stages, int stage_bytes, int a_bytes, int b_plane_bytes,
@@ -151,20 +132,10 @@ __device__ __forceinline__ void mma_tile(float (&acc)[MH][SPLIT ? 2 : 1][NACC], 
 #pragma unroll
     for (int mh = 0; mh < MH; ++mh) {
       const uint32_t half_off = (uint32_t)(cw + mh * H) * (64u * 128u);
-      const uint64_t da = make_sw128_desc(sa + half_off);
-      const uint64_t db = make_sw128_desc(sb);
-#pragma unroll
-      for (int k = 0; k < BLOCK_K / 16; ++k) Wgmma<BN>::mma(acc[mh][0], da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1u);
-      if (SPLIT) {
-        const uint64_t dal = make_sw128_desc(sa + (uint32_t)A_STAGE_BYTES + half_off);
-        const uint64_t dbl = make_sw128_desc(sb + (uint32_t)b_plane_bytes);
-#pragma unroll
-        for (int k = 0; k < BLOCK_K / 16; ++k)
-          Wgmma<BN>::mma(acc[mh][NPL - 1], dal + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1u);
-#pragma unroll
-        for (int k = 0; k < BLOCK_K / 16; ++k)
-          Wgmma<BN>::mma(acc[mh][NPL - 1], da + (uint64_t)(2 * k), dbl + (uint64_t)(2 * k), 1u);
-      }
+      mma_passes<BN, BLOCK_K / 16, SPLIT>(
+          acc[mh][0], acc[mh][NPL - 1],
+          [&](int pl, int k) { return make_sw128_desc(sa + (uint32_t)(pl * A_STAGE_BYTES) + half_off) + (uint64_t)(2 * k); },
+          [&](int pl, int k) { return make_sw128_desc(sb + (uint32_t)(pl * b_plane_bytes)) + (uint64_t)(2 * k); });
     }
     wgmma_commit();
     if (stages == 1) {   // a single stage: the next k-block can only land once these wgmmas have read this one
@@ -185,7 +156,7 @@ __device__ __forceinline__ void mma_tile(float (&acc)[MH][SPLIT ? 2 : 1][NACC], 
 #pragma unroll
     for (int mh = 0; mh < MH; ++mh)
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[mh][0][i] = __fmaf_rn(acc[mh][NPL - 1][i], YB_LO_INV, acc[mh][0][i]);
+      for (int i = 0; i < BN / 2; ++i) acc[mh][0][i] = split_combine(acc[mh][0][i], acc[mh][NPL - 1][i]);
   }
 }
 
@@ -248,13 +219,13 @@ __device__ __forceinline__ void epi_staged(float (&acc)[MH][SPLIT ? 2 : 1][NACC]
         for (int h = 0; h < 2; ++h) {
           const int row = (cw + mh * H) * 64 + wq * 16 + (lane >> 2) + 8 * h;
           const int i = (c * 8 + j) * 4 + 2 * h;
-          float v0 = SPLIT ? __fmaf_rn(acc[mh][0][i], e.out_scale, b0) : acc[mh][0][i] + b0;
-          float v1 = SPLIT ? __fmaf_rn(acc[mh][0][i + 1], e.out_scale, b1) : acc[mh][0][i + 1] + b1;
+          float v0 = scale_bias<SPLIT>(acc[mh][0][i], e.out_scale, b0);
+          float v1 = scale_bias<SPLIT>(acc[mh][0][i + 1], e.out_scale, b1);
           if (RES_AFTER) {
             v0 = act_t<ACT>(v0);
             v1 = act_t<ACT>(v1);
           }
-          const uint32_t off = (uint32_t)row * 128u + ((((uint32_t)j) ^ ((uint32_t)row & 7u)) << 4) + (uint32_t)(lane & 3) * 4u;
+          const uint32_t off = sw128_off((uint32_t)row, (uint32_t)j) + (uint32_t)(lane & 3) * 4u;
           if (has_res_tile || e.res_g) {
             __half2 rh, rl;
             if (has_res_tile) {
@@ -271,11 +242,12 @@ __device__ __forceinline__ void epi_staged(float (&acc)[MH][SPLIT ? 2 : 1][NACC]
             } else {
               rh = rl = __floats2half2_rn(0.f, 0.f);
             }
+            // one plane at a time, (v + hi) + lo: v + split2_to_f32(rh, rl) rounds differently
             const float2 f = __half22float2(rh);
             v0 += f.x;
             v1 += f.y;
             if (SPLIT) {
-              const float2 fl = lo2_to_f32(rl);   // lo plane: 2^11-scaled
+              const float2 fl = lo2_to_f32(rl);
               v0 += fl.x;
               v1 += fl.y;
             }
@@ -284,15 +256,11 @@ __device__ __forceinline__ void epi_staged(float (&acc)[MH][SPLIT ? 2 : 1][NACC]
             v0 = act_t<ACT>(v0);
             v1 = act_t<ACT>(v1);
           }
-          const __half2 o = pack_sat(v0, v1);
-          *reinterpret_cast<__half2*>(out_tile + off) = o;
-          if (SPLIT) {
-            // hi saturates at +-65504 (pack_sat); the residual is taken against the clamped value, so a saturated
-            // element gets lo = 0 and hi + lo stays finite
-            const float2 hf = __half22float2(o);
-            const float c0 = fminf(fmaxf(v0, -65504.f), 65504.f), c1 = fminf(fmaxf(v1, -65504.f), 65504.f);
-            *reinterpret_cast<__half2*>(out_tile + A_STAGE_BYTES + off) = lo2_from_f32(c0 - hf.x, c1 - hf.y);
-          }
+          __half2 hi, lo;
+          if (SPLIT) split2_from_f32(v0, v1, hi, lo);
+          else hi = f16x2_from_f32(v0, v1);
+          *reinterpret_cast<__half2*>(out_tile + off) = hi;
+          if (SPLIT) *reinterpret_cast<__half2*>(out_tile + A_STAGE_BYTES + off) = lo;
         }
     }
     fence_proxy_async();   // generic-proxy smem writes -> visible to the TMA (async proxy)
@@ -538,7 +506,7 @@ tc_conv_kernel(const __grid_constant__ TcParams p) {
           for (int i = 0; i < NACC; ++i) __stcg(w + (mh * NACC + i) * ws_stride, acc[mh][0][i]);
         __threadfence();     // the partial is visible device-wide before the flag
         mma_bar_sync(128 * H);
-        if (ct == 0) asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p.sk_flags + 2 * sk_slot), "r"(1) : "memory");
+        if (ct == 0) st_release_gpu(p.sk_flags + 2 * sk_slot, 1);
         continue;
       }
       int sk_parts = 0;
@@ -548,10 +516,8 @@ tc_conv_kernel(const __grid_constant__ TcParams p) {
         if (ct == 0)
           for (int j = 1; j <= sk_parts; ++j) {
             const int* f = p.sk_flags + 2 * (PAIR ? 2 * (unit0 + j) + rank : unit0 + j);
-            int v;
-            do {
-              asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(f) : "memory");
-            } while (v == 0);
+            while (ld_acquire_gpu(f) == 0) {
+            }
           }
         mma_bar_sync(128 * H);
         for (int j = 1; j <= sk_parts; ++j) {
@@ -625,15 +591,14 @@ tc_conv_kernel(const __grid_constant__ TcParams p) {
                 if (trow >= p.tw * p.th || oy >= p.Ho || ox >= p.Wo || b >= p.nb) continue;
                 const long long pix = (long long)oy * p.Wo + ox;
                 const float a = acc[mh][0][j * 4 + 2 * h + e2];
-                float v = SPLIT ? __fmaf_rn(a, p.out_scale, bias_n) : a + bias_n;
+                float v = scale_bias<SPLIT>(a, p.out_scale, bias_n);
                 float rsd = 0.f;
                 if (p.residual) {
                   const __half* rp = p.residual + ((long long)b * p.res_batch_stride + pix * p.Cout) * NPL + n;
-                  rsd = __half2float(rp[0]);
-                  if (SPLIT) rsd += lo_to_f32(rp[p.Cout]);
+                  rsd = SPLIT ? split_to_f32(rp[0], rp[p.Cout]) : __half2float(rp[0]);
                 }
                 if (!raa) v += rsd;
-                v = (act == ACT_RELU) ? fmaxf(v, 0.f) : (act == ACT_TANH) ? tanhf(v) : (act == ACT_LEAKY) ? (v > 0.f ? v : 0.1f * v) : v;
+                v = apply_act(v, act);
                 if (raa) v += rsd;
                 if (p.nseg > 0) {
                   if (seg_base) seg_base[(long long)b * seg_bs + pix * seg_ps + seg_c] = v;
@@ -657,10 +622,7 @@ tc_conv_kernel(const __grid_constant__ TcParams p) {
       if (sk_head) {   // every thread has read the partials: re-arm the flags
         mma_bar_sync(128 * H);
         if (ct == 0)
-          for (int j = 1; j <= sk_parts; ++j)
-            asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(p.sk_flags + 2 * (PAIR ? 2 * (unit0 + j) + rank : unit0 + j)),
-                         "r"(0)
-                         : "memory");
+          for (int j = 1; j <= sk_parts; ++j) st_relaxed_gpu(p.sk_flags + 2 * (PAIR ? 2 * (unit0 + j) + rank : unit0 + j), 0);
       }
     }
     if (p.epi_tma && ct == 0) bulk_wait_read<0>();  // smem must outlive the bulk reads
@@ -742,33 +704,9 @@ __host__ __device__ __forceinline__ void chain_tiles_of_rows(const ChainLayer& p
   }
 }
 
-__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
-  int v;
-  asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void red_release_gpu_add(int* p, int v) {
-  asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-
 // pipeline stages of the chain kernel: the ring plus NPL x 16 KB staging tiles per buffer (two buffers in the fp16 mode,
 // one in the split mode) fill the 227 KB of an SM
 __host__ __device__ constexpr int chain_stages(bool split) { return split ? 3 : 6; }
-__device__ __forceinline__ bool mbar_test_wait(uint32_t addr, uint32_t parity) {   // non-blocking
-  uint32_t ok;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P1;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 P1, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, P1;\n\t"
-      "}"
-      : "=r"(ok)
-      : "r"(addr), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
 
 // first unit of a layer that belongs to CTA `cta` when the chain's unit list is dealt round-robin over G CTAs
 __device__ __forceinline__ int chain_first_unit(int cta, int ubase, int G) {
