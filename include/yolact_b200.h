@@ -28,6 +28,8 @@
  *                         sanitize_coordinates (layers/box_utils.py:327-373), F.interpolate bilinear
  *   yb_maskiou         <- FastMaskIoUNet.forward (yolact.py:363-375) + gather (output_utils.py:79-83)
  *   yb_fast_base_transform <- FastBaseTransform.forward (utils/augmentations.py:616-658)
+ *   yb_infer_frames    <- FastBaseTransform()(frames) followed by Yolact.forward in eval mode, as evalimage /
+ *                         evalvideo call them (eval.py:597-598, :695-704)
  *   yb_mask_iou / yb_box_iou <- mask_iou / jaccard (layers/box_utils.py:98-113, :54-79) as used by
  *                         eval.py:435-445 (_mask_iou, _bbox_iou)
  *   yb_mask_rle        <- pycocotools.mask.encode in Detections.add_mask (eval.py:320-330)
@@ -193,6 +195,18 @@ YB_API int yb_set_detect_params(yb_handle* h, int top_k, float conf_thresh, floa
 YB_API int yb_infer(yb_handle* h, const float* d_x, int B, int H, int W, int cross_class, int max_out,
              float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count,
              float* d_proto, void* stream);
+
+/* yb_infer from uint8 frames: d_img [B,H,W,3] BGR uint8 is FastBaseTransform'ed (as yb_fast_base_transform with
+ * img_is_u8 = 1, out_h, out_w, mode, h_mean_bgr, h_std_bgr; NULL = MEANS / STD) and run through the network and Detect
+ * as yb_infer(out_h, out_w) does, with the same outputs, bit for bit.  In the tensor-core modes the transform happens
+ * inside the stem's operand loader, so no [B,3,out_h,out_w] fp32 input is written; in YB_PREC_F32 it runs as one
+ * more kernel in the graph.  Replayed as one CUDA graph per frame size, transform and NMS mode.  Each (B, out_h, out_w)
+ * keeps the buffers and graphs of its 4 most recently used frame sizes / transforms; the first call with another one
+ * allocates (and, past four, synchronises the device to free the least recently used). */
+YB_API int yb_infer_frames(yb_handle* h, const uint8_t* d_img, int B, int H, int W, int out_h, int out_w, int mode,
+                           const float* h_mean_bgr, const float* h_std_bgr, int cross_class, int max_out,
+                           float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count,
+                           float* d_proto, void* stream);
 
 /* ---- postprocess (mask assembly) -------------------------------------------------------------- */
 /* One image.  proto [ph,pw,k] fp32 NHWC, coef [n,k], box [n,4] relative (NOT modified: the

@@ -70,6 +70,9 @@ SIGNATURES = {
     "yb_set_detect_params": (c_int, [c_void_p, c_int, c_float, c_float, c_int]),
     "yb_infer": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                          c_void_p, c_void_p, c_void_p, c_void_p]),
+    "yb_infer_frames": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
+                                POINTER(c_float), POINTER(c_float), c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                c_void_p, c_void_p, c_void_p, c_void_p]),
     "yb_postprocess": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "yb_postprocess_batch": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,

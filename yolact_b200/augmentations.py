@@ -27,6 +27,34 @@ def calc_size_preserve_ar(img_w, img_h, max_size):
     return int(w), int(h)
 
 
+def transform_mode(cfg):
+    """cfg.backbone.transform as a yb_transform_mode (utils/augmentations.py:645-650)."""
+    if getattr(cfg, "normalize", True):
+        return _lib.YB_XFORM_NORMALIZE
+    if getattr(cfg, "subtract_means", False):
+        return _lib.YB_XFORM_SUBTRACT_MEANS
+    if getattr(cfg, "to_float", False):
+        return _lib.YB_XFORM_TO_FLOAT
+    return _lib.YB_XFORM_NONE
+
+
+def frame_geometry(cfg, img, who="FastBaseTransform"):
+    """FastBaseTransform's checks and size rule for a [n, h, w, 3] BGR frame batch: (n, h, w, out_h, out_w)."""
+    if not img.is_cuda:
+        raise _lib.YbError("yolact_b200.%s runs on CUDA (H100) only; there is no CPU path." % who)
+    if getattr(cfg, "channel_order", "RGB") != "RGB":
+        raise NotImplementedError   # utils/augmentations.py:648-649
+    B, H, W, C = (int(s) for s in img.shape)
+    if C != 3:
+        raise ValueError("%s expects [n, h, w, 3] BGR frames" % who)
+    S = int(cfg.max_size)
+    if getattr(cfg, "preserve_aspect_ratio", False):
+        ow, oh = calc_size_preserve_ar(W, H, S)
+    else:
+        oh = ow = S
+    return B, H, W, oh, ow
+
+
 class FastBaseTransform(torch.nn.Module):
     def __init__(self, cfg=None):
         super().__init__()
@@ -34,29 +62,8 @@ class FastBaseTransform(torch.nn.Module):
         self.mean = _config.MEANS
         self.std = _config.STD
 
-    def _mode(self):
-        c = self.cfg
-        if getattr(c, "normalize", True):
-            return _lib.YB_XFORM_NORMALIZE
-        if getattr(c, "subtract_means", False):
-            return _lib.YB_XFORM_SUBTRACT_MEANS
-        if getattr(c, "to_float", False):
-            return _lib.YB_XFORM_TO_FLOAT
-        return _lib.YB_XFORM_NONE
-
     def forward(self, img):
-        if not img.is_cuda:
-            raise _lib.YbError("yolact_b200.FastBaseTransform runs on CUDA (H100) only; there is no CPU path.")
-        if getattr(self.cfg, "channel_order", "RGB") != "RGB":
-            raise NotImplementedError   # utils/augmentations.py:648-649
-        B, H, W, C = (int(s) for s in img.shape)
-        if C != 3:
-            raise ValueError("FastBaseTransform expects [n, h, w, 3] BGR frames")
-        S = int(self.cfg.max_size)
-        if getattr(self.cfg, "preserve_aspect_ratio", False):
-            ow, oh = calc_size_preserve_ar(W, H, S)
-        else:
-            oh = ow = S
+        B, H, W, oh, ow = frame_geometry(self.cfg, img)
         is_u8 = img.dtype == torch.uint8
         x = img.contiguous() if is_u8 else img.contiguous().float()
         out = torch.empty(B, 3, oh, ow, dtype=torch.float32, device=img.device)
@@ -64,6 +71,6 @@ class FastBaseTransform(torch.nn.Module):
         std = (ctypes.c_float * 3)(*self.std)
         lib = _lib.load()
         _lib.check(lib.yb_fast_base_transform(_ops_handle(img.device), _lib.ptr(x), 1 if is_u8 else 0, B, H, W, oh, ow,
-                                              self._mode(), mean, std, _lib.ptr(out), _lib.current_stream(img.device)),
+                                              transform_mode(self.cfg), mean, std, _lib.ptr(out), _lib.current_stream(img.device)),
                    "yb_fast_base_transform")
         return out

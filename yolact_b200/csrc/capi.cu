@@ -112,6 +112,10 @@ struct TempPool {  // RAII device temporaries for the op-level hooks
   }
 };
 
+// data/config.py:28-29 (BGR order): the transform's mean / std when the caller passes NULL
+const float kMeans[3] = {103.94f, 116.78f, 123.68f};
+const float kStd[3] = {57.38f, 57.12f, 58.40f};
+
 inline int grid1d(int64_t n) { return (int)std::min<int64_t>(132 * 16, (n + 255) / 256); }
 
 }  // namespace
@@ -264,6 +268,21 @@ int yb_infer(yb_handle* h, const float* d_x, int B, int H, int W, int cross_clas
   CallGuard g(h, (cudaStream_t)stream);   // shared workspaces: ordered behind the previous call
   h->infer(d_x, B, H, W, cross_class, max_out, d_box, d_coef_out, d_cls, d_score, d_count, d_proto,
            (cudaStream_t)stream);
+  YB_API_END
+}
+
+int yb_infer_frames(yb_handle* h, const uint8_t* d_img, int B, int H, int W, int out_h, int out_w, int mode,
+                    const float* h_mean_bgr, const float* h_std_bgr, int cross_class, int max_out, float* d_box,
+                    float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto,
+                    void* stream) {
+  YB_API_BEGIN
+  YB_REQUIRE(h && d_img && B > 0 && H > 0 && W > 0 && out_h > 0 && out_w > 0, "yb_infer_frames: bad argument");
+  YB_REQUIRE(!h->ops_only, "yb_infer_frames: handle has no network");
+  YB_REQUIRE(d_box && d_coef_out && d_cls && d_score && d_count, "yb_infer_frames: null output");
+  YB_REQUIRE(mode >= YB_XFORM_NORMALIZE && mode <= YB_XFORM_NONE, "yb_infer_frames: unknown transform mode");
+  CallGuard g(h, (cudaStream_t)stream);   // shared workspaces: ordered behind the previous call
+  h->infer_frames(d_img, B, H, W, out_h, out_w, mode, h_mean_bgr ? h_mean_bgr : kMeans, h_std_bgr ? h_std_bgr : kStd,
+                  cross_class, max_out, d_box, d_coef_out, d_cls, d_score, d_count, d_proto, (cudaStream_t)stream);
   YB_API_END
 }
 
@@ -436,9 +455,6 @@ int yb_fast_base_transform(yb_handle* h, const void* d_img, int img_is_u8, int B
   YB_API_BEGIN
   YB_REQUIRE(h && d_img && d_out, "yb_fast_base_transform: null argument");
   YB_REQUIRE(mode >= YB_XFORM_NORMALIZE && mode <= YB_XFORM_NONE, "yb_fast_base_transform: unknown transform mode");
-  // data/config.py:28-29 (BGR order)
-  static const float kMeans[3] = {103.94f, 116.78f, 123.68f};
-  static const float kStd[3] = {57.38f, 57.12f, 58.40f};
   CallGuard g(h);
   launch_fast_base_transform(d_img, img_is_u8, B, H, W, out_h, out_w, mode, h_mean_bgr ? h_mean_bgr : kMeans,
                              h_std_bgr ? h_std_bgr : kStd, d_out, (cudaStream_t)stream, &h->lc);

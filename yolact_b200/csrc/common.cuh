@@ -135,6 +135,56 @@ __device__ __forceinline__ float apply_act(float v, int act) {
   }
 }
 
+// ---- FastBaseTransform's per-pixel arithmetic (utils/augmentations.py:616-658) ---------------------------------------
+// The only definition: evalops.cu's fast_base_transform_kernel writes it to an NCHW fp32 tensor, the frame-source stem
+// (stem_tc.cu) computes it inside its loader, so both give the network bit for bit the same input.
+struct XformAffine {   // BGR order
+  float mean[3];
+  float stdv[3];
+};
+// One axis of ATen's area_pixel_compute_source_index + guard_index_and_lambda (UpSample.h), align_corners=False:
+// output coordinate o reads source taps i0 and i1 with weights 1 - l1 and l1.  scale = (float)in_n / (float)out_n.
+struct XformTap {
+  int i0, i1;
+  float l1;
+};
+__device__ __forceinline__ XformTap xform_tap(int o, int out_n, int in_n, float scale) {
+  XformTap t{o, o, 0.f};
+  if (out_n != in_n) {
+    const float s = fmaxf(__fsub_rn(__fmul_rn(scale, (float)o + 0.5f), 0.5f), 0.f);
+    t.i0 = min((int)s, in_n - 1);
+    t.i1 = t.i0 + (t.i0 < in_n - 1 ? 1 : 0);
+    t.l1 = fminf(fmaxf(s - (float)t.i0, 0.f), 1.f);
+  }
+  return t;
+}
+__device__ __forceinline__ float xform_load(const uint8_t* p) { return (float)*p; }
+__device__ __forceinline__ float xform_load(const float* p) { return *p; }
+// One output pixel of an HWC BGR image of width W: four-tap blend, then (v - mean) / std | v - mean | v / 255 | v
+// (yb_transform_mode), written to rgb[] in RGB order.
+template <typename TIn>
+__device__ __forceinline__ void xform_pixel(const TIn* img, int W, XformTap th, XformTap tw, int mode,
+                                            const XformAffine& aff, float rgb[3]) {
+  const float l0h = 1.f - th.l1, l0w = 1.f - tw.l1;
+  const TIn* p00 = img + ((size_t)th.i0 * W + tw.i0) * 3;
+  const TIn* p01 = img + ((size_t)th.i0 * W + tw.i1) * 3;
+  const TIn* p10 = img + ((size_t)th.i1 * W + tw.i0) * 3;
+  const TIn* p11 = img + ((size_t)th.i1 * W + tw.i1) * 3;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {   // c indexes the SOURCE (BGR) channel; it lands in 2 - c (RGB)
+    const float top = __fadd_rn(__fmul_rn(l0w, xform_load(p00 + c)), __fmul_rn(tw.l1, xform_load(p01 + c)));
+    const float bot = __fadd_rn(__fmul_rn(l0w, xform_load(p10 + c)), __fmul_rn(tw.l1, xform_load(p11 + c)));
+    float v = __fadd_rn(__fmul_rn(l0h, top), __fmul_rn(th.l1, bot));
+    if (mode == YB_XFORM_NORMALIZE)
+      v = __fdiv_rn(__fsub_rn(v, aff.mean[c]), aff.stdv[c]);
+    else if (mode == YB_XFORM_SUBTRACT_MEANS)
+      v = __fsub_rn(v, aff.mean[c]);
+    else if (mode == YB_XFORM_TO_FLOAT)
+      v = __fdiv_rn(v, 255.f);
+    rgb[2 - c] = v;
+  }
+}
+
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 

@@ -8,6 +8,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <array>
 #include <set>
 
 namespace yb {
@@ -26,6 +27,11 @@ void Executor::drop_detect_state() {
   for (auto& kv : infer_graphs)
     if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   infer_graphs.clear();
+  for (auto& fi : frame_inputs) {
+    for (auto& kv : fi.second.graphs)
+      if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+    fi.second.graphs.clear();
+  }
   void* bufs[6] = {det_ws, det_box, det_coef, det_cls, det_score, det_count};
   for (void* b : bufs) {
     if (!b) continue;
@@ -40,10 +46,27 @@ void Executor::drop_detect_state() {
   det_cap = 0;
 }
 
+void Executor::drop_frame_input(std::map<std::string, FrameInput>::iterator it) {
+  YB_CHECK_CUDA(cudaDeviceSynchronize());   // the buffer may still be read by an earlier replay
+  FrameInput& fi = it->second;
+  for (auto& kv : fi.graphs)
+    if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+  if (fi.stem) {
+    stem_plans.erase(std::find(stem_plans.begin(), stem_plans.end(), fi.stem));
+    stem_tc_plan_destroy(fi.stem);
+  }
+  allocs.erase(std::find(allocs.begin(), allocs.end(), (void*)fi.d_frames));
+  cudaFree(fi.d_frames);
+  frame_inputs.erase(it);
+}
+
 Executor::~Executor() {
   if (graph_fwd) cudaGraphExecDestroy(graph_fwd);
   for (auto& kv : infer_graphs)
     if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+  for (auto& fi : frame_inputs)
+    for (auto& kv : fi.second.graphs)
+      if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   for (auto* c : chains) tc_chain_destroy(c);
   for (auto* p : plans) tc_conv_plan_destroy(p);
   for (auto* p : stem_plans) stem_tc_plan_destroy(p);
@@ -276,6 +299,8 @@ struct NetBuilder {
     op.name = key + " " + std::to_string(in.C) + "->" + std::to_string(w.Cout) + " k" + std::to_string(k) + "s" +
               std::to_string(stride) + " " + std::to_string(p.Ho) + "x" + std::to_string(p.Wo);
     if (stem_tc) {
+      // yb_infer_frames replaces ops[0] with the frame-source stem
+      YB_REQUIRE(ex->ops.empty() && ex->stem_plans.empty(), ("conv " + key + ": the stem must be the first op").c_str());
       StemTcPlan* sp = stem_tc_plan_create((const float*)in.ptr, w.w_tc, w.bias, (__half*)out.ptr, in.B, in.H, in.W, k,
                                            stride, pad, w.Cout, act, split ? 1 : 0, w.out_scale, out.C);
       ex->stem_plans.push_back(sp);
@@ -1103,26 +1128,32 @@ Executor* yb_handle::get_executor(int B, int H, int W) {
   return raw;
 }
 
-static void run_ops(yb_handle* h, Executor* ex, cudaStream_t stream, bool branches = false) {
+// fin (yb_infer_frames): its entry op runs first, in place of ops[0] when it replaces the stem
+static void run_ops(yb_handle* h, Executor* ex, cudaStream_t stream, bool branches = false,
+                    const Executor::FrameInput* fin = nullptr) {
   static const bool trace = getenv("YB_TRACE") != nullptr;   // debug: name every op and sync after it
+  const size_t first = (fin && fin->replaces_stem) ? 1 : 0;
   if (trace) {
-    for (auto& op : ex->ops) {
+    auto run = [&](const Op& op) {
       fprintf(stderr, "[yb] %s ...", op.name.c_str());
       fflush(stderr);
       op.fn(stream);
       cudaError_t e = cudaStreamSynchronize(stream);
       fprintf(stderr, " %s\n", e == cudaSuccess ? "ok" : cudaGetErrorString(e));
       fflush(stderr);
-    }
+    };
+    if (fin) run(fin->entry);
+    for (size_t i = first; i < ex->ops.size(); ++i) run(ex->ops[i]);
     return;
   }
+  if (fin) fin->entry.fn(stream);
   if (!branches || ex->fork_index == 0 || ex->fork_index >= ex->ops.size()) {
-    for (auto& op : ex->ops) op.fn(stream);
+    for (size_t i = first; i < ex->ops.size(); ++i) ex->ops[i].fn(stream);
     return;
   }
   // trunk, then fork: each lane gets its own stream so that the captured graph has parallel branches
   // (small latency-bound head convs fill the gaps of the large protonet convs)
-  for (size_t i = 0; i < ex->fork_index; ++i) ex->ops[i].fn(stream);
+  for (size_t i = first; i < ex->fork_index; ++i) ex->ops[i].fn(stream);
   if (!h->ev_fork) YB_CHECK_CUDA(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
   YB_CHECK_CUDA(cudaEventRecord(h->ev_fork, stream));
   bool used[8] = {false, false, false, false, false, false, false, false};
@@ -1214,6 +1245,58 @@ void yb_handle::infer(const float* d_x, int B, int H, int W, int cross_class, in
                       float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto,
                       cudaStream_t stream) {
   Executor* ex = get_executor(B, H, W);
+  infer_on(ex, nullptr, d_x, cross_class, max_out, d_box, d_coef_out, d_cls, d_score, d_count, d_proto, stream);
+}
+
+void yb_handle::infer_frames(const uint8_t* d_img, int B, int fh, int fw, int H, int W, int mode,
+                             const float* mean_bgr, const float* std_bgr, int cross_class, int max_out, float* d_box,
+                             float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto,
+                             cudaStream_t stream) {
+  Executor* ex = get_executor(B, H, W);
+  char key[256];
+  snprintf(key, sizeof(key), "%dx%d m%d %a %a %a / %a %a %a", fh, fw, mode, mean_bgr[0], mean_bgr[1], mean_bgr[2],
+           std_bgr[0], std_bgr[1], std_bgr[2]);
+  auto it = ex->frame_inputs.find(key);
+  if (it == ex->frame_inputs.end()) {
+    if (ex->frame_inputs.size() >= Executor::kMaxFrameInputs)
+      ex->drop_frame_input(std::min_element(ex->frame_inputs.begin(), ex->frame_inputs.end(), [](auto& a, auto& b) {
+        return a.second.last_use < b.second.last_use;
+      }));
+    Executor::FrameInput fi;
+    fi.d_frames = (uint8_t*)dmalloc(ex->allocs, (size_t)B * fh * fw * 3);
+    fi.fh = fh;
+    fi.fw = fw;
+    LaunchCounter* lc = &this->lc;
+    if (cfg.precision == YB_PREC_F32) {
+      // no tensor-core stem to fuse into: FastBaseTransform into d_in, then the network's own stem
+      const uint8_t* img = fi.d_frames;
+      float* d_in = ex->d_in;
+      std::array<float, 3> mean{mean_bgr[0], mean_bgr[1], mean_bgr[2]}, stdv{std_bgr[0], std_bgr[1], std_bgr[2]};
+      fi.entry.name = "fast_base_transform " + std::to_string(fh) + "x" + std::to_string(fw);
+      fi.entry.fn = [=](cudaStream_t s) {
+        launch_fast_base_transform(img, 1, B, fh, fw, H, W, mode, mean.data(), stdv.data(), d_in, s, lc);
+      };
+    } else {
+      YB_REQUIRE(!ex->stem_plans.empty() && !ex->ops.empty(), "yb_infer_frames: the network has no tensor-core stem");
+      StemTcPlan* sp = stem_tc_plan_create_frames(ex->stem_plans[0], fi.d_frames, fh, fw, mode, mean_bgr, std_bgr);
+      ex->stem_plans.push_back(sp);
+      fi.stem = sp;
+      fi.entry.name = ex->ops[0].name + " frames " + std::to_string(fh) + "x" + std::to_string(fw);
+      fi.entry.fn = [sp, lc](cudaStream_t s) { launch_stem_tc(sp, s, lc); };
+      fi.replaces_stem = true;
+    }
+    it = ex->frame_inputs.emplace(key, std::move(fi)).first;
+  }
+  it->second.last_use = ++ex->frame_clock;
+  infer_on(ex, &it->second, d_img, cross_class, max_out, d_box, d_coef_out, d_cls, d_score, d_count, d_proto, stream);
+}
+
+// Forward + Detect on an executor; fin == null takes NCHW fp32 input d_x into d_in, otherwise uint8 frames d_x into
+// fin->d_frames.  Each input keeps its own captured graphs.
+void yb_handle::infer_on(Executor* ex, Executor::FrameInput* fin, const void* d_x, int cross_class, int max_out,
+                         float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count,
+                         float* d_proto, cudaStream_t stream) {
+  const int B = ex->B, H = ex->H, W = ex->W;
   DetectParams dp;
   dp.B = B;
   dp.P = ex->P;
@@ -1242,13 +1325,17 @@ void yb_handle::infer(const float* d_x, int B, int H, int W, int cross_class, in
     ex->det_count = (int32_t*)dmalloc(ex->allocs, (size_t)B * 4);
     ex->det_cap = cap;
   }
-  Executor::InferGraph& ig = ex->infer_graphs[(cross_class & 0xFFF) | (max_out << 12)];
+  Executor::InferGraph& ig = (fin ? fin->graphs : ex->infer_graphs)[(cross_class & 0xFFF) | (max_out << 12)];
   auto run_all = [&](cudaStream_t s, bool branches) {
-    run_ops(this, ex, s, branches);
+    run_ops(this, ex, s, branches, fin);
     launch_detect(dp, ex->loc, ex->conf, ex->coef, ex->priors, ex->dws, ex->det_box, ex->det_coef, ex->det_cls,
                   ex->det_score, ex->det_count, s, &lc);
   };
-  YB_CHECK_CUDA(cudaMemcpyAsync(ex->d_in, d_x, (size_t)B * 3 * H * W * 4, cudaMemcpyDeviceToDevice, stream));
+  if (fin)
+    YB_CHECK_CUDA(cudaMemcpyAsync(fin->d_frames, d_x, (size_t)B * fin->fh * fin->fw * 3, cudaMemcpyDeviceToDevice,
+                                  stream));
+  else
+    YB_CHECK_CUDA(cudaMemcpyAsync(ex->d_in, d_x, (size_t)B * 3 * H * W * 4, cudaMemcpyDeviceToDevice, stream));
   last_exec = ex;
   if (!use_graphs || ig.calls == 0) {
     run_all(stream, false);   // first call of this mode eager: validates launches, sets function attributes
@@ -1271,7 +1358,8 @@ void yb_handle::infer(const float* d_x, int B, int H, int W, int cross_class, in
       cudaGraphDestroy(g);
     }
     YB_CHECK_CUDA(cudaGraphLaunch(ig.exec, stream));
-    lc.n += (int64_t)ex->ops.size() + (dp.cross_class == YB_NMS_CROSS_CLASS ? 2 : 3);
+    const int64_t net_ops = (int64_t)ex->ops.size() + ((fin && !fin->replaces_stem) ? 1 : 0);
+    lc.n += net_ops + (dp.cross_class == YB_NMS_CROSS_CLASS ? 2 : 3);
   }
   ig.calls++;
   const void* src[6] = {ex->det_box, ex->det_coef, ex->det_cls, ex->det_score, ex->det_count, ex->proto};

@@ -115,7 +115,25 @@ struct Executor {
   cudaGraphExec_t graph_fwd = nullptr;
   std::map<int, InferGraph> infer_graphs;
   int fwd_calls = 0;
-  void drop_detect_state();      // frees the Detect buffers and every captured yb_infer graph (Detect parameters changed)
+  // uint8 frame input (yb_infer_frames), one per frame size, transform mode, mean and std.  The frames replace only
+  // the input: the half modes run the frame-source stem in place of ops[0], f32 runs fast_base_transform into d_in
+  // ahead of ops[0]; every other op, plan and chain is this executor's.
+  struct FrameInput {
+    uint8_t* d_frames = nullptr;   // [B,fh,fw,3] copy of the caller's frames (stable address for graph replay)
+    int fh = 0, fw = 0;
+    Op entry;                      // the frame stem, or fast_base_transform in YB_PREC_F32
+    StemTcPlan* stem = nullptr;    // the frame stem's plan (half modes; also listed in stem_plans)
+    bool replaces_stem = false;    // entry runs instead of ops[0] (half modes) or before it (f32)
+    std::map<int, InferGraph> graphs;   // keyed like infer_graphs
+    uint64_t last_use = 0;
+  };
+  // A folder of images gives nearly every call its own frame size: at most kMaxFrameInputs are kept, and a new one
+  // beyond that synchronises the device and drops the least recently used.
+  static constexpr size_t kMaxFrameInputs = 4;
+  std::map<std::string, FrameInput> frame_inputs;
+  uint64_t frame_clock = 0;
+  void drop_frame_input(std::map<std::string, FrameInput>::iterator it);   // frees its buffer, plan and graphs
+  void drop_detect_state();      // frees the Detect buffers and every captured yb_infer / yb_infer_frames graph
   ~Executor();
 };
 
@@ -168,6 +186,13 @@ struct yb_handle {
                cudaStream_t stream);
   void infer(const float* d_x, int B, int H, int W, int cross_class, int max_out, float* d_box, float* d_coef_out,
              int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto, cudaStream_t stream);
+  // infer on [B,fh,fw,3] uint8 BGR frames, FastBaseTransform'ed to H x W on the way in (same executor as infer(B,H,W))
+  void infer_frames(const uint8_t* d_img, int B, int fh, int fw, int H, int W, int mode, const float* mean_bgr,
+                    const float* std_bgr, int cross_class, int max_out, float* d_box, float* d_coef_out,
+                    int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto, cudaStream_t stream);
+  void infer_on(yb::Executor* ex, yb::Executor::FrameInput* fin, const void* d_x, int cross_class, int max_out,
+                float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto,
+                cudaStream_t stream);
   void* get_scratch(size_t bytes);
   void* get_detect_ws(size_t bytes);
 };

@@ -21,57 +21,21 @@ namespace {
 // -------------------------------------------------------------------------------------------------
 // FastBaseTransform
 // -------------------------------------------------------------------------------------------------
-struct Affine3 {
-  float mean[3];
-  float stdv[3];
-};
-
-__device__ __forceinline__ float load_px(const uint8_t* p) { return (float)*p; }
-__device__ __forceinline__ float load_px(const float* p) { return *p; }
-
+// the per-pixel arithmetic is common.cuh xform_pixel, shared with the frame-source stem (stem_tc.cu)
 template <typename TIn>
 __global__ void __launch_bounds__(256)
 fast_base_transform_kernel(const TIn* __restrict__ img, int H, int W, int oh, int ow, float scale_h,
-                           float scale_w, int mode, Affine3 aff, float* __restrict__ out) {
+                           float scale_w, int mode, XformAffine aff, float* __restrict__ out) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x;
   const int y = blockIdx.y, b = blockIdx.z;
   if (x >= ow) return;
-  // ATen area_pixel_compute_source_index + guard_index_and_lambda (UpSample.h), align_corners=False
-  int h0 = y, h1 = y, w0 = x, w1 = x;
-  float l1h = 0.f, l1w = 0.f;
-  if (oh != H) {
-    float sh = fmaxf(__fsub_rn(__fmul_rn(scale_h, (float)y + 0.5f), 0.5f), 0.f);
-    h0 = min((int)sh, H - 1);
-    h1 = h0 + (h0 < H - 1 ? 1 : 0);
-    l1h = fminf(fmaxf(sh - (float)h0, 0.f), 1.f);
-  }
-  if (ow != W) {
-    float sw = fmaxf(__fsub_rn(__fmul_rn(scale_w, (float)x + 0.5f), 0.5f), 0.f);
-    w0 = min((int)sw, W - 1);
-    w1 = w0 + (w0 < W - 1 ? 1 : 0);
-    l1w = fminf(fmaxf(sw - (float)w0, 0.f), 1.f);
-  }
-  const float l0h = 1.f - l1h, l0w = 1.f - l1w;
-  const TIn* base = img + (size_t)b * H * W * 3;
-  const TIn* p00 = base + ((size_t)h0 * W + w0) * 3;
-  const TIn* p01 = base + ((size_t)h0 * W + w1) * 3;
-  const TIn* p10 = base + ((size_t)h1 * W + w0) * 3;
-  const TIn* p11 = base + ((size_t)h1 * W + w1) * 3;
+  float rgb[3];
+  xform_pixel(img + (size_t)b * H * W * 3, W, xform_tap(y, oh, H, scale_h), xform_tap(x, ow, W, scale_w), mode, aff,
+              rgb);
   const size_t plane = (size_t)oh * ow;
   float* o = out + (size_t)b * 3 * plane + (size_t)y * ow + x;
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {   // c indexes the SOURCE (BGR) channel; it lands in plane 2 - c (RGB)
-    float top = __fadd_rn(__fmul_rn(l0w, load_px(p00 + c)), __fmul_rn(l1w, load_px(p01 + c)));
-    float bot = __fadd_rn(__fmul_rn(l0w, load_px(p10 + c)), __fmul_rn(l1w, load_px(p11 + c)));
-    float v = __fadd_rn(__fmul_rn(l0h, top), __fmul_rn(l1h, bot));
-    if (mode == YB_XFORM_NORMALIZE)
-      v = __fdiv_rn(__fsub_rn(v, aff.mean[c]), aff.stdv[c]);
-    else if (mode == YB_XFORM_SUBTRACT_MEANS)
-      v = __fsub_rn(v, aff.mean[c]);
-    else if (mode == YB_XFORM_TO_FLOAT)
-      v = __fdiv_rn(v, 255.f);
-    o[(size_t)(2 - c) * plane] = v;
-  }
+  for (int c = 0; c < 3; ++c) o[(size_t)c * plane] = rgb[c];
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -320,7 +284,7 @@ void launch_fast_base_transform(const void* img, int img_is_u8, int B, int H, in
                                 LaunchCounter* lc) {
   YB_REQUIRE(B > 0 && H > 0 && W > 0 && out_h > 0 && out_w > 0, "fast_base_transform: empty input");
   YB_REQUIRE(out_h <= 65535 && B <= 65535, "fast_base_transform: grid limit");
-  Affine3 aff;
+  XformAffine aff;
   for (int c = 0; c < 3; ++c) {
     aff.mean[c] = mean_bgr[c];
     aff.stdv[c] = std_bgr[c];

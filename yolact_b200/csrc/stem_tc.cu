@@ -12,6 +12,16 @@
 // [Cout][Kpad] weight tile meanwhile; then warpgroup w runs ceil(K/16) wgmmas (M = 64, N = Cout) for the 64-row
 // halves w, w + WG of the tile and stores its rows' pixels from the accumulator registers.
 // Several CTAs per SM overlap gather / MMA / epilogue of different tiles.
+//
+// Frame source (FRAMES, yb_infer_frames): the input is a batch of [fh][fw][3] uint8 BGR frames, and FastBaseTransform
+// (resize to H x W, transform, BGR -> RGB) happens in the loader, so no NCHW fp32 input is ever written.  The 128 rows
+// of a tile are then an 8 x 16 block of output pixels of one image.  Its receptive field is a rectangle of the resized
+// image (FrameWindow: 21 x 37 pixels for 7x7/2, 10 x 18 for 3x3/1): all threads first fill a [3][ROWS][COLS] fp32
+// window of it in shared memory with common.cuh xform_pixel (zero outside the image: the conv's padding), then the
+// gather above reads the window instead of global memory.  A window pixel is shared by up to 16 patches, so staging
+// computes each resized pixel about 1.5 times per CTA where a direct gather would compute it once per tap.
+// Each output pixel's patch, and so its wgmma row and its output, is bit-identical to the NCHW path's on
+// fast_base_transform's output.
 #include "tc_common.cuh"
 
 namespace yb {
@@ -34,11 +44,24 @@ struct alignas(64) StemParams {
   long long M;
   int act;
   float out_scale;   // split: weights are pre-multiplied by 1 / out_scale (a power of two)
+  // frame source: frames [B][fh][fw][3] uint8 BGR resized to H x W with scale = (float)fh / H, (float)fw / W
+  const uint8_t* frames;
+  int fh, fw, xform_mode;
+  float scale_h, scale_w;
+  XformAffine aff;
+  int tiles_x, tiles_y;   // output tiles of FT_H x FT_W pixels per image
+};
+
+constexpr int FT_H = 8, FT_W = 16;   // frame source: a tile's 128 rows are FT_H x FT_W output pixels (row = y * FT_W + x)
+template <int KS, int STRIDE>
+struct FrameWindow {   // resized pixels a tile reads: [3][ROWS][COLS] fp32
+  static constexpr int ROWS = (FT_H - 1) * STRIDE + KS, COLS = (FT_W - 1) * STRIDE + KS;
+  static constexpr int BYTES = 3 * ROWS * COLS * 4;
 };
 
 // SPLIT (YB_PREC_F16X3): the patch is written as a hi and a lo fp16 tile, the weights come as [Cout][hi(Kpad) | lo(Kpad)],
 // three MMA passes (hi*hi into one accumulator, lo*hi + hi*lo into a second one) and the output pixel is [hi(COUT) | lo(COUT)].
-template <int KS, int STRIDE, int PAD, int COUT, int WG, bool SPLIT>
+template <int KS, int STRIDE, int PAD, int COUT, int WG, bool SPLIT, bool FRAMES>
 __global__ void __launch_bounds__(128 * WG)
 stem_tc_kernel(const __grid_constant__ StemParams p) {
   constexpr int NPL = SPLIT ? 2 : 1;
@@ -63,53 +86,117 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
       for (int a = 0; a < ATOMS; ++a)
         tma_load_3d(sB + (pl * ATOMS + a) * B_ATOM_BYTES, &p.tmW, &b_full, pl * ATOMS * 64 + a * 64, 0, 0);
   }
+  using Win = FrameWindow<KS, STRIDE>;
+  int fb = 0, fty = 0, ftx = 0;   // frame source: this tile's image and tile coordinates
+  if constexpr (FRAMES) {
+    int t = blockIdx.x;
+    ftx = t % p.tiles_x;
+    t /= p.tiles_x;
+    fty = t % p.tiles_y;
+    fb = t / p.tiles_y;
+    float* win = reinterpret_cast<float*>(sB + NPL * ATOMS * B_ATOM_BYTES);
+    const int y0 = fty * FT_H * STRIDE - PAD, x0 = ftx * FT_W * STRIDE - PAD;
+    const uint8_t* img = p.frames + (size_t)fb * p.fh * p.fw * 3;
+    for (int i = tid; i < Win::ROWS * Win::COLS; i += 128 * WG) {
+      const int y = y0 + i / Win::COLS, x = x0 + i % Win::COLS;
+      float rgb[3] = {0.f, 0.f, 0.f};
+      if (y >= 0 && y < p.H && x >= 0 && x < p.W)
+        xform_pixel(img, p.fw, xform_tap(y, p.H, p.fh, p.scale_h), xform_tap(x, p.W, p.fw, p.scale_w), p.xform_mode,
+                    p.aff, rgb);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) win[c * Win::ROWS * Win::COLS + i] = rgb[c];
+    }
+    __syncthreads();
+  }
   {
     const int row = tid & 127;
     const int wg = tid >> 7;   // worker group: which k-groups of the patch this thread gathers
-    const long long m = (long long)blockIdx.x * ST_M + row;
-    const bool valid = m < p.M;
-    int b = 0, ho = 0, wo = 0;
-    if (valid) {
-      wo = (int)(m % p.Wo);
-      const long long t = m / p.Wo;
-      ho = (int)(t % p.Ho);
-      b = (int)(t / p.Ho);
-    }
-    const int hb = ho * STRIDE - PAD, wb = wo * STRIDE - PAD;
-    unsigned rmask = 0, cmask = 0;
+    long long m;
+    bool valid;
+    if constexpr (FRAMES) {
+      const int ho = fty * FT_H + row / FT_W, wo = ftx * FT_W + row % FT_W;
+      valid = ho < p.Ho && wo < p.Wo;
+      m = ((long long)fb * p.Ho + ho) * p.Wo + wo;
+      // tap (0, 0) of this pixel in the window, which holds the zero padding: no predication
+      const float* xw = reinterpret_cast<const float*>(sB + NPL * ATOMS * B_ATOM_BYTES) +
+                        (row / FT_W) * STRIDE * Win::COLS + (row % FT_W) * STRIDE;
+      // the NCHW gather below with the window as its source (kept as two loops: through one shared loop the NCHW
+      // instances compile to different SASS)
 #pragma unroll
-    for (int r = 0; r < KS; ++r) {
-      if (valid && hb + r >= 0 && hb + r < p.H) rmask |= 1u << r;
-      if (valid && wb + r >= 0 && wb + r < p.W) cmask |= 1u << r;
-    }
-    const size_t plane = (size_t)p.H * p.W;
-    const float* xb = p.x + (size_t)b * 3 * plane + (long long)hb * p.W + wb;  // may point before the frame: guarded
+      for (int kg = 0; kg < ATOMS * 8; ++kg) {
+        if (WG > 1 && (kg % WG) != wg) continue;   // warp-uniform
+        uint4 pk, pkl;
+        __half2* h2 = reinterpret_cast<__half2*>(&pk);
+        __half2* l2 = reinterpret_cast<__half2*>(&pkl);
 #pragma unroll
-    for (int kg = 0; kg < ATOMS * 8; ++kg) {
-      if (WG > 1 && (kg % WG) != wg) continue;   // warp-uniform
-      uint4 pk, pkl;
-      __half2* h2 = reinterpret_cast<__half2*>(&pk);
-      __half2* l2 = reinterpret_cast<__half2*>(&pkl);
+        for (int j2 = 0; j2 < 4; ++j2) {
+          float v[2];
 #pragma unroll
-      for (int j2 = 0; j2 < 4; ++j2) {
-        float v[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int k = kg * 8 + j2 * 2 + e;   // compile-time after unrolling
-          float val = 0.f;
-          if (k < K) {
-            const int c = k / (KS * KS), r = (k % (KS * KS)) / KS, s = k % KS;
-            if (((rmask >> r) & 1u) && ((cmask >> s) & 1u)) val = __ldg(xb + (size_t)c * plane + r * p.W + s);
+          for (int e = 0; e < 2; ++e) {
+            const int k = kg * 8 + j2 * 2 + e;   // compile-time after unrolling
+            float val = 0.f;
+            if (k < K) {
+              const int c = k / (KS * KS), r = (k % (KS * KS)) / KS, s = k % KS;
+              val = xw[(c * Win::ROWS + r) * Win::COLS + s];
+            }
+            v[e] = val;
           }
-          v[e] = val;
+          if (SPLIT) split2_from_f32(v[0], v[1], h2[j2], l2[j2]);
+          else h2[j2] = __halves2half2(from_f32<__half>(v[0]), from_f32<__half>(v[1]));
         }
-        if (SPLIT) split2_from_f32(v[0], v[1], h2[j2], l2[j2]);
-        else h2[j2] = __halves2half2(from_f32<__half>(v[0]), from_f32<__half>(v[1]));
+        const int atom = kg >> 3;
+        const uint32_t aoff = sw128_off(row, kg & 7);
+        *reinterpret_cast<uint4*>(sA + atom * A_ATOM_BYTES + aoff) = pk;
+        if (SPLIT) *reinterpret_cast<uint4*>(sA + (ATOMS + atom) * A_ATOM_BYTES + aoff) = pkl;
       }
-      const int atom = kg >> 3;
-      const uint32_t aoff = sw128_off(row, kg & 7);
-      *reinterpret_cast<uint4*>(sA + atom * A_ATOM_BYTES + aoff) = pk;
-      if (SPLIT) *reinterpret_cast<uint4*>(sA + (ATOMS + atom) * A_ATOM_BYTES + aoff) = pkl;
+    } else {
+      m = (long long)blockIdx.x * ST_M + row;
+      valid = m < p.M;
+      int b = 0, ho = 0, wo = 0;
+      if (valid) {
+        wo = (int)(m % p.Wo);
+        const long long t = m / p.Wo;
+        ho = (int)(t % p.Ho);
+        b = (int)(t / p.Ho);
+      }
+      const int hb = ho * STRIDE - PAD, wb = wo * STRIDE - PAD;
+      unsigned rmask = 0, cmask = 0;
+#pragma unroll
+      for (int r = 0; r < KS; ++r) {
+        if (valid && hb + r >= 0 && hb + r < p.H) rmask |= 1u << r;
+        if (valid && wb + r >= 0 && wb + r < p.W) cmask |= 1u << r;
+      }
+      const size_t plane = (size_t)p.H * p.W;
+      const float* xb = p.x + (size_t)b * 3 * plane + (long long)hb * p.W + wb;  // may point before the frame: guarded
+      // the frame branch above repeats this loop with the window as its source: the two must keep the same k order and
+      // encoding, or yb_infer_frames stops being bit-identical to yb_infer on fast_base_transform's output
+#pragma unroll
+      for (int kg = 0; kg < ATOMS * 8; ++kg) {
+        if (WG > 1 && (kg % WG) != wg) continue;   // warp-uniform
+        uint4 pk, pkl;
+        __half2* h2 = reinterpret_cast<__half2*>(&pk);
+        __half2* l2 = reinterpret_cast<__half2*>(&pkl);
+#pragma unroll
+        for (int j2 = 0; j2 < 4; ++j2) {
+          float v[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int k = kg * 8 + j2 * 2 + e;   // compile-time after unrolling
+            float val = 0.f;
+            if (k < K) {
+              const int c = k / (KS * KS), r = (k % (KS * KS)) / KS, s = k % KS;
+              if (((rmask >> r) & 1u) && ((cmask >> s) & 1u)) val = __ldg(xb + (size_t)c * plane + r * p.W + s);
+            }
+            v[e] = val;
+          }
+          if (SPLIT) split2_from_f32(v[0], v[1], h2[j2], l2[j2]);
+          else h2[j2] = __halves2half2(from_f32<__half>(v[0]), from_f32<__half>(v[1]));
+        }
+        const int atom = kg >> 3;
+        const uint32_t aoff = sw128_off(row, kg & 7);
+        *reinterpret_cast<uint4*>(sA + atom * A_ATOM_BYTES + aoff) = pk;
+        if (SPLIT) *reinterpret_cast<uint4*>(sA + (ATOMS + atom) * A_ATOM_BYTES + aoff) = pkl;
+      }
     }
     __half* yrow = p.y + m * (long long)(p.cpad * NPL);
     if (valid && wg == 0)
@@ -146,8 +233,15 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       const int row = h * 64 + wq * 16 + (lane >> 2) + 8 * hh;
-      const long long m = (long long)blockIdx.x * ST_M + row;
-      if (m >= p.M) continue;
+      long long m;
+      if constexpr (FRAMES) {
+        const int ho = fty * FT_H + row / FT_W, wo = ftx * FT_W + row % FT_W;
+        if (ho >= p.Ho || wo >= p.Wo) continue;
+        m = ((long long)fb * p.Ho + ho) * p.Wo + wo;
+      } else {
+        m = (long long)blockIdx.x * ST_M + row;
+        if (m >= p.M) continue;
+      }
       __half* yrow = p.y + m * (long long)(p.cpad * NPL);
 #pragma unroll
       for (int j = 0; j < COUT / 8; ++j) {
@@ -167,17 +261,34 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
   }
 }
 
-template <int KS, int STRIDE, int PAD, int COUT, int WG, bool SPLIT>
+template <int KS, int STRIDE, int PAD, int COUT, int WG, bool SPLIT, bool FRAMES>
 void launch_variant(const StemParams& prm, cudaStream_t stream) {
   constexpr int K = 3 * KS * KS;
   constexpr int ATOMS = (K + 63) / 64;
-  const size_t smem = (size_t)(SPLIT ? 2 : 1) * ATOMS * (ST_M * 128 + COUT * 128) + 1024;
+  const size_t smem = (size_t)(SPLIT ? 2 : 1) * ATOMS * (ST_M * 128 + COUT * 128) + 1024 +
+                      (FRAMES ? FrameWindow<KS, STRIDE>::BYTES : 0);
   static PerDeviceOnce attr;
   if (attr.first())
-    YB_CHECK_CUDA(cudaFuncSetAttribute(stem_tc_kernel<KS, STRIDE, PAD, COUT, WG, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)smem));
-  const unsigned grid = (unsigned)((prm.M + ST_M - 1) / ST_M);
-  stem_tc_kernel<KS, STRIDE, PAD, COUT, WG, SPLIT><<<grid, 128 * WG, smem, stream>>>(prm);
+    YB_CHECK_CUDA(cudaFuncSetAttribute(stem_tc_kernel<KS, STRIDE, PAD, COUT, WG, SPLIT, FRAMES>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const unsigned grid = FRAMES ? (unsigned)(prm.B * prm.tiles_y * prm.tiles_x) : (unsigned)((prm.M + ST_M - 1) / ST_M);
+  stem_tc_kernel<KS, STRIDE, PAD, COUT, WG, SPLIT, FRAMES><<<grid, 128 * WG, smem, stream>>>(prm);
+}
+
+template <bool FRAMES>
+void launch_stem(const StemParams& prm, int ks, bool split, cudaStream_t stream) {
+  if (split) {
+    // the split stem holds 144 KB of operand tiles (one CTA per SM): two worker threads per pixel double the warps
+    // that hide the gather's latency
+    if (ks == 7)
+      launch_variant<7, 2, 3, 64, 2, true, FRAMES>(prm, stream);
+    else
+      launch_variant<3, 1, 1, 32, 1, true, FRAMES>(prm, stream);
+  } else if (ks == 7) {
+    launch_variant<7, 2, 3, 64, 1, false, FRAMES>(prm, stream);
+  } else {
+    launch_variant<3, 1, 1, 32, 1, false, FRAMES>(prm, stream);
+  }
 }
 
 }  // namespace
@@ -186,6 +297,7 @@ struct StemTcPlan {
   StemParams prm;
   int ks, stride, pad, cout;
   int split = 0;
+  bool frames = false;
 };
 
 bool stem_tc_supported(int ks, int stride, int pad, int cin, int cout) {
@@ -227,21 +339,39 @@ StemTcPlan* stem_tc_plan_create(const float* x_nchw, const __half* w_packed, con
   return plan;
 }
 
+StemTcPlan* stem_tc_plan_create_frames(const StemTcPlan* net_stem, const uint8_t* frames, int fh, int fw, int mode,
+                                       const float* mean_bgr, const float* std_bgr) {
+  YB_REQUIRE(!net_stem->frames, "stem_tc: the frame stem is derived from the network's NCHW stem");
+  YB_REQUIRE(fh > 0 && fw > 0, "stem_tc: empty frames");
+  YB_REQUIRE(mode >= YB_XFORM_NORMALIZE && mode <= YB_XFORM_NONE, "stem_tc: unknown transform mode");
+  auto* plan = new StemTcPlan(*net_stem);
+  StemParams& q = plan->prm;
+  plan->frames = true;
+  q.x = nullptr;
+  q.frames = frames;
+  q.fh = fh;
+  q.fw = fw;
+  q.xform_mode = mode;
+  // ATen: scale = (float)in / out when the output size is given (area_pixel_compute_scale), as fast_base_transform
+  q.scale_h = (float)fh / (float)q.H;
+  q.scale_w = (float)fw / (float)q.W;
+  for (int c = 0; c < 3; ++c) {
+    q.aff.mean[c] = mean_bgr[c];
+    q.aff.stdv[c] = std_bgr[c];
+  }
+  q.tiles_x = ceil_div(q.Wo, FT_W);
+  q.tiles_y = ceil_div(q.Ho, FT_H);
+  YB_REQUIRE((long long)q.B * q.tiles_y * q.tiles_x < (1ll << 31), "stem_tc: frame batch too large for one grid");
+  return plan;
+}
+
 void stem_tc_plan_destroy(StemTcPlan* plan) { delete plan; }
 
 void launch_stem_tc(const StemTcPlan* plan, cudaStream_t stream, LaunchCounter* lc) {
-  if (plan->split) {
-    // the split stem holds 144 KB of operand tiles (one CTA per SM): two worker threads per pixel double the warps
-    // that hide the gather's latency
-    if (plan->ks == 7)
-      launch_variant<7, 2, 3, 64, 2, true>(plan->prm, stream);
-    else
-      launch_variant<3, 1, 1, 32, 1, true>(plan->prm, stream);
-  } else if (plan->ks == 7) {
-    launch_variant<7, 2, 3, 64, 1, false>(plan->prm, stream);
-  } else {
-    launch_variant<3, 1, 1, 32, 1, false>(plan->prm, stream);
-  }
+  if (plan->frames)
+    launch_stem<true>(plan->prm, plan->ks, plan->split, stream);
+  else
+    launch_stem<false>(plan->prm, plan->ks, plan->split, stream);
   YB_CHECK_LAUNCH();
   if (lc) lc->n++;
 }

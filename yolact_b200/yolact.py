@@ -18,6 +18,7 @@ import torch.nn as nn
 
 from . import _lib
 from . import config as _config
+from .augmentations import frame_geometry, transform_mode
 from .detection import Detect
 
 
@@ -376,6 +377,52 @@ class Yolact(nn.Module):
         lib = _lib.load()
         h = self._handle_for(x.device)
         B, _, H, W = x.shape
+        mode, M, out = self._detect_outputs(h, x.device, B, H, W, cross_class)
+        box, coef, cls, score, count, proto = out
+        _lib.check(lib.yb_infer(h, _lib.ptr(x), B, H, W, mode, M, _lib.ptr(box), _lib.ptr(coef),
+                                _lib.ptr(cls), _lib.ptr(score), _lib.ptr(count), _lib.ptr(proto),
+                                _lib.current_stream(x.device)), "yb_infer")
+        self._last_B = B
+        return out
+
+    def infer_frames(self, frames, cross_class=None):
+        """infer_padded(FastBaseTransform(self.cfg)(frames)) as one call, bit for bit, with no host sync once the frame
+        size has been seen (the library keeps the 4 most recently used frame sizes per network input size).
+        frames: CUDA uint8 [B,h,w,3] BGR, any size; the network input size and the transform come from self.cfg
+        (max_size, preserve_aspect_ratio, normalize / subtract_means / to_float) as in FastBaseTransform.  In the
+        tensor-core precisions the resize and transform run inside the stem kernel: no fp32 input tensor is written."""
+        return self._infer_frames(frames, cross_class)[0]
+
+    def forward_frames(self, frames):
+        """forward(FastBaseTransform(self.cfg)(frames)) in eval mode, from uint8 frames (see infer_frames):
+        [{'detection': dict|None, 'net': net}] * B, which postprocess takes unchanged."""
+        if self.training:
+            raise RuntimeError("Yolact.forward_frames is the eval-mode path; call net.eval() first")
+        out, oh, ow = self._infer_frames(frames, None)
+        _config.cfg._tmp_img_h, _config.cfg._tmp_img_w = oh, ow   # the network input size, as forward sets it
+        return self._detection_list(out)
+
+    def _infer_frames(self, frames, cross_class):
+        B, H, W, oh, ow = frame_geometry(self.cfg, frames, "Yolact.infer_frames")
+        if frames.dtype != torch.uint8:
+            raise ValueError("Yolact.infer_frames takes uint8 frames; run float frames through "
+                             "FastBaseTransform and infer_padded")
+        x = frames.contiguous()
+        lib = _lib.load()
+        h = self._handle_for(x.device)
+        mode, M, out = self._detect_outputs(h, x.device, B, oh, ow, cross_class)
+        box, coef, cls, score, count, proto = out
+        mean = (ctypes.c_float * 3)(*_config.MEANS)
+        std = (ctypes.c_float * 3)(*_config.STD)
+        _lib.check(lib.yb_infer_frames(h, _lib.ptr(x), B, H, W, oh, ow, transform_mode(self.cfg), mean, std, mode, M,
+                                       _lib.ptr(box), _lib.ptr(coef), _lib.ptr(cls), _lib.ptr(score), _lib.ptr(count),
+                                       _lib.ptr(proto), _lib.current_stream(x.device)), "yb_infer_frames")
+        self._last_B = B
+        return out, oh, ow
+
+    def _detect_outputs(self, h, device, B, H, W, cross_class):
+        """The NMS mode, the padded row count M and the empty output tensors of one yb_infer call on [B,3,H,W]."""
+        lib = _lib.load()
         c = self.cfg
         if cross_class is None:
             mode = self.detect.nms_mode()   # fast_nms | cc_fast_nms | traditional_nms (--fast_nms=False)
@@ -384,31 +431,31 @@ class Yolact(nn.Module):
         # net.detect's attributes are live in the reference (detection.py:17-31): push them when they changed
         d = self.detect
         dkey = (int(d.top_k), float(d.conf_thresh), float(d.nms_thresh), int(d.max_num_detections))
-        idx = x.device.index if x.device.index is not None else torch.cuda.current_device()
+        idx = device.index if device.index is not None else torch.cuda.current_device()
         if self._detect_pushed.get(idx) != dkey:
             _lib.check(lib.yb_set_detect_params(h, *dkey), "yb_set_detect_params")
             self._detect_pushed[idx] = dkey
         M = dkey[0] if (mode & 0xFF) == _lib.YB_NMS_CROSS_CLASS else dkey[3]
         ph, pw = ctypes.c_int32(), ctypes.c_int32()
         _lib.check(lib.yb_proto_size(h, H, W, ctypes.byref(ph), ctypes.byref(pw)), "yb_proto_size")
-        o = dict(device=x.device)
+        o = dict(device=device)
         box = torch.empty(B, M, 4, dtype=torch.float32, **o)
         coef = torch.empty(B, M, c.mask_dim, dtype=torch.float32, **o)
         cls = torch.empty(B, M, dtype=torch.int64, **o)
         score = torch.empty(B, M, dtype=torch.float32, **o)
         count = torch.empty(B, dtype=torch.int32, **o)
         proto = torch.empty(B, ph.value, pw.value, c.mask_dim, dtype=torch.float32, **o) if c.eval_mask_branch else None
-        _lib.check(lib.yb_infer(h, _lib.ptr(x), B, H, W, mode, M, _lib.ptr(box), _lib.ptr(coef),
-                                _lib.ptr(cls), _lib.ptr(score), _lib.ptr(count), _lib.ptr(proto),
-                                _lib.current_stream(x.device)), "yb_infer")
-        self._last_B = B
-        return box, coef, cls, score, count, proto
+        return mode, M, (box, coef, cls, score, count, proto)
 
     def forward(self, x):
         _config.cfg._tmp_img_h, _config.cfg._tmp_img_w = int(x.shape[2]), int(x.shape[3])  # yolact.py:567-568
         if self.training:
             return self.forward_raw(x)
-        box, coef, cls, score, count, proto = self.infer_padded(x)
+        return self._detection_list(self.infer_padded(x))
+
+    def _detection_list(self, padded):
+        """infer_padded's outputs -> the eval-mode list of {'detection', 'net'} (detection.py:73-95)."""
+        box, coef, cls, score, count, proto = padded
         # the fixed-size tensors the per-image views below are cut from: what a multi-GPU caller hands to
         # parallel.gather_detections (one pack kernel + one all_gather) instead of re-padding the views
         self.last_padded_detections = (box, coef, cls, score, count)
