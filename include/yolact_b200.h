@@ -30,6 +30,7 @@
  *   yb_fast_base_transform <- FastBaseTransform.forward (utils/augmentations.py:616-658)
  *   yb_infer_frames    <- FastBaseTransform()(frames) followed by Yolact.forward in eval mode, as evalimage /
  *                         evalvideo call them (eval.py:597-598, :695-704)
+ *   yb_infer_frame_list <- the same for a batch of differently sized frames (evalimages over a folder, eval.py:612-625)
  *   yb_mask_iou / yb_box_iou <- mask_iou / jaccard (layers/box_utils.py:98-113, :54-79) as used by
  *                         eval.py:435-445 (_mask_iou, _bbox_iou)
  *   yb_mask_rle        <- pycocotools.mask.encode in Detections.add_mask (eval.py:320-330)
@@ -207,6 +208,18 @@ YB_API int yb_infer_frames(yb_handle* h, const uint8_t* d_img, int B, int H, int
                            const float* h_mean_bgr, const float* h_std_bgr, int cross_class, int max_out,
                            float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count,
                            float* d_proto, void* stream);
+
+/* yb_infer_frames for a list of B frames of any sizes: h_frames[b] (a host array of device pointers) is a [h, w, 3] BGR
+ * uint8 frame with h = h_hw[2b], w = h_hw[2b + 1].  Outputs are yb_infer(out_h, out_w)'s on the B FastBaseTransform'ed
+ * frames, bit for bit.  The frames are read in place (not copied); only the B-entry table of pointers, sizes and
+ * resize scales is uploaded, so the host arrays may be reused as soon as the call returns.  Nothing depends on the
+ * frame sizes: each (B, out_h, out_w) replays one CUDA graph per transform and NMS mode for any mix of them.
+ * YB_ERR_INVALID for a null frame pointer, h <= 0 or w <= 0, or a frame that is not device memory of the handle's
+ * device. */
+YB_API int yb_infer_frame_list(yb_handle* h, const uint8_t* const* h_frames, const int32_t* h_hw, int B, int out_h,
+                               int out_w, int mode, const float* h_mean_bgr, const float* h_std_bgr, int cross_class,
+                               int max_out, float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score,
+                               int32_t* d_count, float* d_proto, void* stream);
 
 /* ---- postprocess (mask assembly) -------------------------------------------------------------- */
 /* One image.  proto [ph,pw,k] fp32 NHWC, coef [n,k], box [n,4] relative (NOT modified: the

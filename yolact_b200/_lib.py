@@ -73,6 +73,9 @@ SIGNATURES = {
     "yb_infer_frames": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                 POINTER(c_float), POINTER(c_float), c_int, c_int, c_void_p, c_void_p, c_void_p,
                                 c_void_p, c_void_p, c_void_p, c_void_p]),
+    "yb_infer_frame_list": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_int32), c_int, c_int, c_int, c_int,
+                                    POINTER(c_float), POINTER(c_float), c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_void_p, c_void_p, c_void_p]),
     "yb_postprocess": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "yb_postprocess_batch": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,

@@ -55,6 +55,27 @@ def frame_geometry(cfg, img, who="FastBaseTransform"):
     return B, H, W, oh, ow
 
 
+def frame_list_geometry(cfg, frames, who="Yolact.infer_frames"):
+    """frame_geometry for a list of [h, w, 3] BGR frames batched into one network input: ([(h, w), ...], out_h, out_w).
+    All frames must be on one device and, with preserve_aspect_ratio, resize to one network input size."""
+    if len(frames) == 0:
+        raise ValueError("%s got an empty frame list" % who)
+    hw, out = [], set()
+    for f in frames:
+        if not isinstance(f, torch.Tensor) or f.dim() != 3:
+            raise ValueError("%s expects a list of [h, w, 3] BGR frames" % who)
+        _, H, W, oh, ow = frame_geometry(cfg, f.unsqueeze(0), who)
+        if f.device != frames[0].device:
+            raise ValueError("%s: all frames of a list must be on one device" % who)
+        hw.append((H, W))
+        out.add((oh, ow))
+    if len(out) != 1:
+        raise ValueError("%s: with preserve_aspect_ratio the frames of a list must resize to one network input size, "
+                         "got %s" % (who, sorted(out)))
+    (oh, ow), = out
+    return hw, oh, ow
+
+
 class FastBaseTransform(torch.nn.Module):
     def __init__(self, cfg=None):
         super().__init__()

@@ -286,6 +286,31 @@ int yb_infer_frames(yb_handle* h, const uint8_t* d_img, int B, int H, int W, int
   YB_API_END
 }
 
+int yb_infer_frame_list(yb_handle* h, const uint8_t* const* h_frames, const int32_t* h_hw, int B, int out_h, int out_w,
+                        int mode, const float* h_mean_bgr, const float* h_std_bgr, int cross_class, int max_out,
+                        float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count,
+                        float* d_proto, void* stream) {
+  YB_API_BEGIN
+  YB_REQUIRE(h && h_frames && h_hw && B > 0 && out_h > 0 && out_w > 0, "yb_infer_frame_list: bad argument");
+  YB_REQUIRE(!h->ops_only, "yb_infer_frame_list: handle has no network");
+  YB_REQUIRE(d_box && d_coef_out && d_cls && d_score && d_count, "yb_infer_frame_list: null output");
+  YB_REQUIRE(mode >= YB_XFORM_NORMALIZE && mode <= YB_XFORM_NONE, "yb_infer_frame_list: unknown transform mode");
+  for (int b = 0; b < B; ++b) {
+    YB_REQUIRE(h_frames[b], "yb_infer_frame_list: null frame pointer");
+    YB_REQUIRE(h_hw[2 * b] > 0 && h_hw[2 * b + 1] > 0, "yb_infer_frame_list: frame height and width must be positive");
+    cudaPointerAttributes a;
+    const bool found = cudaPointerGetAttributes(&a, h_frames[b]) == cudaSuccess;
+    if (!found) cudaGetLastError();   // not a pointer CUDA knows: clear the error, then reject
+    YB_REQUIRE(found && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == h->device,
+               "yb_infer_frame_list: a frame is not device memory of the handle's device");
+  }
+  CallGuard g(h, (cudaStream_t)stream);   // shared workspaces and frame table: ordered behind the previous call
+  h->infer_frame_list(h_frames, h_hw, B, out_h, out_w, mode, h_mean_bgr ? h_mean_bgr : kMeans,
+                      h_std_bgr ? h_std_bgr : kStd, cross_class, max_out, d_box, d_coef_out, d_cls, d_score, d_count,
+                      d_proto, (cudaStream_t)stream);
+  YB_API_END
+}
+
 int yb_debug_feature(yb_handle* h, int which, float* d_out, int32_t* chw, void* stream) {
   YB_API_BEGIN
   YB_REQUIRE(h && h->last_exec && which >= 0 && which < 9, "yb_debug_feature: no forward has run / bad index");

@@ -185,6 +185,17 @@ __device__ __forceinline__ void xform_pixel(const TIn* img, int W, XformTap th, 
   }
 }
 
+// One image of a frame list (yb_infer_frame_list): an [fh][fw][3] uint8 BGR frame resized to the network's H x W.  The
+// kernels read a device table of these, one per image, so one launch serves any mix of frame sizes.
+struct FrameRef {
+  const uint8_t* frame;
+  int fh, fw;
+  float scale_h, scale_w;   // (float)fh / H, (float)fw / W: ATen's scale, as fast_base_transform computes it
+};
+inline FrameRef frame_ref(const uint8_t* frame, int fh, int fw, int H, int W) {
+  return FrameRef{frame, fh, fw, (float)fh / (float)H, (float)fw / (float)W};
+}
+
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 

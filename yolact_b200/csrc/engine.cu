@@ -27,11 +27,12 @@ void Executor::drop_detect_state() {
   for (auto& kv : infer_graphs)
     if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   infer_graphs.clear();
-  for (auto& fi : frame_inputs) {
-    for (auto& kv : fi.second.graphs)
-      if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-    fi.second.graphs.clear();
-  }
+  for (auto* inputs : {&frame_inputs, &frame_list_inputs})
+    for (auto& fi : *inputs) {
+      for (auto& kv : fi.second.graphs)
+        if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+      fi.second.graphs.clear();
+    }
   void* bufs[6] = {det_ws, det_box, det_coef, det_cls, det_score, det_count};
   for (void* b : bufs) {
     if (!b) continue;
@@ -64,9 +65,10 @@ Executor::~Executor() {
   if (graph_fwd) cudaGraphExecDestroy(graph_fwd);
   for (auto& kv : infer_graphs)
     if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-  for (auto& fi : frame_inputs)
-    for (auto& kv : fi.second.graphs)
-      if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+  for (auto* inputs : {&frame_inputs, &frame_list_inputs})
+    for (auto& fi : *inputs)
+      for (auto& kv : fi.second.graphs)
+        if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   for (auto* c : chains) tc_chain_destroy(c);
   for (auto* p : plans) tc_conv_plan_destroy(p);
   for (auto* p : stem_plans) stem_tc_plan_destroy(p);
@@ -1128,7 +1130,7 @@ Executor* yb_handle::get_executor(int B, int H, int W) {
   return raw;
 }
 
-// fin (yb_infer_frames): its entry op runs first, in place of ops[0] when it replaces the stem
+// fin (yb_infer_frames / yb_infer_frame_list): its entry op runs first, in place of ops[0] when it replaces the stem
 static void run_ops(yb_handle* h, Executor* ex, cudaStream_t stream, bool branches = false,
                     const Executor::FrameInput* fin = nullptr) {
   static const bool trace = getenv("YB_TRACE") != nullptr;   // debug: name every op and sync after it
@@ -1291,8 +1293,49 @@ void yb_handle::infer_frames(const uint8_t* d_img, int B, int fh, int fw, int H,
   infer_on(ex, &it->second, d_img, cross_class, max_out, d_box, d_coef_out, d_cls, d_score, d_count, d_proto, stream);
 }
 
+void yb_handle::infer_frame_list(const uint8_t* const* frames, const int32_t* hw, int B, int H, int W, int mode,
+                                 const float* mean_bgr, const float* std_bgr, int cross_class, int max_out,
+                                 float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count,
+                                 float* d_proto, cudaStream_t stream) {
+  Executor* ex = get_executor(B, H, W);
+  if (!ex->d_frame_table) ex->d_frame_table = (FrameRef*)dmalloc(ex->allocs, (size_t)B * sizeof(FrameRef));
+  char key[256];
+  snprintf(key, sizeof(key), "m%d %a %a %a / %a %a %a", mode, mean_bgr[0], mean_bgr[1], mean_bgr[2], std_bgr[0],
+           std_bgr[1], std_bgr[2]);
+  auto it = ex->frame_list_inputs.find(key);
+  if (it == ex->frame_list_inputs.end()) {
+    Executor::FrameInput fi;
+    LaunchCounter* lc = &this->lc;
+    const FrameRef* table = ex->d_frame_table;
+    if (cfg.precision == YB_PREC_F32) {
+      // no tensor-core stem to fuse into: FastBaseTransform into d_in, then the network's own stem
+      float* d_in = ex->d_in;
+      std::array<float, 3> mean{mean_bgr[0], mean_bgr[1], mean_bgr[2]}, stdv{std_bgr[0], std_bgr[1], std_bgr[2]};
+      fi.entry.name = "fast_base_transform frame list";
+      fi.entry.fn = [=](cudaStream_t s) {
+        launch_fast_base_transform_list(table, B, H, W, mode, mean.data(), stdv.data(), d_in, s, lc);
+      };
+    } else {
+      YB_REQUIRE(!ex->stem_plans.empty() && !ex->ops.empty(), "yb_infer_frame_list: the network has no tensor-core stem");
+      StemTcPlan* sp = stem_tc_plan_create_frame_list(ex->stem_plans[0], table, mode, mean_bgr, std_bgr);
+      ex->stem_plans.push_back(sp);
+      fi.stem = sp;
+      fi.entry.name = ex->ops[0].name + " frame list";
+      fi.entry.fn = [sp, lc](cudaStream_t s) { launch_stem_tc(sp, s, lc); };
+      fi.replaces_stem = true;
+    }
+    it = ex->frame_list_inputs.emplace(key, std::move(fi)).first;
+  }
+  // one entry per image, pointing at the caller's frame: nothing is copied but the table itself
+  std::vector<FrameRef> table(B);
+  for (int b = 0; b < B; ++b) table[b] = frame_ref(frames[b], hw[2 * b], hw[2 * b + 1], H, W);
+  infer_on(ex, &it->second, table.data(), cross_class, max_out, d_box, d_coef_out, d_cls, d_score, d_count, d_proto,
+           stream);
+}
+
 // Forward + Detect on an executor; fin == null takes NCHW fp32 input d_x into d_in, otherwise uint8 frames d_x into
-// fin->d_frames.  Each input keeps its own captured graphs.
+// fin->d_frames, or for a frame list (fin->d_frames == null) the host FrameRef table d_x into ex->d_frame_table.  Each
+// input keeps its own captured graphs.
 void yb_handle::infer_on(Executor* ex, Executor::FrameInput* fin, const void* d_x, int cross_class, int max_out,
                          float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count,
                          float* d_proto, cudaStream_t stream) {
@@ -1331,7 +1374,11 @@ void yb_handle::infer_on(Executor* ex, Executor::FrameInput* fin, const void* d_
     launch_detect(dp, ex->loc, ex->conf, ex->coef, ex->priors, ex->dws, ex->det_box, ex->det_coef, ex->det_cls,
                   ex->det_score, ex->det_count, s, &lc);
   };
-  if (fin)
+  if (fin && !fin->d_frames)
+    // pageable source: staged before the call returns, so the host table may go away at once.  Stream-ordered after
+    // the previous call (CallGuard), so an earlier replay has read the table before it is overwritten.
+    YB_CHECK_CUDA(cudaMemcpyAsync(ex->d_frame_table, d_x, (size_t)B * sizeof(FrameRef), cudaMemcpyHostToDevice, stream));
+  else if (fin)
     YB_CHECK_CUDA(cudaMemcpyAsync(fin->d_frames, d_x, (size_t)B * fin->fh * fin->fw * 3, cudaMemcpyDeviceToDevice,
                                   stream));
   else

@@ -119,7 +119,8 @@ struct Executor {
   // the input: the half modes run the frame-source stem in place of ops[0], f32 runs fast_base_transform into d_in
   // ahead of ops[0]; every other op, plan and chain is this executor's.
   struct FrameInput {
-    uint8_t* d_frames = nullptr;   // [B,fh,fw,3] copy of the caller's frames (stable address for graph replay)
+    uint8_t* d_frames = nullptr;   // [B,fh,fw,3] copy of the caller's frames (stable address for graph replay);
+                                   // null for a frame list, whose entry reads d_frame_table
     int fh = 0, fw = 0;
     Op entry;                      // the frame stem, or fast_base_transform in YB_PREC_F32
     StemTcPlan* stem = nullptr;    // the frame stem's plan (half modes; also listed in stem_plans)
@@ -133,7 +134,12 @@ struct Executor {
   std::map<std::string, FrameInput> frame_inputs;
   uint64_t frame_clock = 0;
   void drop_frame_input(std::map<std::string, FrameInput>::iterator it);   // frees its buffer, plan and graphs
-  void drop_detect_state();      // frees the Detect buffers and every captured yb_infer / yb_infer_frames graph
+  // Frame lists (yb_infer_frame_list): every image brings its own frame and size.  The entry op reads them from
+  // d_frame_table (B entries, uploaded before each call), so a FrameInput here has no d_frames and is keyed by the
+  // transform alone (mode, mean, std): no buffer, plan or graph depends on a frame size.
+  FrameRef* d_frame_table = nullptr;
+  std::map<std::string, FrameInput> frame_list_inputs;
+  void drop_detect_state();      // frees the Detect buffers and every captured yb_infer / yb_infer_frames(_list) graph
   ~Executor();
 };
 
@@ -190,6 +196,11 @@ struct yb_handle {
   void infer_frames(const uint8_t* d_img, int B, int fh, int fw, int H, int W, int mode, const float* mean_bgr,
                     const float* std_bgr, int cross_class, int max_out, float* d_box, float* d_coef_out,
                     int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto, cudaStream_t stream);
+  // infer on a list of B uint8 BGR frames of any sizes: frames[b] is a device [hw[2b], hw[2b+1], 3] frame, read in place
+  void infer_frame_list(const uint8_t* const* frames, const int32_t* hw, int B, int H, int W, int mode,
+                        const float* mean_bgr, const float* std_bgr, int cross_class, int max_out, float* d_box,
+                        float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto,
+                        cudaStream_t stream);
   void infer_on(yb::Executor* ex, yb::Executor::FrameInput* fin, const void* d_x, int cross_class, int max_out,
                 float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto,
                 cudaStream_t stream);

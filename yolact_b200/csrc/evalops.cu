@@ -38,6 +38,22 @@ fast_base_transform_kernel(const TIn* __restrict__ img, int H, int W, int oh, in
   for (int c = 0; c < 3; ++c) o[(size_t)c * plane] = rgb[c];
 }
 
+// the same from a frame list (yb_infer_frame_list in YB_PREC_F32): image b's frame, size and scales are frames[b]
+__global__ void __launch_bounds__(256)
+fast_base_transform_list_kernel(const FrameRef* __restrict__ frames, int oh, int ow, int mode, XformAffine aff,
+                                float* __restrict__ out) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  const int y = blockIdx.y, b = blockIdx.z;
+  if (x >= ow) return;
+  const FrameRef f = frames[b];
+  float rgb[3];
+  xform_pixel(f.frame, f.fw, xform_tap(y, oh, f.fh, f.scale_h), xform_tap(x, ow, f.fw, f.scale_w), mode, aff, rgb);
+  const size_t plane = (size_t)oh * ow;
+  float* o = out + (size_t)b * 3 * plane + (size_t)y * ow + x;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) o[(size_t)c * plane] = rgb[c];
+}
+
 // -------------------------------------------------------------------------------------------------
 // bit packing + mask IoU
 // -------------------------------------------------------------------------------------------------
@@ -298,6 +314,22 @@ void launch_fast_base_transform(const void* img, int img_is_u8, int B, int H, in
   else
     fast_base_transform_kernel<float><<<grid, 256, 0, stream>>>((const float*)img, H, W, out_h, out_w, sh, sw, mode, aff,
                                                                 out);
+  YB_CHECK_LAUNCH();
+  if (lc) lc->n++;
+}
+
+void launch_fast_base_transform_list(const FrameRef* d_table, int B, int out_h, int out_w, int mode,
+                                     const float* mean_bgr, const float* std_bgr, float* out, cudaStream_t stream,
+                                     LaunchCounter* lc) {
+  YB_REQUIRE(d_table && B > 0 && out_h > 0 && out_w > 0, "fast_base_transform: empty input");
+  YB_REQUIRE(out_h <= 65535 && B <= 65535, "fast_base_transform: grid limit");
+  XformAffine aff;
+  for (int c = 0; c < 3; ++c) {
+    aff.mean[c] = mean_bgr[c];
+    aff.stdv[c] = std_bgr[c];
+  }
+  dim3 grid(ceil_div(out_w, 256), out_h, B);
+  fast_base_transform_list_kernel<<<grid, 256, 0, stream>>>(d_table, out_h, out_w, mode, aff, out);
   YB_CHECK_LAUNCH();
   if (lc) lc->n++;
 }

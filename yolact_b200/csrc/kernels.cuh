@@ -101,6 +101,10 @@ StemTcPlan* stem_tc_plan_create(const float* x_nchw, const __half* w_packed, con
 // (transform `mode`, BGR mean / std) happens in the loader.  Weights, output and shapes are net_stem's.
 StemTcPlan* stem_tc_plan_create_frames(const StemTcPlan* net_stem, const uint8_t* frames, int fh, int fw, int mode,
                                        const float* mean_bgr, const float* std_bgr);
+// ... or reading a frame list: image b's frame, size and scales come from d_table[b] (device, net_stem's B entries),
+// read at launch time, so the same plan (and graph) serves any frame sizes the table holds.
+StemTcPlan* stem_tc_plan_create_frame_list(const StemTcPlan* net_stem, const FrameRef* d_table, int mode,
+                                           const float* mean_bgr, const float* std_bgr);
 void stem_tc_plan_destroy(StemTcPlan* plan);
 void launch_stem_tc(const StemTcPlan* plan, cudaStream_t stream, LaunchCounter* lc);
 
@@ -175,6 +179,10 @@ void launch_maxpool_gather(const float* x_nhwc, int n, int H, int W, int C, cons
 void launch_fast_base_transform(const void* img, int img_is_u8, int B, int H, int W, int out_h, int out_w, int mode,
                                 const float* mean_bgr, const float* std_bgr, float* out, cudaStream_t stream,
                                 LaunchCounter* lc);
+// the same from a frame list: image b is d_table[b] (device, B entries), uint8, resized to out_h x out_w
+void launch_fast_base_transform_list(const FrameRef* d_table, int B, int out_h, int out_w, int mode,
+                                     const float* mean_bgr, const float* std_bgr, float* out, cudaStream_t stream,
+                                     LaunchCounter* lc);
 void launch_pack_mask_bits(const void* in, int in_format, int64_t rows, int w, uint32_t* out, cudaStream_t stream,
                            LaunchCounter* lc);
 void launch_mask_iou_bits(const uint32_t* a, int n, const uint32_t* b, int m, int64_t words, int iscrowd, float* out,

@@ -18,7 +18,7 @@ import torch.nn as nn
 
 from . import _lib
 from . import config as _config
-from .augmentations import frame_geometry, transform_mode
+from .augmentations import frame_geometry, frame_list_geometry, transform_mode
 from .detection import Detect
 
 
@@ -390,12 +390,16 @@ class Yolact(nn.Module):
         size has been seen (the library keeps the 4 most recently used frame sizes per network input size).
         frames: CUDA uint8 [B,h,w,3] BGR, any size; the network input size and the transform come from self.cfg
         (max_size, preserve_aspect_ratio, normalize / subtract_means / to_float) as in FastBaseTransform.  In the
-        tensor-core precisions the resize and transform run inside the stem kernel: no fp32 input tensor is written."""
+        tensor-core precisions the resize and transform run inside the stem kernel: no fp32 input tensor is written.
+        frames may also be a list or tuple of B CUDA uint8 [h_i,w_i,3] BGR frames of different sizes (a folder of
+        images): the same as infer_padded(torch.cat([FastBaseTransform(self.cfg)(f[None]) for f in frames])), from one
+        call and one CUDA graph whatever the sizes; the frames are read in place."""
         return self._infer_frames(frames, cross_class)[0]
 
     def forward_frames(self, frames):
-        """forward(FastBaseTransform(self.cfg)(frames)) in eval mode, from uint8 frames (see infer_frames):
-        [{'detection': dict|None, 'net': net}] * B, which postprocess takes unchanged."""
+        """forward(FastBaseTransform(self.cfg)(frames)) in eval mode, from uint8 frames (see infer_frames; a list of
+        differently sized frames too): [{'detection': dict|None, 'net': net}] * B, which postprocess takes unchanged
+        (postprocess(preds, w_i, h_i, i) for image i of a list)."""
         if self.training:
             raise RuntimeError("Yolact.forward_frames is the eval-mode path; call net.eval() first")
         out, oh, ow = self._infer_frames(frames, None)
@@ -403,6 +407,8 @@ class Yolact(nn.Module):
         return self._detection_list(out)
 
     def _infer_frames(self, frames, cross_class):
+        if isinstance(frames, (list, tuple)):
+            return self._infer_frame_list(frames, cross_class)
         B, H, W, oh, ow = frame_geometry(self.cfg, frames, "Yolact.infer_frames")
         if frames.dtype != torch.uint8:
             raise ValueError("Yolact.infer_frames takes uint8 frames; run float frames through "
@@ -417,6 +423,27 @@ class Yolact(nn.Module):
         _lib.check(lib.yb_infer_frames(h, _lib.ptr(x), B, H, W, oh, ow, transform_mode(self.cfg), mean, std, mode, M,
                                        _lib.ptr(box), _lib.ptr(coef), _lib.ptr(cls), _lib.ptr(score), _lib.ptr(count),
                                        _lib.ptr(proto), _lib.current_stream(x.device)), "yb_infer_frames")
+        self._last_B = B
+        return out, oh, ow
+
+    def _infer_frame_list(self, frames, cross_class):
+        hw, oh, ow = frame_list_geometry(self.cfg, frames, "Yolact.infer_frames")
+        if any(f.dtype != torch.uint8 for f in frames):
+            raise ValueError("Yolact.infer_frames takes uint8 frames; run float frames through "
+                             "FastBaseTransform and infer_padded")
+        xs = [f.contiguous() for f in frames]   # held until the call has enqueued its reads of them
+        B = len(xs)
+        device = xs[0].device
+        lib = _lib.load()
+        h = self._handle_for(device)
+        mode, M, out = self._detect_outputs(h, device, B, oh, ow, cross_class)
+        mean = (ctypes.c_float * 3)(*_config.MEANS)
+        std = (ctypes.c_float * 3)(*_config.STD)
+        ptrs = (ctypes.c_void_p * B)(*[x.data_ptr() for x in xs])
+        sizes = (ctypes.c_int32 * (2 * B))(*[v for s in hw for v in s])
+        _lib.check(lib.yb_infer_frame_list(h, ptrs, sizes, B, oh, ow, transform_mode(self.cfg), mean, std, mode, M,
+                                           *[_lib.ptr(t) for t in out], _lib.current_stream(device)),
+                   "yb_infer_frame_list")
         self._last_B = B
         return out, oh, ow
 
