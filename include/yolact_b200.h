@@ -26,6 +26,8 @@
  *                         with decode (layers/box_utils.py:267-312) and jaccard (box_utils.py:54-80)
  *   yb_postprocess     <- postprocess lincomb path (layers/output_utils.py:15-99), crop and
  *                         sanitize_coordinates (layers/box_utils.py:327-373), F.interpolate bilinear
+ *   yb_postprocess_list <- the same, called once per image of a batch of differently sized images (evalimages over a
+ *                         folder, eval.py:612-625)
  *   yb_maskiou         <- FastMaskIoUNet.forward (yolact.py:363-375) + gather (output_utils.py:79-83)
  *   yb_fast_base_transform <- FastBaseTransform.forward (utils/augmentations.py:616-658)
  *   yb_infer_frames    <- FastBaseTransform()(frames) followed by Yolact.forward in eval mode, as evalimage /
@@ -237,6 +239,31 @@ YB_API int yb_postprocess(yb_handle* h, const float* d_proto, int ph, int pw, in
 YB_API int yb_postprocess_batch(yb_handle* h, const float* d_proto, int ph, int pw, int k, const float* d_coef,
                                 const float* d_box, int n, int batch, int out_h, int out_w, int crop_masks,
                                 int mask_format, void* d_masks, int64_t* d_boxes_px, void* stream);
+
+/* One image of a yb_postprocess_list call (all pointers device memory):
+ *   proto [ph,pw,k], coef [n,k], box [n,4] relative: as yb_postprocess's (may be NULL when n == 0);
+ *   masks: [n, out_h, out_w] in the call's yb_mask_format (16-byte aligned), or NULL for boxes only;
+ *   boxes_px int64 [n,4] (nullable); proto_masks [n,ph,pw] fp32 (nullable; the FastMaskIoUNet input). */
+typedef struct {
+  const float* proto;
+  const float* coef;
+  const float* box;
+  void* masks;
+  int64_t* boxes_px;
+  float* proto_masks;
+  int32_t n;
+  int32_t out_h;
+  int32_t out_w;
+} yb_post_item;
+
+/* yb_postprocess for a list of B images of any output sizes and row counts, in ONE launch per kernel for the whole
+ * list (boxes, prototype-resolution masks, masks): every image's outputs are yb_postprocess's on it, bit for bit.
+ * h_items is host memory; it is uploaded into a table the handle owns (stream-ordered behind the handle's previous
+ * call) and may be reused as soon as the call returns.  n == 0 is allowed.  YB_ERR_INVALID for a null proto, coef or
+ * box with n > 0, n < 0, out_h <= 0 or out_w <= 0, masks not 16-byte aligned, or a pointer that is not device memory
+ * of the handle's device. */
+YB_API int yb_postprocess_list(yb_handle* h, const yb_post_item* h_items, int B, int ph, int pw, int k,
+                               int crop_masks, int mask_format, void* stream);
 
 /* maskiou_net on [n,1,ph,pw] fp32 masks -> d_maskiou [n] = net(mask)[i, cls[i]];
  * d_cls == NULL: d_maskiou [n, num_classes-1] = net(mask) (FastMaskIoUNet.forward itself). */

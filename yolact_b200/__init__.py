@@ -2,7 +2,7 @@
 Yolact.forward() / Detect() / postprocess() surface.  See DESIGN.md and INTEGRATION.md."""
 from .config import cfg, set_cfg, CONFIGS, MEANS, STD  # noqa: F401
 
-__all__ = ["cfg", "set_cfg", "CONFIGS", "Yolact", "Detect", "postprocess", "FastBaseTransform"]
+__all__ = ["cfg", "set_cfg", "CONFIGS", "Yolact", "Detect", "postprocess", "postprocess_list", "FastBaseTransform"]
 
 
 def __getattr__(name):  # lazy: importing the package must not require torch/CUDA
@@ -15,6 +15,9 @@ def __getattr__(name):  # lazy: importing the package must not require torch/CUD
     if name == "postprocess":
         from .output_utils import postprocess
         return postprocess
+    if name == "postprocess_list":
+        from .output_utils import postprocess_list
+        return postprocess_list
     if name == "FastBaseTransform":
         from .augmentations import FastBaseTransform
         return FastBaseTransform

@@ -40,6 +40,21 @@ class YbConfig(ctypes.Structure):
     ]
 
 
+class YbPostItem(ctypes.Structure):
+    """Mirror of yb_post_item (one image of yb_postprocess_list)."""
+    _fields_ = [
+        ("proto", c_void_p),
+        ("coef", c_void_p),
+        ("box", c_void_p),
+        ("masks", c_void_p),
+        ("boxes_px", c_void_p),
+        ("proto_masks", c_void_p),
+        ("n", c_int32),
+        ("out_h", c_int32),
+        ("out_w", c_int32),
+    ]
+
+
 YB_BACKBONE_NONE, YB_BACKBONE_RESNET, YB_BACKBONE_DARKNET = -1, 0, 1
 YB_PREC_F32, YB_PREC_F16TC, YB_PREC_F16X3 = 0, 1, 2
 PRECISIONS = {"f32": YB_PREC_F32, "f16tc": YB_PREC_F16TC, "f16x3": YB_PREC_F16X3}
@@ -80,6 +95,7 @@ SIGNATURES = {
                                c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "yb_postprocess_batch": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                      c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "yb_postprocess_list": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "yb_maskiou": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "yb_fast_base_transform": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                        POINTER(c_float), POINTER(c_float), c_void_p, c_void_p]),

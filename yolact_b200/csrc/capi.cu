@@ -415,6 +415,37 @@ int yb_postprocess_batch(yb_handle* h, const float* d_proto, int ph, int pw, int
   YB_API_END
 }
 
+int yb_postprocess_list(yb_handle* h, const yb_post_item* h_items, int B, int ph, int pw, int k, int crop_masks,
+                        int mask_format, void* stream) {
+  YB_API_BEGIN
+  YB_REQUIRE(h && B >= 0 && (B == 0 || h_items), "yb_postprocess_list: bad argument");
+  auto on_device = [h](const void* p) {
+    if (!p) return true;
+    cudaPointerAttributes a;
+    const bool found = cudaPointerGetAttributes(&a, p) == cudaSuccess;
+    if (!found) cudaGetLastError();   // not a pointer CUDA knows: clear the error, then reject
+    return found && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == h->device;
+  };
+  for (int b = 0; b < B; ++b) {
+    const yb_post_item& it = h_items[b];
+    YB_REQUIRE(it.n >= 0 && it.out_h > 0 && it.out_w > 0, "yb_postprocess_list: n must be >= 0 and out_h, out_w > 0");
+    YB_REQUIRE(it.n == 0 || (it.proto && it.coef && it.box), "yb_postprocess_list: null proto, coef or box");
+    YB_REQUIRE((reinterpret_cast<uintptr_t>(it.masks) & 15) == 0, "yb_postprocess_list: masks must be 16-byte aligned");
+    YB_REQUIRE(on_device(it.proto) && on_device(it.coef) && on_device(it.box) && on_device(it.masks) &&
+                   on_device(it.boxes_px) && on_device(it.proto_masks),
+               "yb_postprocess_list: a pointer is not device memory of the handle's device");
+  }
+  if (B == 0) return YB_OK;
+  CallGuard g(h, (cudaStream_t)stream);   // shared item table: ordered behind the previous call
+  yb_post_item* table = h->get_post_table(B);
+  // pageable source: staged before the call returns, so the caller may reuse h_items at once.  Stream-ordered after
+  // the previous call (CallGuard), so its launches have read the table before it is overwritten.
+  YB_CHECK_CUDA(cudaMemcpyAsync(table, h_items, (size_t)B * sizeof(yb_post_item), cudaMemcpyHostToDevice,
+                                (cudaStream_t)stream));
+  launch_mask_assembly_list(table, h_items, B, ph, pw, k, crop_masks, mask_format, (cudaStream_t)stream, &h->lc);
+  YB_API_END
+}
+
 int yb_maskiou(yb_handle* h, const float* d_proto_masks, int n, int ph, int pw, const int64_t* d_cls,
                float* d_maskiou, void* stream) {
   YB_API_BEGIN

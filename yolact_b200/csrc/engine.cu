@@ -879,6 +879,7 @@ yb_handle::~yb_handle() {
   for (void* p : weight_allocs) cudaFree(p);
   if (detect_ws) cudaFree(detect_ws);
   if (scratch) cudaFree(scratch);
+  if (post_table) cudaFree(post_table);
   if (cap_stream) cudaStreamDestroy(cap_stream);
   if (tune_stream) cudaStreamDestroy(tune_stream);
   for (auto s : lane_streams)
@@ -905,6 +906,22 @@ void* yb_handle::get_scratch(size_t bytes) {
     scratch_bytes = bytes;
   }
   return scratch;
+}
+
+// Grows by doubling; the old table is freed only after the device has drained, since a queued launch may still read it
+yb_post_item* yb_handle::get_post_table(int entries) {
+  if (entries > post_table_cap) {
+    const int cap = std::max(entries, std::max(16, 2 * post_table_cap));
+    if (post_table) {
+      YB_CHECK_CUDA(cudaDeviceSynchronize());
+      cudaFree(post_table);
+      post_table = nullptr;
+      post_table_cap = 0;
+    }
+    YB_CHECK_CUDA(cudaMalloc(&post_table, (size_t)cap * sizeof(yb_post_item)));
+    post_table_cap = cap;
+  }
+  return post_table;
 }
 
 void* yb_handle::get_detect_ws(size_t bytes) {

@@ -169,6 +169,8 @@ struct yb_handle {
   size_t detect_ws_bytes = 0;
   void* scratch = nullptr;   // maskiou / dcn / conv2d temporaries
   size_t scratch_bytes = 0;
+  yb_post_item* post_table = nullptr;   // yb_postprocess_list's device item table
+  int post_table_cap = 0;
   cudaStream_t cap_stream = nullptr;  // private stream used only for CUDA-graph capture
   cudaStream_t lane_streams[8] = {};  // branch streams joined into the capture (parallel graph branches)
   cudaEvent_t ev_fork = nullptr, ev_join[8] = {};
@@ -206,6 +208,7 @@ struct yb_handle {
                 cudaStream_t stream);
   void* get_scratch(size_t bytes);
   void* get_detect_ws(size_t bytes);
+  yb_post_item* get_post_table(int entries);
 };
 
 namespace yb {

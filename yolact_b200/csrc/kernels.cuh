@@ -171,6 +171,11 @@ void launch_mask_assembly(const float* proto, int ph, int pw, int k, const float
                           const float* box, int n, int out_h, int out_w, int crop, int mask_format,
                           void* masks, int64_t* boxes_px, float* proto_masks, cudaStream_t stream,
                           LaunchCounter* lc, int batch = 1);
+// the same for a list of B images of any sizes (yb_postprocess_list): d_items is the device copy of h_items, which the
+// host reads for the grid sizes.  One launch per kernel for the whole list: boxes (when an item has boxes_px),
+// prototype-resolution masks (when an item has proto_masks), masks (when an item has masks).
+void launch_mask_assembly_list(const yb_post_item* d_items, const yb_post_item* h_items, int B, int ph, int pw, int k,
+                               int crop, int mask_format, cudaStream_t stream, LaunchCounter* lc);
 // global max over HxW per (n, c) then gather channel cls[n] (yolact.py:373, output_utils.py:83)
 void launch_maxpool_gather(const float* x_nhwc, int n, int H, int W, int C, const int64_t* cls,
                            float* out, cudaStream_t stream, LaunchCounter* lc);

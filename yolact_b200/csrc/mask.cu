@@ -48,17 +48,38 @@ __device__ __forceinline__ void sanitize(float a, float b, int size, int padding
   *hi = fminf(__fadd_rn(mx, (float)padding), (float)size);
 }
 
-template <int FORMAT>
+// LIST = false: dense batch (yb_postprocess / yb_postprocess_batch), blockIdx.z = image, every per-image tensor dense.
+// LIST = true (yb_postprocess_list): blockIdx.z = image, whose tensors, row count and output size come from
+// items[blockIdx.z] in place of proto / coef / box / n / out_h / out_w / masks_v.  The grid and the shared-memory tables
+// are sized for the largest image of the list, so CTAs past this image's rows or detections exit at once; scale_h /
+// scale_w are computed as launch_mask_assembly computes them, so every pixel goes through the per-image arithmetic.
+// (items is the last parameter: the other instances keep their parameter layout.)
+template <int FORMAT, bool LIST>
 __global__ void __launch_bounds__(MT)
 mask_assembly_kernel(const float* __restrict__ proto, int ph, int pw, int k,
                      const float* __restrict__ coef, const float* __restrict__ box, int n, int out_h,
                      int out_w, int crop, int band, int group, int max_rows, float scale_h,
-                     float scale_w, void* __restrict__ masks_v, long long mask_img_stride_bytes) {
-  // blockIdx.z = image of the batch (yb_postprocess_batch); every per-image tensor is dense
-  proto += (size_t)blockIdx.z * ph * pw * k;
-  coef += (size_t)blockIdx.z * n * k;
-  box += (size_t)blockIdx.z * n * 4;
-  masks_v = reinterpret_cast<unsigned char*>(masks_v) + (size_t)blockIdx.z * mask_img_stride_bytes;
+                     float scale_w, void* __restrict__ masks_v, long long mask_img_stride_bytes,
+                     const yb_post_item* __restrict__ items) {
+  if constexpr (LIST) {
+    const yb_post_item it = items[blockIdx.z];
+    if (it.masks == nullptr || (int)blockIdx.x * band >= it.out_h || (int)blockIdx.y * group >= it.n) return;
+    proto = it.proto;
+    coef = it.coef;
+    box = it.box;
+    masks_v = it.masks;
+    n = it.n;
+    out_h = it.out_h;
+    out_w = it.out_w;
+    scale_h = __fdiv_rn((float)ph, (float)out_h);
+    scale_w = __fdiv_rn((float)pw, (float)out_w);
+  } else {
+    // blockIdx.z = image of the batch (yb_postprocess_batch); every per-image tensor is dense
+    proto += (size_t)blockIdx.z * ph * pw * k;
+    coef += (size_t)blockIdx.z * n * k;
+    box += (size_t)blockIdx.z * n * 4;
+    masks_v = reinterpret_cast<unsigned char*>(masks_v) + (size_t)blockIdx.z * mask_img_stride_bytes;
+  }
   extern __shared__ unsigned char smem_raw[];
   ColTab* coltab = reinterpret_cast<ColTab*>(smem_raw);                 // [out_w]
   float* mrows = reinterpret_cast<float*>(coltab + out_w);               // [max_rows][pw]
@@ -232,10 +253,8 @@ mask_assembly_kernel(const float* __restrict__ proto, int ph, int pw, int k,
 }
 
 // boxes: sanitize_coordinates(cast=False) for x with w, y with h, then .long() (output_utils.py:97-99)
-__global__ void boxes_px_kernel(const float* __restrict__ box, int n, int out_h, int out_w,
-                                int64_t* __restrict__ out) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;   // n = total boxes over the batch
-  if (i >= n) return;
+__device__ __forceinline__ void box_px(const float* __restrict__ box, int i, int out_h, int out_w,
+                                       int64_t* __restrict__ out) {
   float x1, x2, y1, y2;
   sanitize(box[i * 4 + 0], box[i * 4 + 2], out_w, 0, &x1, &x2);
   sanitize(box[i * 4 + 1], box[i * 4 + 3], out_h, 0, &y1, &y2);
@@ -245,13 +264,27 @@ __global__ void boxes_px_kernel(const float* __restrict__ box, int n, int out_h,
   out[i * 4 + 3] = (int64_t)y2;
 }
 
-// Cropped sigmoid masks at prototype resolution [n,ph,pw] (FastMaskIoUNet input, output_utils.py:77-82)
-__global__ void __launch_bounds__(MT)
-proto_masks_kernel(const float* __restrict__ proto, int ph, int pw, int k,
-                   const float* __restrict__ coef, const float* __restrict__ box, int crop,
-                   float* __restrict__ out) {
+__global__ void boxes_px_kernel(const float* __restrict__ box, int n, int out_h, int out_w,
+                                int64_t* __restrict__ out) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;   // n = total boxes over the batch
+  if (i >= n) return;
+  box_px(box, i, out_h, out_w, out);
+}
+
+// list source: blockIdx.y = image, each with its own rows and output size
+__global__ void boxes_px_list_kernel(const yb_post_item* __restrict__ items) {
+  const yb_post_item& it = items[blockIdx.y];
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (it.boxes_px == nullptr || i >= it.n) return;
+  box_px(it.box, i, it.out_h, it.out_w, it.boxes_px);
+}
+
+// Cropped sigmoid masks at prototype resolution [n,ph,pw] (FastMaskIoUNet input, output_utils.py:77-82): prototype
+// row r of detection d
+__device__ __forceinline__ void proto_masks_row(const float* __restrict__ proto, int ph, int pw, int k,
+                                                const float* __restrict__ coef, const float* __restrict__ box,
+                                                int crop, float* __restrict__ out, int r, int d) {
   __shared__ float s_coef[128];
-  const int r = blockIdx.x, d = blockIdx.y;
   for (int j = threadIdx.x; j < k; j += MT) s_coef[j] = coef[(size_t)d * k + j];
   __syncthreads();
   float cx1 = 0.f, cx2 = (float)pw, cy1 = 0.f, cy2 = (float)ph;
@@ -278,6 +311,22 @@ proto_masks_kernel(const float* __restrict__ proto, int ph, int pw, int k,
   }
 }
 
+__global__ void __launch_bounds__(MT)
+proto_masks_kernel(const float* __restrict__ proto, int ph, int pw, int k,
+                   const float* __restrict__ coef, const float* __restrict__ box, int crop,
+                   float* __restrict__ out) {
+  proto_masks_row(proto, ph, pw, k, coef, box, crop, out, blockIdx.x, blockIdx.y);
+}
+
+// list source: blockIdx.z = image; its rows land wherever items[z].proto_masks points (yb_postprocess_list's callers
+// point consecutive images at consecutive rows of one [sum n, ph, pw] buffer, so that maskiou_net runs once on all)
+__global__ void __launch_bounds__(MT)
+proto_masks_list_kernel(const yb_post_item* __restrict__ items, int ph, int pw, int k, int crop) {
+  const yb_post_item it = items[blockIdx.z];
+  if (it.proto_masks == nullptr || (int)blockIdx.y >= it.n) return;
+  proto_masks_row(it.proto, ph, pw, k, it.coef, it.box, crop, it.proto_masks, blockIdx.x, blockIdx.y);
+}
+
 // out[i] = max_{h,w} x[i,h,w,cls[i]]   (F.max_pool2d over the full map + gather);
 // cls == nullptr: out[i][c] for every channel (grid.y = C), i.e. FastMaskIoUNet.forward itself
 __global__ void maxpool_gather_kernel(const float* __restrict__ x, int HW, int C,
@@ -299,6 +348,29 @@ __global__ void maxpool_gather_kernel(const float* __restrict__ x, int HW, int C
     else
       out[(size_t)i * C + c] = r;
   }
+}
+
+// Rows per band (the largest of 8, 4, 2, 1 whose tables fit in 200 KB of shared memory), prototype rows per band and
+// dynamic shared memory of mask_assembly for an output width out_w and vertical scale scale_h = ph / out_h.
+void mask_band(float scale_h, int out_w, int pw, int* band, int* max_rows, size_t* smem) {
+  *band = 8;
+  for (;;) {
+    *max_rows = (int)((double)(*band - 1) * scale_h) + 4;
+    *smem = (size_t)out_w * sizeof(ColTab) + (size_t)*max_rows * pw * sizeof(float);
+    if (*smem <= 200 * 1024 || *band == 1) break;
+    *band = *band / 2;
+  }
+  YB_REQUIRE(*smem <= 200 * 1024, "mask_assembly: output too wide for the shared-memory tables");
+}
+
+// Detections per CTA: >= ~4 waves of 8 resident CTAs per SM, enough stores in flight to approach the HBM write rate
+// and a short tail (bands that cross many boxes take several times longer than empty ones); groups stay >= 8
+// detections so the band's prototype rows are reused from L1.
+int mask_group(int bands, int n, int batch) {
+  const int ctas_per_sm = 32;
+  int group = n;
+  while (group > 8 && (int64_t)bands * ceil_div(n, group) * batch < (int64_t)ctas_per_sm * 132) group = (group + 1) / 2;
+  return group;
 }
 
 }  // namespace
@@ -325,23 +397,11 @@ void launch_mask_assembly(const float* proto, int ph, int pw, int k, const float
   }
   if (masks) {
     YB_REQUIRE((reinterpret_cast<uintptr_t>(masks) & 15) == 0, "mask_assembly: masks must be 16-byte aligned");
-    int band = 8;
-    int max_rows;
+    int band, max_rows;
     size_t smem;
-    for (;;) {
-      max_rows = (int)((double)(band - 1) * scale_h) + 4;
-      smem = (size_t)out_w * sizeof(ColTab) + (size_t)max_rows * pw * sizeof(float);
-      if (smem <= 200 * 1024 || band == 1) break;
-      band = band / 2;
-    }
-    YB_REQUIRE(smem <= 200 * 1024, "mask_assembly: output too wide for the shared-memory tables");
+    mask_band(scale_h, out_w, pw, &band, &max_rows, &smem);
     const int bands = ceil_div(out_h, band);
-    // >= ~4 waves of 8 resident CTAs per SM: enough stores in flight to approach the HBM write rate and a short
-    // tail (bands that cross many boxes take several times longer than empty ones); groups stay >= 8 detections
-    // so the band's prototype rows are reused from L1.
-    const int ctas_per_sm = 32;
-    int group = n;
-    while (group > 8 && (int64_t)bands * ceil_div(n, group) * batch < (int64_t)ctas_per_sm * 132) group = (group + 1) / 2;
+    const int group = mask_group(bands, n, batch);
     dim3 grid(bands, ceil_div(n, group), batch);
     const size_t plane = (size_t)out_h * out_w;
     const long long img_stride = (long long)n * (mask_format == YB_MASK_F32 ? plane * 4
@@ -350,11 +410,12 @@ void launch_mask_assembly(const float* proto, int ph, int pw, int k, const float
 #define YB_LAUNCH_MASK(FMT)                                                                       \
   do {                                                                                            \
     if (smem > 48 * 1024)                                                                         \
-      YB_CHECK_CUDA(cudaFuncSetAttribute(mask_assembly_kernel<FMT>,                               \
+      YB_CHECK_CUDA(cudaFuncSetAttribute(mask_assembly_kernel<FMT, false>,                        \
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    mask_assembly_kernel<FMT><<<grid, MT, smem, stream>>>(proto, ph, pw, k, coef, box, n, out_h,  \
-                                                         out_w, crop, band, group, max_rows,     \
-                                                         scale_h, scale_w, masks, img_stride);   \
+    mask_assembly_kernel<FMT, false><<<grid, MT, smem, stream>>>(proto, ph, pw, k, coef, box, n,  \
+                                                                out_h, out_w, crop, band, group, \
+                                                                max_rows, scale_h, scale_w,      \
+                                                                masks, img_stride, nullptr);     \
   } while (0)
     switch (mask_format) {
       case YB_MASK_F32: YB_LAUNCH_MASK(YB_MASK_F32); break;
@@ -363,6 +424,68 @@ void launch_mask_assembly(const float* proto, int ph, int pw, int k, const float
       default: YB_REQUIRE(false, "mask_assembly: unknown mask format");
     }
 #undef YB_LAUNCH_MASK
+    YB_CHECK_LAUNCH();
+    if (lc) lc->n++;
+  }
+}
+
+void launch_mask_assembly_list(const yb_post_item* d_items, const yb_post_item* h_items, int B, int ph, int pw, int k,
+                               int crop, int mask_format, cudaStream_t stream, LaunchCounter* lc) {
+  YB_REQUIRE(k % 4 == 0 && k <= 128, "mask_assembly: mask_dim must be a multiple of 4 and <= 128");
+  YB_REQUIRE(ph > 0 && pw > 0, "mask_assembly: bad sizes");
+  YB_REQUIRE(mask_format == YB_MASK_F32 || mask_format == YB_MASK_U8 || mask_format == YB_MASK_BITS,
+             "mask_assembly: unknown mask format");
+  // the grid covers the most rows of any image; the masks' grid and shared-memory tables also the tallest and widest
+  // output and the largest vertical scale (the smallest out_h) among the images that want masks
+  int max_n = 0, mask_n = 0, max_h = 0, max_w = 0, min_h = 0;
+  bool any_boxes = false, any_pm = false;
+  for (int b = 0; b < B; ++b) {
+    const yb_post_item& it = h_items[b];
+    YB_REQUIRE(it.n >= 0 && it.out_h > 0 && it.out_w > 0, "mask_assembly: bad sizes");
+    if (it.n == 0) continue;
+    max_n = std::max(max_n, it.n);
+    any_boxes |= it.boxes_px != nullptr;
+    any_pm |= it.proto_masks != nullptr;
+    if (it.masks) {
+      YB_REQUIRE((reinterpret_cast<uintptr_t>(it.masks) & 15) == 0, "mask_assembly: masks must be 16-byte aligned");
+      mask_n = std::max(mask_n, it.n);
+      max_h = std::max(max_h, it.out_h);
+      max_w = std::max(max_w, it.out_w);
+      min_h = min_h ? std::min(min_h, it.out_h) : it.out_h;
+    }
+  }
+  if (any_boxes) {
+    boxes_px_list_kernel<<<dim3(ceil_div(max_n, 128), B), 128, 0, stream>>>(d_items);
+    YB_CHECK_LAUNCH();
+    if (lc) lc->n++;
+  }
+  if (any_pm) {
+    proto_masks_list_kernel<<<dim3(ph, max_n, B), MT, 0, stream>>>(d_items, ph, pw, k, crop);
+    YB_CHECK_LAUNCH();
+    if (lc) lc->n++;
+  }
+  if (mask_n > 0) {
+    int band, max_rows;
+    size_t smem;
+    mask_band((float)ph / (float)min_h, max_w, pw, &band, &max_rows, &smem);
+    const int bands = ceil_div(max_h, band);
+    const int group = mask_group(bands, mask_n, B);
+    const dim3 grid(bands, ceil_div(mask_n, group), B);
+#define YB_LAUNCH_MASK_LIST(FMT)                                                                            \
+  do {                                                                                                      \
+    if (smem > 48 * 1024)                                                                                   \
+      YB_CHECK_CUDA(cudaFuncSetAttribute(mask_assembly_kernel<FMT, true>,                                   \
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));          \
+    mask_assembly_kernel<FMT, true><<<grid, MT, smem, stream>>>(nullptr, ph, pw, k, nullptr, nullptr, 0, 0, \
+                                                                0, crop, band, group, max_rows, 0.f, 0.f,  \
+                                                                nullptr, 0, d_items);                      \
+  } while (0)
+    switch (mask_format) {
+      case YB_MASK_F32: YB_LAUNCH_MASK_LIST(YB_MASK_F32); break;
+      case YB_MASK_U8: YB_LAUNCH_MASK_LIST(YB_MASK_U8); break;
+      default: YB_LAUNCH_MASK_LIST(YB_MASK_BITS); break;
+    }
+#undef YB_LAUNCH_MASK_LIST
     YB_CHECK_LAUNCH();
     if (lc) lc->n++;
   }

@@ -14,6 +14,9 @@ Differences (documented in INTEGRATION.md): the reference writes the sanitised a
 into det_output['box'] in place (output_utils.py:97-98, SURVEY.md Appendix D.1); this function
 leaves its input untouched.  `mask_format` ('f32' | 'u8' | 'bits') is an extension: 'bits' returns
 uint32 words, 1 bit per pixel, row pitch ceil(w/32) -- 32x less HBM/PCIe traffic than fp32.
+
+postprocess_list(det_output, sizes, ...) is postprocess for every image of a list at its own size (a folder of images
+through Yolact.forward_frames), in one call with one launch per kernel for the whole list.
 """
 import ctypes
 
@@ -157,6 +160,146 @@ def postprocess(det_output, w, h, batch_idx=0, interpolation_mode='bilinear', vi
         _, boxes_px, _ = _boxes_only(boxes, h, w)
 
     return classes, scores, boxes_px, masks
+
+
+def postprocess_list(det_output, sizes, interpolation_mode='bilinear', visualize_lincomb=False, crop_masks=True,
+                     score_threshold=0, mask_format="f32"):
+    """postprocess for every image of det_output at its own size, in one call:
+    [postprocess(det_output, w_i, h_i, i, ...) for i, (h_i, w_i) in enumerate(sizes)], bit for bit, and det_output is
+    left as those calls leave it.  sizes[i] = (h_i, w_i), i.e. frame i's shape[:2] -- what Yolact.forward_frames' list
+    of differently sized frames needs back.
+
+    One yb_postprocess_list call covers the whole list (boxes and masks, plus the prototype-resolution masks of
+    YOLACT++), and YOLACT++ runs maskiou_net once over the rows of all images, so the launches do not grow with the
+    list.  With score_threshold == 0 there is no host sync; with score_threshold > 0 there is one, for the kept-row
+    counts of all images together.  The threshold keeps each image's leading rows (Detect's scores are descending):
+    rows that are not a prefix raise ValueError rather than silently differ from postprocess."""
+    if len(sizes) != len(det_output):
+        raise ValueError("postprocess_list: %d sizes for %d images" % (len(sizes), len(det_output)))
+    hw = []
+    for s in sizes:
+        h, w = (int(v) for v in s)
+        if h <= 0 or w <= 0:
+            raise ValueError("postprocess_list: image sizes must be positive, got %s" % (tuple(s),))
+        hw.append((h, w))
+    empty = [torch.Tensor()] * 4   # output_utils.py:39-40,49-50
+    live = [i for i, d in enumerate(det_output) if d['detection'] is not None]
+    for i in live:
+        if not det_output[i]['detection']['box'].is_cuda:
+            raise _lib.YbError("yolact_b200.postprocess runs on CUDA (H100) only; there is no CPU path.")
+    dev = det_output[live[0]]['detection']['box'].device if live else None
+
+    if score_threshold > 0 and live:
+        _keep_leading_rows(det_output, live, score_threshold, dev)
+        live = [i for i in live if det_output[i]['detection']['score'].size(0) > 0]
+    out = [empty] * len(det_output)
+    if not live:
+        return out
+
+    cfg = _config.cfg
+    dets = [det_output[i]['detection'] for i in live]
+    with_proto = ['proto' in d for d in dets]
+    if any(with_proto) and not all(with_proto):
+        raise ValueError("postprocess_list: some detections carry 'proto' and some do not")
+    eval_mask_branch = getattr(cfg, "eval_mask_branch", True) and with_proto[0]
+    lib = _lib.load()
+    stream = _lib.current_stream(dev)
+    ns = [int(d['box'].shape[0]) for d in dets]
+    keep_alive = []   # the contiguous inputs, held until the call has enqueued its reads of them
+    items = (_lib.YbPostItem * len(dets))()
+
+    if not eval_mask_branch:
+        # cfg.eval_mask_branch == False (--detect): boxes only, masks are the raw coefficients (Appendix D.15)
+        dummy = torch.empty(4, dtype=torch.float32, device=dev)   # never read without masks
+        for j, (i, d, n) in enumerate(zip(live, dets, ns)):
+            box = d['box'].contiguous().float()
+            boxes_px = torch.empty(n, 4, dtype=torch.int64, device=dev)
+            keep_alive.append(box)
+            items[j] = _lib.YbPostItem(dummy.data_ptr(), dummy.data_ptr(), box.data_ptr(), None, boxes_px.data_ptr(),
+                                       None, n, hw[i][0], hw[i][1])
+            out[i] = (d['class'], d['score'], boxes_px, d['mask'])
+        _lib.check(lib.yb_postprocess_list(_ops_handle(dev, 4), items, len(dets), 1, 1, 4, 0, _lib.YB_MASK_F32, stream),
+                   "yb_postprocess_list(boxes)")
+        return out
+
+    if interpolation_mode != 'bilinear':
+        raise NotImplementedError("yolact_b200.postprocess implements bilinear upsampling only "
+                                  "(the only mode eval.py uses)")
+    if visualize_lincomb:
+        raise NotImplementedError("display_lincomb (debug visualisation) is out of scope")
+    shapes = {tuple(int(s) for s in d['proto'].shape) for d in dets}
+    if len(shapes) != 1:
+        raise ValueError("postprocess_list: the images' prototypes differ in (ph, pw, k): %s" % sorted(shapes))
+    ph, pw, k = shapes.pop()
+    net = det_output[live[0]]['net']
+    ncfg = getattr(net, "cfg", cfg)
+    use_maskiou = bool(getattr(ncfg, "use_maskiou", False))
+    if use_maskiou and any(det_output[i]['net'] is not net for i in live):
+        raise ValueError("postprocess_list: maskiou rescoring needs every image to come from the same net")
+    fmt = _FORMATS[mask_format]
+    pm = torch.empty(sum(ns), ph, pw, dtype=torch.float32, device=dev) if use_maskiou else None
+    off = 0
+    for j, (i, d, n) in enumerate(zip(live, dets, ns)):
+        h, w = hw[i]
+        proto, coef, box = d['proto'].contiguous().float(), d['mask'].contiguous().float(), d['box'].contiguous().float()
+        if fmt == _lib.YB_MASK_F32:
+            masks = torch.empty(n, h, w, dtype=torch.float32, device=dev)
+        elif fmt == _lib.YB_MASK_U8:
+            masks = torch.empty(n, h, w, dtype=torch.uint8, device=dev)
+        else:
+            masks = torch.empty(n, h, (w + 31) // 32, dtype=torch.int32, device=dev)
+        boxes_px = torch.empty(n, 4, dtype=torch.int64, device=dev)
+        keep_alive += [proto, coef, box]
+        items[j] = _lib.YbPostItem(proto.data_ptr(), coef.data_ptr(), box.data_ptr(), masks.data_ptr() or None,
+                                   boxes_px.data_ptr() or None, pm[off:off + n].data_ptr() if use_maskiou else None,
+                                   n, h, w)
+        out[i] = (d['class'], d['score'], boxes_px, masks)
+        off += n
+    _lib.check(lib.yb_postprocess_list(_ops_handle(dev, k), items, len(dets), ph, pw, k, 1 if crop_masks else 0, fmt,
+                                       stream), "yb_postprocess_list")
+
+    if use_maskiou and off > 0:
+        # output_utils.py:79-88 over the rows of every image at once: maskiou_net and the gather are per row
+        cat = (lambda ts: torch.cat(ts)) if len(dets) > 1 else (lambda ts: ts[0])
+        cls64 = cat([d['class'] for d in dets]).contiguous().long()
+        miou = torch.empty(off, dtype=torch.float32, device=dev)
+        _lib.check(lib.yb_maskiou(net._handle_for(dev), _lib.ptr(pm), off, ph, pw, _lib.ptr(cls64), _lib.ptr(miou),
+                                  stream), "yb_maskiou")
+        if getattr(ncfg, "rescore_mask", False):
+            rescored = cat([d['score'] for d in dets]) * miou
+            bbox = getattr(cfg, "rescore_bbox", False) or getattr(ncfg, "rescore_bbox", False)
+            off = 0
+            for i, d, n in zip(live, dets, ns):
+                r = rescored[off:off + n]
+                out[i] = (d['class'], r if bbox else [d['score'], r]) + out[i][2:]
+                off += n
+    return out
+
+
+def _keep_leading_rows(det_output, live, score_threshold, dev):
+    """postprocess's `dets[k] = dets[k][dets['score'] > score_threshold]` for every live image, with ONE host sync:
+    the kept-row counts of all images are computed together, and each image keeps that many leading rows.  Raises
+    ValueError (before changing anything) when an image's kept rows are not its leading rows."""
+    scores = [det_output[i]['detection']['score'] for i in live]
+    lens = [int(s.shape[0]) for s in scores]
+    flat = torch.cat(scores) if len(scores) > 1 else scores[0]
+    keep = flat > score_threshold
+    # image index and row index of every row, built on the host from the shapes and uploaded without a sync
+    seg_pos = torch.stack([torch.repeat_interleave(torch.arange(len(lens)), torch.tensor(lens)),
+                           torch.cat([torch.arange(n) for n in lens])]).to(dev, non_blocking=True)
+    seg, pos = seg_pos[0], seg_pos[1]
+    counts = torch.zeros(len(lens), dtype=torch.int64, device=dev).index_add_(0, seg, keep.long())
+    stray = torch.zeros(len(lens), dtype=torch.int64, device=dev).index_add_(0, seg, (keep != (pos < counts[seg])).long())
+    counts, stray = torch.stack([counts, stray]).tolist()   # the one host sync
+    for i, n, bad in zip(live, counts, stray):
+        if bad:
+            raise ValueError("postprocess_list: score_threshold keeps rows of image %d that are not its leading rows "
+                             "(its scores are not in descending order); run postprocess on it" % i)
+    for i, n in zip(live, counts):
+        dets = det_output[i]['detection']
+        for k in dets:
+            if k != 'proto':
+                dets[k] = dets[k][:n]
 
 
 def _boxes_only(boxes, h, w):
