@@ -203,9 +203,9 @@ YB_API int yb_infer(yb_handle* h, const float* d_x, int B, int H, int W, int cro
  * img_is_u8 = 1, out_h, out_w, mode, h_mean_bgr, h_std_bgr; NULL = MEANS / STD) and run through the network and Detect
  * as yb_infer(out_h, out_w) does, with the same outputs, bit for bit.  In the tensor-core modes the transform happens
  * inside the stem's operand loader, so no [B,3,out_h,out_w] fp32 input is written; in YB_PREC_F32 it runs as one
- * more kernel in the graph.  Replayed as one CUDA graph per frame size, transform and NMS mode.  Each (B, out_h, out_w)
- * keeps the buffers and graphs of its 4 most recently used frame sizes / transforms; the first call with another one
- * allocates (and, past four, synchronises the device to free the least recently used). */
+ * more kernel in the graph.  The frames are read in place on `stream` (not copied), as the list of B frames
+ * yb_infer_frame_list takes, H * W * 3 bytes apart; each (B, out_h, out_w) replays one CUDA graph per transform and
+ * NMS mode for any frame size.  YB_ERR_INVALID if d_img is not device memory of the handle's device. */
 YB_API int yb_infer_frames(yb_handle* h, const uint8_t* d_img, int B, int H, int W, int out_h, int out_w, int mode,
                            const float* h_mean_bgr, const float* h_std_bgr, int cross_class, int max_out,
                            float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count,

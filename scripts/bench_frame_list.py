@@ -1,7 +1,6 @@
 """Time per image of a folder of differently sized images (COCO-like sizes) through yolact_base at 550^2, three ways:
 
-  (a) Yolact.infer_frames(f[None]) per image: batch 1, one frame-size input per size (4 kept per network input size,
-      so with 16 sizes nearly every call synchronises the device, allocates and runs eagerly);
+  (a) Yolact.infer_frames(f[None]) per image: batch 1, one call and one graph launch per image;
   (b) FastBaseTransform per image + torch.cat + Yolact.infer_padded at batch 8;
   (c) Yolact.infer_frames(list of 8 frames): one call and one graph whatever the sizes.
 

@@ -231,3 +231,25 @@ def test_frame_list_c_abi_rejects_bad_frames():
     assert call([f.data_ptr(), host.ctypes.data], [64, 80, 64, 80]) == YB_ERR_INVALID
     torch.cuda.synchronize()
     assert net.infer_frames([f, f]) is not None   # the handle is still usable
+
+
+def test_frames_c_abi_rejects_host_memory():
+    """yb_infer_frames reads its batch in place: a host d_img is refused before anything runs."""
+    net = make_net("yolact_resnet50_config", "f16x3")
+    lib = _lib.load()
+    dev = torch.device("cuda", torch.cuda.current_device())
+    h = net._handle_for(dev)
+    mode, M, out = net._detect_outputs(h, dev, 2, SIZE, SIZE, None)
+    f = torch.stack([frame(64, 80, 231), frame(64, 80, 232)])
+    host = np.zeros((2, 64, 80, 3), np.uint8)
+    mean = (ctypes.c_float * 3)(*yolact_b200.config.MEANS)
+    std = (ctypes.c_float * 3)(*yolact_b200.config.STD)
+
+    def call(ptr):
+        return lib.yb_infer_frames(h, ptr, 2, 64, 80, SIZE, SIZE, _lib.YB_XFORM_NORMALIZE, mean, std, mode, M,
+                                   *[_lib.ptr(t) for t in out], _lib.current_stream(dev))
+
+    assert call(f.data_ptr()) == 0, lib.yb_last_error()
+    assert call(host.ctypes.data) == YB_ERR_INVALID
+    torch.cuda.synchronize()
+    assert net.infer_frames(f) is not None   # the handle is still usable

@@ -118,9 +118,9 @@ def test_graph_replay_and_isolation_between_frame_sizes_and_infer_padded():
 
 
 
-def test_frame_sizes_beyond_the_held_ones_are_dropped_and_rebuilt():
-    """One network input size holds a few frame sizes; cycling through more drops the least recently used, and coming
-    back to a dropped size rebuilds it with the same results."""
+def test_many_frame_sizes_share_one_input_and_repeat_their_results():
+    """One network input size serves any number of frame sizes: cycling through six of them, then through them again,
+    gives the same results both times and the same as the two-call path."""
     net = make_net("yolact_resnet50_config", "f16x3")
     fs = [frames(1, 100 + 7 * i, 140 + 5 * i, 60 + i) for i in range(6)]
     first = [net.infer_frames(f) for f in fs]

@@ -118,6 +118,15 @@ const float kStd[3] = {57.38f, 57.12f, 58.40f};
 
 inline int grid1d(int64_t n) { return (int)std::min<int64_t>(132 * 16, (n + 255) / 256); }
 
+// The frame inputs are read in place by the network's kernels: YB_ERR_INVALID unless frame is device (or managed)
+// memory of the handle's device.
+void require_device_frame(const yb_handle* h, const void* frame, const char* msg) {
+  cudaPointerAttributes a;
+  const bool found = cudaPointerGetAttributes(&a, frame) == cudaSuccess;
+  if (!found) cudaGetLastError();   // not a pointer CUDA knows: clear the error, then reject
+  YB_REQUIRE(found && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == h->device, msg);
+}
+
 }  // namespace
 
 extern "C" {
@@ -280,9 +289,19 @@ int yb_infer_frames(yb_handle* h, const uint8_t* d_img, int B, int H, int W, int
   YB_REQUIRE(!h->ops_only, "yb_infer_frames: handle has no network");
   YB_REQUIRE(d_box && d_coef_out && d_cls && d_score && d_count, "yb_infer_frames: null output");
   YB_REQUIRE(mode >= YB_XFORM_NORMALIZE && mode <= YB_XFORM_NONE, "yb_infer_frames: unknown transform mode");
-  CallGuard g(h, (cudaStream_t)stream);   // shared workspaces: ordered behind the previous call
-  h->infer_frames(d_img, B, H, W, out_h, out_w, mode, h_mean_bgr ? h_mean_bgr : kMeans, h_std_bgr ? h_std_bgr : kStd,
-                  cross_class, max_out, d_box, d_coef_out, d_cls, d_score, d_count, d_proto, (cudaStream_t)stream);
+  require_device_frame(h, d_img, "yb_infer_frames: the frames are not device memory of the handle's device");
+  // a frame list whose B entries lie H * W * 3 bytes apart
+  std::vector<const uint8_t*> frames(B);
+  std::vector<int32_t> hw(2 * (size_t)B);
+  for (int b = 0; b < B; ++b) {
+    frames[b] = d_img + (size_t)b * H * W * 3;
+    hw[2 * b] = H;
+    hw[2 * b + 1] = W;
+  }
+  CallGuard g(h, (cudaStream_t)stream);   // shared workspaces and frame table: ordered behind the previous call
+  h->infer_frame_list(frames.data(), hw.data(), B, out_h, out_w, mode, h_mean_bgr ? h_mean_bgr : kMeans,
+                      h_std_bgr ? h_std_bgr : kStd, cross_class, max_out, d_box, d_coef_out, d_cls, d_score, d_count,
+                      d_proto, (cudaStream_t)stream);
   YB_API_END
 }
 
@@ -298,11 +317,7 @@ int yb_infer_frame_list(yb_handle* h, const uint8_t* const* h_frames, const int3
   for (int b = 0; b < B; ++b) {
     YB_REQUIRE(h_frames[b], "yb_infer_frame_list: null frame pointer");
     YB_REQUIRE(h_hw[2 * b] > 0 && h_hw[2 * b + 1] > 0, "yb_infer_frame_list: frame height and width must be positive");
-    cudaPointerAttributes a;
-    const bool found = cudaPointerGetAttributes(&a, h_frames[b]) == cudaSuccess;
-    if (!found) cudaGetLastError();   // not a pointer CUDA knows: clear the error, then reject
-    YB_REQUIRE(found && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == h->device,
-               "yb_infer_frame_list: a frame is not device memory of the handle's device");
+    require_device_frame(h, h_frames[b], "yb_infer_frame_list: a frame is not device memory of the handle's device");
   }
   CallGuard g(h, (cudaStream_t)stream);   // shared workspaces and frame table: ordered behind the previous call
   h->infer_frame_list(h_frames, h_hw, B, out_h, out_w, mode, h_mean_bgr ? h_mean_bgr : kMeans,

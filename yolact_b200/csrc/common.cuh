@@ -136,7 +136,7 @@ __device__ __forceinline__ float apply_act(float v, int act) {
 }
 
 // ---- FastBaseTransform's per-pixel arithmetic (utils/augmentations.py:616-658) ---------------------------------------
-// The only definition: evalops.cu's fast_base_transform_kernel writes it to an NCHW fp32 tensor, the frame-source stem
+// The only definition: evalops.cu's fast_base_transform_kernel writes it to an NCHW fp32 tensor, the frame-list stem
 // (stem_tc.cu) computes it inside its loader, so both give the network bit for bit the same input.
 struct XformAffine {   // BGR order
   float mean[3];

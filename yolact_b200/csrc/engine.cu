@@ -27,12 +27,11 @@ void Executor::drop_detect_state() {
   for (auto& kv : infer_graphs)
     if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   infer_graphs.clear();
-  for (auto* inputs : {&frame_inputs, &frame_list_inputs})
-    for (auto& fi : *inputs) {
-      for (auto& kv : fi.second.graphs)
-        if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-      fi.second.graphs.clear();
-    }
+  for (auto& fi : frame_inputs) {
+    for (auto& kv : fi.second.graphs)
+      if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+    fi.second.graphs.clear();
+  }
   void* bufs[6] = {det_ws, det_box, det_coef, det_cls, det_score, det_count};
   for (void* b : bufs) {
     if (!b) continue;
@@ -47,28 +46,13 @@ void Executor::drop_detect_state() {
   det_cap = 0;
 }
 
-void Executor::drop_frame_input(std::map<std::string, FrameInput>::iterator it) {
-  YB_CHECK_CUDA(cudaDeviceSynchronize());   // the buffer may still be read by an earlier replay
-  FrameInput& fi = it->second;
-  for (auto& kv : fi.graphs)
-    if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-  if (fi.stem) {
-    stem_plans.erase(std::find(stem_plans.begin(), stem_plans.end(), fi.stem));
-    stem_tc_plan_destroy(fi.stem);
-  }
-  allocs.erase(std::find(allocs.begin(), allocs.end(), (void*)fi.d_frames));
-  cudaFree(fi.d_frames);
-  frame_inputs.erase(it);
-}
-
 Executor::~Executor() {
   if (graph_fwd) cudaGraphExecDestroy(graph_fwd);
   for (auto& kv : infer_graphs)
     if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-  for (auto* inputs : {&frame_inputs, &frame_list_inputs})
-    for (auto& fi : *inputs)
-      for (auto& kv : fi.second.graphs)
-        if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+  for (auto& fi : frame_inputs)
+    for (auto& kv : fi.second.graphs)
+      if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   for (auto* c : chains) tc_chain_destroy(c);
   for (auto* p : plans) tc_conv_plan_destroy(p);
   for (auto* p : stem_plans) stem_tc_plan_destroy(p);
@@ -301,7 +285,7 @@ struct NetBuilder {
     op.name = key + " " + std::to_string(in.C) + "->" + std::to_string(w.Cout) + " k" + std::to_string(k) + "s" +
               std::to_string(stride) + " " + std::to_string(p.Ho) + "x" + std::to_string(p.Wo);
     if (stem_tc) {
-      // yb_infer_frames replaces ops[0] with the frame-source stem
+      // yb_infer_frame_list replaces ops[0] with the frame-list stem
       YB_REQUIRE(ex->ops.empty() && ex->stem_plans.empty(), ("conv " + key + ": the stem must be the first op").c_str());
       StemTcPlan* sp = stem_tc_plan_create((const float*)in.ptr, w.w_tc, w.bias, (__half*)out.ptr, in.B, in.H, in.W, k,
                                            stride, pad, w.Cout, act, split ? 1 : 0, w.out_scale, out.C);
@@ -1147,7 +1131,7 @@ Executor* yb_handle::get_executor(int B, int H, int W) {
   return raw;
 }
 
-// fin (yb_infer_frames / yb_infer_frame_list): its entry op runs first, in place of ops[0] when it replaces the stem
+// fin (yb_infer_frame_list): its entry op runs first, in place of ops[0] when it replaces the stem
 static void run_ops(yb_handle* h, Executor* ex, cudaStream_t stream, bool branches = false,
                     const Executor::FrameInput* fin = nullptr) {
   static const bool trace = getenv("YB_TRACE") != nullptr;   // debug: name every op and sync after it
@@ -1267,49 +1251,6 @@ void yb_handle::infer(const float* d_x, int B, int H, int W, int cross_class, in
   infer_on(ex, nullptr, d_x, cross_class, max_out, d_box, d_coef_out, d_cls, d_score, d_count, d_proto, stream);
 }
 
-void yb_handle::infer_frames(const uint8_t* d_img, int B, int fh, int fw, int H, int W, int mode,
-                             const float* mean_bgr, const float* std_bgr, int cross_class, int max_out, float* d_box,
-                             float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto,
-                             cudaStream_t stream) {
-  Executor* ex = get_executor(B, H, W);
-  char key[256];
-  snprintf(key, sizeof(key), "%dx%d m%d %a %a %a / %a %a %a", fh, fw, mode, mean_bgr[0], mean_bgr[1], mean_bgr[2],
-           std_bgr[0], std_bgr[1], std_bgr[2]);
-  auto it = ex->frame_inputs.find(key);
-  if (it == ex->frame_inputs.end()) {
-    if (ex->frame_inputs.size() >= Executor::kMaxFrameInputs)
-      ex->drop_frame_input(std::min_element(ex->frame_inputs.begin(), ex->frame_inputs.end(), [](auto& a, auto& b) {
-        return a.second.last_use < b.second.last_use;
-      }));
-    Executor::FrameInput fi;
-    fi.d_frames = (uint8_t*)dmalloc(ex->allocs, (size_t)B * fh * fw * 3);
-    fi.fh = fh;
-    fi.fw = fw;
-    LaunchCounter* lc = &this->lc;
-    if (cfg.precision == YB_PREC_F32) {
-      // no tensor-core stem to fuse into: FastBaseTransform into d_in, then the network's own stem
-      const uint8_t* img = fi.d_frames;
-      float* d_in = ex->d_in;
-      std::array<float, 3> mean{mean_bgr[0], mean_bgr[1], mean_bgr[2]}, stdv{std_bgr[0], std_bgr[1], std_bgr[2]};
-      fi.entry.name = "fast_base_transform " + std::to_string(fh) + "x" + std::to_string(fw);
-      fi.entry.fn = [=](cudaStream_t s) {
-        launch_fast_base_transform(img, 1, B, fh, fw, H, W, mode, mean.data(), stdv.data(), d_in, s, lc);
-      };
-    } else {
-      YB_REQUIRE(!ex->stem_plans.empty() && !ex->ops.empty(), "yb_infer_frames: the network has no tensor-core stem");
-      StemTcPlan* sp = stem_tc_plan_create_frames(ex->stem_plans[0], fi.d_frames, fh, fw, mode, mean_bgr, std_bgr);
-      ex->stem_plans.push_back(sp);
-      fi.stem = sp;
-      fi.entry.name = ex->ops[0].name + " frames " + std::to_string(fh) + "x" + std::to_string(fw);
-      fi.entry.fn = [sp, lc](cudaStream_t s) { launch_stem_tc(sp, s, lc); };
-      fi.replaces_stem = true;
-    }
-    it = ex->frame_inputs.emplace(key, std::move(fi)).first;
-  }
-  it->second.last_use = ++ex->frame_clock;
-  infer_on(ex, &it->second, d_img, cross_class, max_out, d_box, d_coef_out, d_cls, d_score, d_count, d_proto, stream);
-}
-
 void yb_handle::infer_frame_list(const uint8_t* const* frames, const int32_t* hw, int B, int H, int W, int mode,
                                  const float* mean_bgr, const float* std_bgr, int cross_class, int max_out,
                                  float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count,
@@ -1319,8 +1260,8 @@ void yb_handle::infer_frame_list(const uint8_t* const* frames, const int32_t* hw
   char key[256];
   snprintf(key, sizeof(key), "m%d %a %a %a / %a %a %a", mode, mean_bgr[0], mean_bgr[1], mean_bgr[2], std_bgr[0],
            std_bgr[1], std_bgr[2]);
-  auto it = ex->frame_list_inputs.find(key);
-  if (it == ex->frame_list_inputs.end()) {
+  auto it = ex->frame_inputs.find(key);
+  if (it == ex->frame_inputs.end()) {
     Executor::FrameInput fi;
     LaunchCounter* lc = &this->lc;
     const FrameRef* table = ex->d_frame_table;
@@ -1341,7 +1282,7 @@ void yb_handle::infer_frame_list(const uint8_t* const* frames, const int32_t* hw
       fi.entry.fn = [sp, lc](cudaStream_t s) { launch_stem_tc(sp, s, lc); };
       fi.replaces_stem = true;
     }
-    it = ex->frame_list_inputs.emplace(key, std::move(fi)).first;
+    it = ex->frame_inputs.emplace(key, std::move(fi)).first;
   }
   // one entry per image, pointing at the caller's frame: nothing is copied but the table itself
   std::vector<FrameRef> table(B);
@@ -1350,9 +1291,8 @@ void yb_handle::infer_frame_list(const uint8_t* const* frames, const int32_t* hw
            stream);
 }
 
-// Forward + Detect on an executor; fin == null takes NCHW fp32 input d_x into d_in, otherwise uint8 frames d_x into
-// fin->d_frames, or for a frame list (fin->d_frames == null) the host FrameRef table d_x into ex->d_frame_table.  Each
-// input keeps its own captured graphs.
+// Forward + Detect on an executor; fin == null takes NCHW fp32 input d_x into d_in, otherwise the host FrameRef table
+// d_x into ex->d_frame_table.  Each input keeps its own captured graphs.
 void yb_handle::infer_on(Executor* ex, Executor::FrameInput* fin, const void* d_x, int cross_class, int max_out,
                          float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count,
                          float* d_proto, cudaStream_t stream) {
@@ -1391,13 +1331,10 @@ void yb_handle::infer_on(Executor* ex, Executor::FrameInput* fin, const void* d_
     launch_detect(dp, ex->loc, ex->conf, ex->coef, ex->priors, ex->dws, ex->det_box, ex->det_coef, ex->det_cls,
                   ex->det_score, ex->det_count, s, &lc);
   };
-  if (fin && !fin->d_frames)
+  if (fin)
     // pageable source: staged before the call returns, so the host table may go away at once.  Stream-ordered after
     // the previous call (CallGuard), so an earlier replay has read the table before it is overwritten.
     YB_CHECK_CUDA(cudaMemcpyAsync(ex->d_frame_table, d_x, (size_t)B * sizeof(FrameRef), cudaMemcpyHostToDevice, stream));
-  else if (fin)
-    YB_CHECK_CUDA(cudaMemcpyAsync(fin->d_frames, d_x, (size_t)B * fin->fh * fin->fw * 3, cudaMemcpyDeviceToDevice,
-                                  stream));
   else
     YB_CHECK_CUDA(cudaMemcpyAsync(ex->d_in, d_x, (size_t)B * 3 * H * W * 4, cudaMemcpyDeviceToDevice, stream));
   last_exec = ex;

@@ -115,31 +115,20 @@ struct Executor {
   cudaGraphExec_t graph_fwd = nullptr;
   std::map<int, InferGraph> infer_graphs;
   int fwd_calls = 0;
-  // uint8 frame input (yb_infer_frames), one per frame size, transform mode, mean and std.  The frames replace only
-  // the input: the half modes run the frame-source stem in place of ops[0], f32 runs fast_base_transform into d_in
+  // uint8 frame input (yb_infer_frame_list, and yb_infer_frames as a list of equally sized frames), one per transform
+  // mode, mean and std.  Every image brings its own frame and size; the entry op reads them from d_frame_table (B
+  // entries, uploaded before each call), so no buffer, plan or graph depends on a frame size.  The frames replace only
+  // the input: the half modes run the frame-list stem in place of ops[0], f32 runs fast_base_transform into d_in
   // ahead of ops[0]; every other op, plan and chain is this executor's.
   struct FrameInput {
-    uint8_t* d_frames = nullptr;   // [B,fh,fw,3] copy of the caller's frames (stable address for graph replay);
-                                   // null for a frame list, whose entry reads d_frame_table
-    int fh = 0, fw = 0;
     Op entry;                      // the frame stem, or fast_base_transform in YB_PREC_F32
     StemTcPlan* stem = nullptr;    // the frame stem's plan (half modes; also listed in stem_plans)
     bool replaces_stem = false;    // entry runs instead of ops[0] (half modes) or before it (f32)
     std::map<int, InferGraph> graphs;   // keyed like infer_graphs
-    uint64_t last_use = 0;
   };
-  // A folder of images gives nearly every call its own frame size: at most kMaxFrameInputs are kept, and a new one
-  // beyond that synchronises the device and drops the least recently used.
-  static constexpr size_t kMaxFrameInputs = 4;
-  std::map<std::string, FrameInput> frame_inputs;
-  uint64_t frame_clock = 0;
-  void drop_frame_input(std::map<std::string, FrameInput>::iterator it);   // frees its buffer, plan and graphs
-  // Frame lists (yb_infer_frame_list): every image brings its own frame and size.  The entry op reads them from
-  // d_frame_table (B entries, uploaded before each call), so a FrameInput here has no d_frames and is keyed by the
-  // transform alone (mode, mean, std): no buffer, plan or graph depends on a frame size.
   FrameRef* d_frame_table = nullptr;
-  std::map<std::string, FrameInput> frame_list_inputs;
-  void drop_detect_state();      // frees the Detect buffers and every captured yb_infer / yb_infer_frames(_list) graph
+  std::map<std::string, FrameInput> frame_inputs;
+  void drop_detect_state();      // frees the Detect buffers and every captured yb_infer / yb_infer_frame_list graph
   ~Executor();
 };
 
@@ -194,11 +183,8 @@ struct yb_handle {
                cudaStream_t stream);
   void infer(const float* d_x, int B, int H, int W, int cross_class, int max_out, float* d_box, float* d_coef_out,
              int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto, cudaStream_t stream);
-  // infer on [B,fh,fw,3] uint8 BGR frames, FastBaseTransform'ed to H x W on the way in (same executor as infer(B,H,W))
-  void infer_frames(const uint8_t* d_img, int B, int fh, int fw, int H, int W, int mode, const float* mean_bgr,
-                    const float* std_bgr, int cross_class, int max_out, float* d_box, float* d_coef_out,
-                    int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto, cudaStream_t stream);
   // infer on a list of B uint8 BGR frames of any sizes: frames[b] is a device [hw[2b], hw[2b+1], 3] frame, read in place
+  // and FastBaseTransform'ed to H x W on the way in (same executor as infer(B,H,W))
   void infer_frame_list(const uint8_t* const* frames, const int32_t* hw, int B, int H, int W, int mode,
                         const float* mean_bgr, const float* std_bgr, int cross_class, int max_out, float* d_box,
                         float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto,

@@ -21,7 +21,7 @@ namespace {
 // -------------------------------------------------------------------------------------------------
 // FastBaseTransform
 // -------------------------------------------------------------------------------------------------
-// the per-pixel arithmetic is common.cuh xform_pixel, shared with the frame-source stem (stem_tc.cu)
+// the per-pixel arithmetic is common.cuh xform_pixel, shared with the frame-list stem (stem_tc.cu)
 template <typename TIn>
 __global__ void __launch_bounds__(256)
 fast_base_transform_kernel(const TIn* __restrict__ img, int H, int W, int oh, int ow, float scale_h,

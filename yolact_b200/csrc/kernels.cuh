@@ -97,12 +97,10 @@ int stem_tc_kpad(int ks);   // K = 3*ks*ks rounded up to 64
 StemTcPlan* stem_tc_plan_create(const float* x_nchw, const __half* w_packed, const float* bias, __half* y, int B,
                                 int H, int W, int ks, int stride, int pad, int cout, int act, int split = 0,
                                 float out_scale = 1.f, int cpad = 0);   // cpad > cout: zero-padded output pixels
-// The same stem reading a batch of [fh][fw][3] uint8 BGR frames instead: FastBaseTransform to the network's H x W
-// (transform `mode`, BGR mean / std) happens in the loader.  Weights, output and shapes are net_stem's.
-StemTcPlan* stem_tc_plan_create_frames(const StemTcPlan* net_stem, const uint8_t* frames, int fh, int fw, int mode,
-                                       const float* mean_bgr, const float* std_bgr);
-// ... or reading a frame list: image b's frame, size and scales come from d_table[b] (device, net_stem's B entries),
-// read at launch time, so the same plan (and graph) serves any frame sizes the table holds.
+// The same stem reading a list of uint8 BGR frames instead: FastBaseTransform to the network's H x W (transform
+// `mode`, BGR mean / std) happens in the loader.  Image b's frame, size and scales come from d_table[b] (device,
+// net_stem's B entries), read at launch time, so the same plan (and graph) serves any frame sizes the table holds.
+// Weights, output and shapes are net_stem's.
 StemTcPlan* stem_tc_plan_create_frame_list(const StemTcPlan* net_stem, const FrameRef* d_table, int mode,
                                            const float* mean_bgr, const float* std_bgr);
 void stem_tc_plan_destroy(StemTcPlan* plan);

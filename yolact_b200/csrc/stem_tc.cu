@@ -13,19 +13,17 @@
 // halves w, w + WG of the tile and stores its rows' pixels from the accumulator registers.
 // Several CTAs per SM overlap gather / MMA / epilogue of different tiles.
 //
-// Frame source (SRC_FRAMES, yb_infer_frames): the input is a batch of [fh][fw][3] uint8 BGR frames, and FastBaseTransform
-// (resize to H x W, transform, BGR -> RGB) happens in the loader, so no NCHW fp32 input is ever written.  The 128 rows
-// of a tile are then an 8 x 16 block of output pixels of one image.  Its receptive field is a rectangle of the resized
-// image (FrameWindow: 21 x 37 pixels for 7x7/2, 10 x 18 for 3x3/1): all threads first fill a [3][ROWS][COLS] fp32
-// window of it in shared memory with common.cuh xform_pixel (zero outside the image: the conv's padding), then the
+// Frame-list source (FRAME_LIST, yb_infer_frame_list and yb_infer_frames): the input is a list of [fh][fw][3] uint8 BGR
+// frames, each of its own size, and FastBaseTransform (resize to H x W, transform, BGR -> RGB) happens in the loader, so
+// no NCHW fp32 input is ever written.  The 128 rows of a tile are then an 8 x 16 block of output pixels of one image.
+// A CTA reads its image's FrameRef (frame, fh, fw, scales) from a device table; nothing else about the launch depends on
+// the frame sizes, so one plan and one graph serve any mix of them.  The tile's receptive field is a rectangle of the
+// resized image (FrameWindow: 21 x 37 pixels for 7x7/2, 10 x 18 for 3x3/1): all threads first fill a [3][ROWS][COLS]
+// fp32 window of it in shared memory with common.cuh xform_pixel (zero outside the image: the conv's padding), then the
 // gather above reads the window instead of global memory.  A window pixel is shared by up to 16 patches, so staging
 // computes each resized pixel about 1.5 times per CTA where a direct gather would compute it once per tap.
 // Each output pixel's patch, and so its wgmma row and its output, is bit-identical to the NCHW path's on
 // fast_base_transform's output.
-//
-// Frame-list source (SRC_FRAME_LIST, yb_infer_frame_list): as SRC_FRAMES, but every image has its own frame size.  A CTA
-// reads its image's FrameRef (frame, fh, fw, scales) from a device table before the window fill; nothing else about the
-// launch depends on the frame sizes, so one plan and one graph serve any mix of them.
 #include "tc_common.cuh"
 
 namespace yb {
@@ -48,18 +46,14 @@ struct alignas(64) StemParams {
   long long M;
   int act;
   float out_scale;   // split: weights are pre-multiplied by 1 / out_scale (a power of two)
-  // frame source: frames [B][fh][fw][3] uint8 BGR resized to H x W with scale = (float)fh / H, (float)fw / W
-  const uint8_t* frames;
-  int fh, fw, xform_mode;
-  float scale_h, scale_w;
+  // frame-list source: image b is frame_list[b], resized to H x W
+  int xform_mode;
   XformAffine aff;
   int tiles_x, tiles_y;   // output tiles of FT_H x FT_W pixels per image
-  const FrameRef* frame_list;   // frame-list source: [B] entries, in place of frames / fh / fw / scale_h / scale_w
+  const FrameRef* frame_list;   // [B] entries
 };
 
-enum StemSrc : int { SRC_NCHW = 0, SRC_FRAMES = 1, SRC_FRAME_LIST = 2 };
-
-constexpr int FT_H = 8, FT_W = 16;   // frame source: a tile's 128 rows are FT_H x FT_W output pixels (row = y * FT_W + x)
+constexpr int FT_H = 8, FT_W = 16;   // frame list: a tile's 128 rows are FT_H x FT_W output pixels (row = y * FT_W + x)
 template <int KS, int STRIDE>
 struct FrameWindow {   // resized pixels a tile reads: [3][ROWS][COLS] fp32
   static constexpr int ROWS = (FT_H - 1) * STRIDE + KS, COLS = (FT_W - 1) * STRIDE + KS;
@@ -68,7 +62,7 @@ struct FrameWindow {   // resized pixels a tile reads: [3][ROWS][COLS] fp32
 
 // SPLIT (YB_PREC_F16X3): the patch is written as a hi and a lo fp16 tile, the weights come as [Cout][hi(Kpad) | lo(Kpad)],
 // three MMA passes (hi*hi into one accumulator, lo*hi + hi*lo into a second one) and the output pixel is [hi(COUT) | lo(COUT)].
-template <int KS, int STRIDE, int PAD, int COUT, int WG, bool SPLIT, int SRC>
+template <int KS, int STRIDE, int PAD, int COUT, int WG, bool SPLIT, bool FRAME_LIST>
 __global__ void __launch_bounds__(128 * WG)
 stem_tc_kernel(const __grid_constant__ StemParams p) {
   constexpr int NPL = SPLIT ? 2 : 1;
@@ -94,8 +88,8 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
         tma_load_3d(sB + (pl * ATOMS + a) * B_ATOM_BYTES, &p.tmW, &b_full, pl * ATOMS * 64 + a * 64, 0, 0);
   }
   using Win = FrameWindow<KS, STRIDE>;
-  int fb = 0, fty = 0, ftx = 0;   // frame source: this tile's image and tile coordinates
-  if constexpr (SRC != SRC_NCHW) {
+  int fb = 0, fty = 0, ftx = 0;   // frame list: this tile's image and tile coordinates
+  if constexpr (FRAME_LIST) {
     int t = blockIdx.x;
     ftx = t % p.tiles_x;
     t /= p.tiles_x;
@@ -103,25 +97,15 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
     fb = t / p.tiles_y;
     float* win = reinterpret_cast<float*>(sB + NPL * ATOMS * B_ATOM_BYTES);
     const int y0 = fty * FT_H * STRIDE - PAD, x0 = ftx * FT_W * STRIDE - PAD;
-    // img: this image's frame; f: its fh, fw, scale_h and scale_w -- the params' own (one frame size for the batch) or
-    // the image's frame-list entry, read once (FrameRef has the same field names).  The params are read at their uses:
-    // copying them into locals first changes the SRC_FRAMES instances' register allocation and code.
-    auto fill_window = [&](const uint8_t* img, const auto& f) {
-      for (int i = tid; i < Win::ROWS * Win::COLS; i += 128 * WG) {
-        const int y = y0 + i / Win::COLS, x = x0 + i % Win::COLS;
-        float rgb[3] = {0.f, 0.f, 0.f};
-        if (y >= 0 && y < p.H && x >= 0 && x < p.W)
-          xform_pixel(img, f.fw, xform_tap(y, p.H, f.fh, f.scale_h), xform_tap(x, p.W, f.fw, f.scale_w), p.xform_mode,
-                      p.aff, rgb);
+    const FrameRef f = p.frame_list[fb];   // this image's frame, size and resize scales
+    for (int i = tid; i < Win::ROWS * Win::COLS; i += 128 * WG) {
+      const int y = y0 + i / Win::COLS, x = x0 + i % Win::COLS;
+      float rgb[3] = {0.f, 0.f, 0.f};
+      if (y >= 0 && y < p.H && x >= 0 && x < p.W)
+        xform_pixel(f.frame, f.fw, xform_tap(y, p.H, f.fh, f.scale_h), xform_tap(x, p.W, f.fw, f.scale_w), p.xform_mode,
+                    p.aff, rgb);
 #pragma unroll
-        for (int c = 0; c < 3; ++c) win[c * Win::ROWS * Win::COLS + i] = rgb[c];
-      }
-    };
-    if constexpr (SRC == SRC_FRAME_LIST) {
-      const FrameRef f = p.frame_list[fb];
-      fill_window(f.frame, f);
-    } else {
-      fill_window(p.frames + (size_t)fb * p.fh * p.fw * 3, p);
+      for (int c = 0; c < 3; ++c) win[c * Win::ROWS * Win::COLS + i] = rgb[c];
     }
     __syncthreads();
   }
@@ -130,7 +114,7 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
     const int wg = tid >> 7;   // worker group: which k-groups of the patch this thread gathers
     long long m;
     bool valid;
-    if constexpr (SRC != SRC_NCHW) {
+    if constexpr (FRAME_LIST) {
       const int ho = fty * FT_H + row / FT_W, wo = ftx * FT_W + row % FT_W;
       valid = ho < p.Ho && wo < p.Wo;
       m = ((long long)fb * p.Ho + ho) * p.Wo + wo;
@@ -185,8 +169,8 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
       }
       const size_t plane = (size_t)p.H * p.W;
       const float* xb = p.x + (size_t)b * 3 * plane + (long long)hb * p.W + wb;  // may point before the frame: guarded
-      // the frame branch above repeats this loop with the window as its source: the two must keep the same k order and
-      // encoding, or yb_infer_frames stops being bit-identical to yb_infer on fast_base_transform's output
+      // the frame-list branch above repeats this loop with the window as its source: the two must keep the same k order
+      // and encoding, or yb_infer_frame_list stops being bit-identical to yb_infer on fast_base_transform's output
 #pragma unroll
       for (int kg = 0; kg < ATOMS * 8; ++kg) {
         if (WG > 1 && (kg % WG) != wg) continue;   // warp-uniform
@@ -251,7 +235,7 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
     for (int hh = 0; hh < 2; ++hh) {
       const int row = h * 64 + wq * 16 + (lane >> 2) + 8 * hh;
       long long m;
-      if constexpr (SRC != SRC_NCHW) {
+      if constexpr (FRAME_LIST) {
         const int ho = fty * FT_H + row / FT_W, wo = ftx * FT_W + row % FT_W;
         if (ho >= p.Ho || wo >= p.Wo) continue;
         m = ((long long)fb * p.Ho + ho) * p.Wo + wo;
@@ -278,33 +262,33 @@ stem_tc_kernel(const __grid_constant__ StemParams p) {
   }
 }
 
-template <int KS, int STRIDE, int PAD, int COUT, int WG, bool SPLIT, int SRC>
+template <int KS, int STRIDE, int PAD, int COUT, int WG, bool SPLIT, bool FRAME_LIST>
 void launch_variant(const StemParams& prm, cudaStream_t stream) {
   constexpr int K = 3 * KS * KS;
   constexpr int ATOMS = (K + 63) / 64;
   const size_t smem = (size_t)(SPLIT ? 2 : 1) * ATOMS * (ST_M * 128 + COUT * 128) + 1024 +
-                      (SRC != SRC_NCHW ? FrameWindow<KS, STRIDE>::BYTES : 0);
+                      (FRAME_LIST ? FrameWindow<KS, STRIDE>::BYTES : 0);
   static PerDeviceOnce attr;
   if (attr.first())
-    YB_CHECK_CUDA(cudaFuncSetAttribute(stem_tc_kernel<KS, STRIDE, PAD, COUT, WG, SPLIT, SRC>,
+    YB_CHECK_CUDA(cudaFuncSetAttribute(stem_tc_kernel<KS, STRIDE, PAD, COUT, WG, SPLIT, FRAME_LIST>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const unsigned grid = SRC != SRC_NCHW ? (unsigned)(prm.B * prm.tiles_y * prm.tiles_x) : (unsigned)((prm.M + ST_M - 1) / ST_M);
-  stem_tc_kernel<KS, STRIDE, PAD, COUT, WG, SPLIT, SRC><<<grid, 128 * WG, smem, stream>>>(prm);
+  const unsigned grid = FRAME_LIST ? (unsigned)(prm.B * prm.tiles_y * prm.tiles_x) : (unsigned)((prm.M + ST_M - 1) / ST_M);
+  stem_tc_kernel<KS, STRIDE, PAD, COUT, WG, SPLIT, FRAME_LIST><<<grid, 128 * WG, smem, stream>>>(prm);
 }
 
-template <int SRC>
+template <bool FRAME_LIST>
 void launch_stem(const StemParams& prm, int ks, bool split, cudaStream_t stream) {
   if (split) {
     // the split stem holds 144 KB of operand tiles (one CTA per SM): two worker threads per pixel double the warps
     // that hide the gather's latency
     if (ks == 7)
-      launch_variant<7, 2, 3, 64, 2, true, SRC>(prm, stream);
+      launch_variant<7, 2, 3, 64, 2, true, FRAME_LIST>(prm, stream);
     else
-      launch_variant<3, 1, 1, 32, 1, true, SRC>(prm, stream);
+      launch_variant<3, 1, 1, 32, 1, true, FRAME_LIST>(prm, stream);
   } else if (ks == 7) {
-    launch_variant<7, 2, 3, 64, 1, false, SRC>(prm, stream);
+    launch_variant<7, 2, 3, 64, 1, false, FRAME_LIST>(prm, stream);
   } else {
-    launch_variant<3, 1, 1, 32, 1, false, SRC>(prm, stream);
+    launch_variant<3, 1, 1, 32, 1, false, FRAME_LIST>(prm, stream);
   }
 }
 
@@ -314,7 +298,7 @@ struct StemTcPlan {
   StemParams prm;
   int ks, stride, pad, cout;
   int split = 0;
-  int src = SRC_NCHW;
+  bool frame_list = false;
 };
 
 bool stem_tc_supported(int ks, int stride, int pad, int cin, int cout) {
@@ -356,16 +340,16 @@ StemTcPlan* stem_tc_plan_create(const float* x_nchw, const __half* w_packed, con
   return plan;
 }
 
-// the transform and tiling a frame-source plan shares with the frame-list one; the source is the caller's to set
-static StemTcPlan* plan_create_windowed(const StemTcPlan* net_stem, int src, int mode, const float* mean_bgr,
-                                        const float* std_bgr) {
-  YB_REQUIRE(net_stem->src == SRC_NCHW, "stem_tc: the frame stem is derived from the network's NCHW stem");
+StemTcPlan* stem_tc_plan_create_frame_list(const StemTcPlan* net_stem, const FrameRef* d_table, int mode,
+                                           const float* mean_bgr, const float* std_bgr) {
+  YB_REQUIRE(d_table, "stem_tc: no frame table");
+  YB_REQUIRE(!net_stem->frame_list, "stem_tc: the frame stem is derived from the network's NCHW stem");
   YB_REQUIRE(mode >= YB_XFORM_NORMALIZE && mode <= YB_XFORM_NONE, "stem_tc: unknown transform mode");
   const int tiles_x = ceil_div(net_stem->prm.Wo, FT_W), tiles_y = ceil_div(net_stem->prm.Ho, FT_H);
   YB_REQUIRE((long long)net_stem->prm.B * tiles_y * tiles_x < (1ll << 31), "stem_tc: frame batch too large for one grid");
   auto* plan = new StemTcPlan(*net_stem);
   StemParams& q = plan->prm;
-  plan->src = src;
+  plan->frame_list = true;
   q.x = nullptr;
   q.xform_mode = mode;
   for (int c = 0; c < 3; ++c) {
@@ -374,40 +358,17 @@ static StemTcPlan* plan_create_windowed(const StemTcPlan* net_stem, int src, int
   }
   q.tiles_x = tiles_x;
   q.tiles_y = tiles_y;
-  return plan;
-}
-
-StemTcPlan* stem_tc_plan_create_frames(const StemTcPlan* net_stem, const uint8_t* frames, int fh, int fw, int mode,
-                                       const float* mean_bgr, const float* std_bgr) {
-  YB_REQUIRE(fh > 0 && fw > 0, "stem_tc: empty frames");
-  StemTcPlan* plan = plan_create_windowed(net_stem, SRC_FRAMES, mode, mean_bgr, std_bgr);
-  StemParams& q = plan->prm;
-  q.frames = frames;
-  q.fh = fh;
-  q.fw = fw;
-  // ATen: scale = (float)in / out when the output size is given (area_pixel_compute_scale), as fast_base_transform
-  q.scale_h = (float)fh / (float)q.H;
-  q.scale_w = (float)fw / (float)q.W;
-  return plan;
-}
-
-StemTcPlan* stem_tc_plan_create_frame_list(const StemTcPlan* net_stem, const FrameRef* d_table, int mode,
-                                           const float* mean_bgr, const float* std_bgr) {
-  YB_REQUIRE(d_table, "stem_tc: no frame table");
-  StemTcPlan* plan = plan_create_windowed(net_stem, SRC_FRAME_LIST, mode, mean_bgr, std_bgr);
-  plan->prm.frame_list = d_table;
+  q.frame_list = d_table;
   return plan;
 }
 
 void stem_tc_plan_destroy(StemTcPlan* plan) { delete plan; }
 
 void launch_stem_tc(const StemTcPlan* plan, cudaStream_t stream, LaunchCounter* lc) {
-  if (plan->src == SRC_FRAME_LIST)
-    launch_stem<SRC_FRAME_LIST>(plan->prm, plan->ks, plan->split, stream);
-  else if (plan->src == SRC_FRAMES)
-    launch_stem<SRC_FRAMES>(plan->prm, plan->ks, plan->split, stream);
+  if (plan->frame_list)
+    launch_stem<true>(plan->prm, plan->ks, plan->split, stream);
   else
-    launch_stem<SRC_NCHW>(plan->prm, plan->ks, plan->split, stream);
+    launch_stem<false>(plan->prm, plan->ks, plan->split, stream);
   YB_CHECK_LAUNCH();
   if (lc) lc->n++;
 }

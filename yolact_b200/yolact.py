@@ -386,8 +386,8 @@ class Yolact(nn.Module):
         return out
 
     def infer_frames(self, frames, cross_class=None):
-        """infer_padded(FastBaseTransform(self.cfg)(frames)) as one call, bit for bit, with no host sync once the frame
-        size has been seen (the library keeps the 4 most recently used frame sizes per network input size).
+        """infer_padded(FastBaseTransform(self.cfg)(frames)) as one call, bit for bit, with no host sync and one CUDA
+        graph per network input size whatever the frame size; the frames are read in place.
         frames: CUDA uint8 [B,h,w,3] BGR, any size; the network input size and the transform come from self.cfg
         (max_size, preserve_aspect_ratio, normalize / subtract_means / to_float) as in FastBaseTransform.  In the
         tensor-core precisions the resize and transform run inside the stem kernel: no fp32 input tensor is written.
