@@ -412,9 +412,11 @@ int yb_postprocess(yb_handle* h, const float* d_proto, int ph, int pw, int k, co
   YB_API_BEGIN
   YB_REQUIRE(h && d_proto && d_coef && d_box, "yb_postprocess: null argument");
   YB_REQUIRE(n >= 0, "yb_postprocess: negative detection count");
+  if (n == 0) return YB_OK;
   CallGuard g(h);
-  launch_mask_assembly(d_proto, ph, pw, k, d_coef, d_box, n, out_h, out_w, crop_masks, mask_format, d_masks,
-                       d_boxes_px, d_proto_masks, (cudaStream_t)stream, &h->lc);
+  const PostSrc src = dense_post_src({d_proto, d_coef, d_box, d_masks, d_boxes_px, d_proto_masks, n, out_h, out_w}, ph,
+                                     pw, k, mask_format);
+  launch_mask_assembly(src, &src.base, 1, ph, pw, k, crop_masks, mask_format, (cudaStream_t)stream, &h->lc);
   YB_API_END
 }
 
@@ -424,9 +426,11 @@ int yb_postprocess_batch(yb_handle* h, const float* d_proto, int ph, int pw, int
   YB_API_BEGIN
   YB_REQUIRE(h && d_proto && d_coef && d_box, "yb_postprocess_batch: null argument");
   YB_REQUIRE(n >= 0 && batch >= 0, "yb_postprocess_batch: negative count");
+  if (n == 0 || batch == 0) return YB_OK;
   CallGuard g(h);
-  launch_mask_assembly(d_proto, ph, pw, k, d_coef, d_box, n, out_h, out_w, crop_masks, mask_format, d_masks,
-                       d_boxes_px, nullptr, (cudaStream_t)stream, &h->lc, batch);
+  const PostSrc src =
+      dense_post_src({d_proto, d_coef, d_box, d_masks, d_boxes_px, nullptr, n, out_h, out_w}, ph, pw, k, mask_format);
+  launch_mask_assembly(src, &src.base, batch, ph, pw, k, crop_masks, mask_format, (cudaStream_t)stream, &h->lc);
   YB_API_END
 }
 
@@ -451,13 +455,17 @@ int yb_postprocess_list(yb_handle* h, const yb_post_item* h_items, int B, int ph
                "yb_postprocess_list: a pointer is not device memory of the handle's device");
   }
   if (B == 0) return YB_OK;
+  YB_REQUIRE(mask_format == YB_MASK_F32 || mask_format == YB_MASK_U8 || mask_format == YB_MASK_BITS,
+             "mask_assembly: unknown mask format");
   CallGuard g(h, (cudaStream_t)stream);   // shared item table: ordered behind the previous call
   yb_post_item* table = h->get_post_table(B);
   // pageable source: staged before the call returns, so the caller may reuse h_items at once.  Stream-ordered after
   // the previous call (CallGuard), so its launches have read the table before it is overwritten.
   YB_CHECK_CUDA(cudaMemcpyAsync(table, h_items, (size_t)B * sizeof(yb_post_item), cudaMemcpyHostToDevice,
                                 (cudaStream_t)stream));
-  launch_mask_assembly_list(table, h_items, B, ph, pw, k, crop_masks, mask_format, (cudaStream_t)stream, &h->lc);
+  PostSrc src{};
+  src.table = table;
+  launch_mask_assembly(src, h_items, B, ph, pw, k, crop_masks, mask_format, (cudaStream_t)stream, &h->lc);
   YB_API_END
 }
 

@@ -165,15 +165,22 @@ void launch_detect(const DetectParams& dp, const float* loc, const float* conf, 
                    LaunchCounter* lc);
 
 // ---- mask assembly -----------------------------------------------------------------------------
-void launch_mask_assembly(const float* proto, int ph, int pw, int k, const float* coef,
-                          const float* box, int n, int out_h, int out_w, int crop, int mask_format,
-                          void* masks, int64_t* boxes_px, float* proto_masks, cudaStream_t stream,
-                          LaunchCounter* lc, int batch = 1);
-// the same for a list of B images of any sizes (yb_postprocess_list): d_items is the device copy of h_items, which the
-// host reads for the grid sizes.  One launch per kernel for the whole list: boxes (when an item has boxes_px),
-// prototype-resolution masks (when an item has proto_masks), masks (when an item has masks).
-void launch_mask_assembly_list(const yb_post_item* d_items, const yb_post_item* h_items, int B, int ph, int pw, int k,
-                               int crop, int mask_format, cudaStream_t stream, LaunchCounter* lc);
+// The images of one postprocess call: a table of B items in device memory (yb_postprocess_list), or, with table ==
+// nullptr, a dense batch whose image z is base with every pointer advanced by z times its step (elements, or bytes
+// for masks).  Passed by value to the kernels.
+struct PostSrc {
+  const yb_post_item* table;
+  yb_post_item base;
+  long long proto_step, coef_step, box_step, masks_step_bytes, boxes_px_step, pm_step;
+};
+// the dense source of a batch of images like `first`: proto [B,ph,pw,k], coef [B,n,k], box [B,n,4], masks [B,n,...],
+// boxes_px [B,n,4], proto_masks [B,n,ph,pw]
+PostSrc dense_post_src(const yb_post_item& first, int ph, int pw, int k, int mask_format);
+// One launch per kernel for the B images of src: boxes (when an item has boxes_px), prototype-resolution masks (when
+// an item has proto_masks), masks (when an item has masks).  h_items is the host view the grid is sized from: the
+// table's B entries, or the one dense item.
+void launch_mask_assembly(const PostSrc& src, const yb_post_item* h_items, int B, int ph, int pw, int k, int crop,
+                          int mask_format, cudaStream_t stream, LaunchCounter* lc);
 // global max over HxW per (n, c) then gather channel cls[n] (yolact.py:373, output_utils.py:83)
 void launch_maxpool_gather(const float* x_nhwc, int n, int H, int W, int C, const int64_t* cls,
                            float* out, cudaStream_t stream, LaunchCounter* lc);

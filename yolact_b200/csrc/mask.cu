@@ -13,6 +13,9 @@
 // the CTA evaluates the cropped sigmoid mask on the few prototype rows the band interpolates from
 // (crop happens BEFORE the upsample, output_utils.py:72-74: each output pixel interpolates four
 // already-cropped values), parks them in shared memory and streams out the band.
+//
+// Every kernel here takes a PostSrc and works on image blockIdx.z (boxes: blockIdx.y): yb_postprocess and
+// yb_postprocess_batch pass a strided dense batch, yb_postprocess_list a device table, through the same instances.
 #include <stdlib.h>
 #include <algorithm>
 #include "kernels.cuh"
@@ -48,38 +51,40 @@ __device__ __forceinline__ void sanitize(float a, float b, int size, int padding
   *hi = fminf(__fadd_rn(mx, (float)padding), (float)size);
 }
 
-// LIST = false: dense batch (yb_postprocess / yb_postprocess_batch), blockIdx.z = image, every per-image tensor dense.
-// LIST = true (yb_postprocess_list): blockIdx.z = image, whose tensors, row count and output size come from
-// items[blockIdx.z] in place of proto / coef / box / n / out_h / out_w / masks_v.  The grid and the shared-memory tables
-// are sized for the largest image of the list, so CTAs past this image's rows or detections exit at once; scale_h /
-// scale_w are computed as launch_mask_assembly computes them, so every pixel goes through the per-image arithmetic.
-// (items is the last parameter: the other instances keep their parameter layout.)
-template <int FORMAT, bool LIST>
+// Image z of a call: the list's table entry, or the dense batch's first image advanced by z strides.
+__device__ __forceinline__ yb_post_item post_item(const PostSrc& s, int z) {
+  if (s.table) return s.table[z];
+  yb_post_item it = s.base;
+  it.proto += z * s.proto_step;
+  it.coef += z * s.coef_step;
+  it.box += z * s.box_step;
+  it.masks = static_cast<unsigned char*>(it.masks) + z * s.masks_step_bytes;
+  it.boxes_px += z * s.boxes_px_step;
+  it.proto_masks += z * s.pm_step;
+  return it;
+}
+
+// blockIdx.z = image, read through post_item.  The grid and the shared-memory tables are sized for the largest image
+// of the call, so CTAs past this image's rows or detections exit at once.  The image's fields stay in shared memory
+// and are read where they are used: held in registers through the kernel they would cost 8 more (48 instead of 40).
+template <int FORMAT>
 __global__ void __launch_bounds__(MT)
-mask_assembly_kernel(const float* __restrict__ proto, int ph, int pw, int k,
-                     const float* __restrict__ coef, const float* __restrict__ box, int n, int out_h,
-                     int out_w, int crop, int band, int group, int max_rows, float scale_h,
-                     float scale_w, void* __restrict__ masks_v, long long mask_img_stride_bytes,
-                     const yb_post_item* __restrict__ items) {
-  if constexpr (LIST) {
-    const yb_post_item it = items[blockIdx.z];
-    if (it.masks == nullptr || (int)blockIdx.x * band >= it.out_h || (int)blockIdx.y * group >= it.n) return;
-    proto = it.proto;
-    coef = it.coef;
-    box = it.box;
-    masks_v = it.masks;
-    n = it.n;
-    out_h = it.out_h;
-    out_w = it.out_w;
-    scale_h = __fdiv_rn((float)ph, (float)out_h);
-    scale_w = __fdiv_rn((float)pw, (float)out_w);
-  } else {
-    // blockIdx.z = image of the batch (yb_postprocess_batch); every per-image tensor is dense
-    proto += (size_t)blockIdx.z * ph * pw * k;
-    coef += (size_t)blockIdx.z * n * k;
-    box += (size_t)blockIdx.z * n * 4;
-    masks_v = reinterpret_cast<unsigned char*>(masks_v) + (size_t)blockIdx.z * mask_img_stride_bytes;
+mask_assembly_kernel(const PostSrc src, int ph, int pw, int k, int crop, int band, int group, int max_rows) {
+  __shared__ yb_post_item it;
+  __shared__ float scale_h, scale_w;
+  if (threadIdx.x == 0) {
+    it = post_item(src, blockIdx.z);
+    scale_h = __fdiv_rn((float)ph, (float)it.out_h);
+    scale_w = __fdiv_rn((float)pw, (float)it.out_w);
   }
+  __syncthreads();
+  if (it.masks == nullptr || (int)blockIdx.x * band >= it.out_h || (int)blockIdx.y * group >= it.n) return;
+  const float* const& proto = it.proto;
+  const float* const& coef = it.coef;
+  const float* const& box = it.box;
+  // masks are global memory: stores through a pointer read from shared memory would otherwise be generic stores
+  const auto masks_v = [] { __builtin_assume(__isGlobal(it.masks)); return it.masks; };
+  const int &n = it.n, &out_h = it.out_h, &out_w = it.out_w;
   extern __shared__ unsigned char smem_raw[];
   ColTab* coltab = reinterpret_cast<ColTab*>(smem_raw);                 // [out_w]
   float* mrows = reinterpret_cast<float*>(coltab + out_w);               // [max_rows][pw]
@@ -113,18 +118,18 @@ mask_assembly_kernel(const float* __restrict__ proto, int ph, int pw, int k,
       const size_t band_off = (size_t)d * plane + (size_t)y0 * out_w;
       // elements up to the next 4-element boundary of the ACTUAL address (the per-image offset of a batched
       // call need not be 16-byte aligned)
-      const int head = (int)((4 - (((reinterpret_cast<uintptr_t>(masks_v) / esz) + band_off) & 3)) & 3);
+      const int head = (int)((4 - (((reinterpret_cast<uintptr_t>(masks_v()) / esz) + band_off) & 3)) & 3);
       const int hd = min(head, L);
       const int nq = (L - hd) >> 2;            // aligned 4-element stores
       const int tail = L - hd - 4 * nq;        // < 4 trailing elements
       if (FORMAT == YB_MASK_F32) {
-        float* base = reinterpret_cast<float*>(masks_v) + band_off;
+        float* base = reinterpret_cast<float*>(masks_v()) + band_off;
         float4* body = reinterpret_cast<float4*>(base + hd);
         for (int q = tid; q < nq; q += MT) __stcs(body + q, make_float4(0.f, 0.f, 0.f, 0.f));
         if (tid < hd) base[tid] = 0.f;
         if (tid < tail) base[hd + 4 * nq + tid] = 0.f;
       } else {
-        unsigned char* base = reinterpret_cast<unsigned char*>(masks_v) + band_off;
+        unsigned char* base = reinterpret_cast<unsigned char*>(masks_v()) + band_off;
         uchar4* body = reinterpret_cast<uchar4*>(base + hd);
         for (int q = tid; q < nq; q += MT) body[q] = make_uchar4(0, 0, 0, 0);
         if (tid < hd) base[tid] = 0;
@@ -165,6 +170,8 @@ mask_assembly_kernel(const float* __restrict__ proto, int ph, int pw, int k,
         const int pr = q_lo + rr;
         const float4* pp = reinterpret_cast<const float4*>(proto + ((size_t)pr * pw + c) * k);
         float acc = 0.f;
+        // not unrolled: an unrolled body keeps more loads in flight than the 40 registers that leave 6 CTAs per SM
+#pragma unroll 1
         for (int j = 0; j < k / 4; ++j) {
           const float4 q = __ldg(pp + j);
           const float4 w4 = __ldg(reinterpret_cast<const float4*>(cf) + j);   // same address in every lane: one L1 broadcast
@@ -181,7 +188,7 @@ mask_assembly_kernel(const float* __restrict__ proto, int ph, int pw, int k,
     // ---- stream out the band -------------------------------------------------------------
     if (FORMAT == YB_MASK_BITS) {
       // one warp per output word: lane j evaluates pixel 32*wx + j, the ballot is the packed word
-      uint32_t* out = reinterpret_cast<uint32_t*>(masks_v) + (size_t)d * out_h * wpr;
+      uint32_t* out = reinterpret_cast<uint32_t*>(masks_v()) + (size_t)d * out_h * wpr;
       const int words = (y1 - y0) * wpr;
       if (!any) {
         for (int wi = tid; wi < words; wi += MT) out[(size_t)y0 * wpr + wi] = 0u;   // the band's words are contiguous
@@ -241,9 +248,9 @@ mask_assembly_kernel(const float* __restrict__ proto, int ph, int pw, int k,
           float v = __fadd_rn(__fmul_rn(rt.l0, top), __fmul_rn(rt.l1, bot));
           if (v > 0.5f) {
             if (FORMAT == YB_MASK_F32)
-              reinterpret_cast<float*>(masks_v)[band_off + (size_t)yy * out_w + x] = 1.f;
+              reinterpret_cast<float*>(masks_v())[band_off + (size_t)yy * out_w + x] = 1.f;
             else
-              reinterpret_cast<unsigned char*>(masks_v)[band_off + (size_t)yy * out_w + x] = 1;
+              reinterpret_cast<unsigned char*>(masks_v())[band_off + (size_t)yy * out_w + x] = 1;
           }
         }
       }
@@ -264,16 +271,8 @@ __device__ __forceinline__ void box_px(const float* __restrict__ box, int i, int
   out[i * 4 + 3] = (int64_t)y2;
 }
 
-__global__ void boxes_px_kernel(const float* __restrict__ box, int n, int out_h, int out_w,
-                                int64_t* __restrict__ out) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;   // n = total boxes over the batch
-  if (i >= n) return;
-  box_px(box, i, out_h, out_w, out);
-}
-
-// list source: blockIdx.y = image, each with its own rows and output size
-__global__ void boxes_px_list_kernel(const yb_post_item* __restrict__ items) {
-  const yb_post_item& it = items[blockIdx.y];
+__global__ void boxes_px_kernel(const PostSrc src) {
+  const yb_post_item it = post_item(src, blockIdx.y);
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (it.boxes_px == nullptr || i >= it.n) return;
   box_px(it.box, i, it.out_h, it.out_w, it.boxes_px);
@@ -311,18 +310,11 @@ __device__ __forceinline__ void proto_masks_row(const float* __restrict__ proto,
   }
 }
 
+// blockIdx.z = image.  yb_postprocess_list's callers point consecutive images at consecutive rows of one
+// [sum n, ph, pw] buffer, so that maskiou_net runs once on all of them.
 __global__ void __launch_bounds__(MT)
-proto_masks_kernel(const float* __restrict__ proto, int ph, int pw, int k,
-                   const float* __restrict__ coef, const float* __restrict__ box, int crop,
-                   float* __restrict__ out) {
-  proto_masks_row(proto, ph, pw, k, coef, box, crop, out, blockIdx.x, blockIdx.y);
-}
-
-// list source: blockIdx.z = image; its rows land wherever items[z].proto_masks points (yb_postprocess_list's callers
-// point consecutive images at consecutive rows of one [sum n, ph, pw] buffer, so that maskiou_net runs once on all)
-__global__ void __launch_bounds__(MT)
-proto_masks_list_kernel(const yb_post_item* __restrict__ items, int ph, int pw, int k, int crop) {
-  const yb_post_item it = items[blockIdx.z];
+proto_masks_kernel(const PostSrc src, int ph, int pw, int k, int crop) {
+  const yb_post_item it = post_item(src, blockIdx.z);
   if (it.proto_masks == nullptr || (int)blockIdx.y >= it.n) return;
   proto_masks_row(it.proto, ph, pw, k, it.coef, it.box, crop, it.proto_masks, blockIdx.x, blockIdx.y);
 }
@@ -373,73 +365,49 @@ int mask_group(int bands, int n, int batch) {
   return group;
 }
 
-}  // namespace
-
-void launch_mask_assembly(const float* proto, int ph, int pw, int k, const float* coef,
-                          const float* box, int n, int out_h, int out_w, int crop, int mask_format,
-                          void* masks, int64_t* boxes_px, float* proto_masks, cudaStream_t stream,
-                          LaunchCounter* lc, int batch) {
-  if (n <= 0 || batch <= 0) return;
-  YB_REQUIRE(batch == 1 || proto_masks == nullptr, "mask_assembly: proto_masks output is per image");
-  YB_REQUIRE(k % 4 == 0 && k <= 128, "mask_assembly: mask_dim must be a multiple of 4 and <= 128");
-  YB_REQUIRE(out_h > 0 && out_w > 0 && ph > 0 && pw > 0, "mask_assembly: bad sizes");
-  const float scale_h = (float)ph / (float)out_h;
-  const float scale_w = (float)pw / (float)out_w;
-  if (boxes_px) {
-    boxes_px_kernel<<<ceil_div(n * batch, 128), 128, 0, stream>>>(box, n * batch, out_h, out_w, boxes_px);
-    YB_CHECK_LAUNCH();
-    if (lc) lc->n++;
-  }
-  if (proto_masks) {
-    proto_masks_kernel<<<dim3(ph, n), MT, 0, stream>>>(proto, ph, pw, k, coef, box, crop, proto_masks);
-    YB_CHECK_LAUNCH();
-    if (lc) lc->n++;
-  }
-  if (masks) {
-    YB_REQUIRE((reinterpret_cast<uintptr_t>(masks) & 15) == 0, "mask_assembly: masks must be 16-byte aligned");
-    int band, max_rows;
-    size_t smem;
-    mask_band(scale_h, out_w, pw, &band, &max_rows, &smem);
-    const int bands = ceil_div(out_h, band);
-    const int group = mask_group(bands, n, batch);
-    dim3 grid(bands, ceil_div(n, group), batch);
-    const size_t plane = (size_t)out_h * out_w;
-    const long long img_stride = (long long)n * (mask_format == YB_MASK_F32 ? plane * 4
-                                                : mask_format == YB_MASK_U8 ? plane
-                                                                            : (size_t)out_h * ((out_w + 31) / 32) * 4);
-#define YB_LAUNCH_MASK(FMT)                                                                       \
-  do {                                                                                            \
-    if (smem > 48 * 1024)                                                                         \
-      YB_CHECK_CUDA(cudaFuncSetAttribute(mask_assembly_kernel<FMT, false>,                        \
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    mask_assembly_kernel<FMT, false><<<grid, MT, smem, stream>>>(proto, ph, pw, k, coef, box, n,  \
-                                                                out_h, out_w, crop, band, group, \
-                                                                max_rows, scale_h, scale_w,      \
-                                                                masks, img_stride, nullptr);     \
-  } while (0)
-    switch (mask_format) {
-      case YB_MASK_F32: YB_LAUNCH_MASK(YB_MASK_F32); break;
-      case YB_MASK_U8: YB_LAUNCH_MASK(YB_MASK_U8); break;
-      case YB_MASK_BITS: YB_LAUNCH_MASK(YB_MASK_BITS); break;
-      default: YB_REQUIRE(false, "mask_assembly: unknown mask format");
-    }
-#undef YB_LAUNCH_MASK
-    YB_CHECK_LAUNCH();
-    if (lc) lc->n++;
-  }
+// Static shared memory of a mask_assembly instance.  Without opting in, a kernel may use 48 KB of shared memory in all,
+// static and dynamic together.
+template <int FORMAT>
+size_t mask_static_smem() {
+  static const size_t bytes = [] {
+    cudaFuncAttributes a{};
+    YB_CHECK_CUDA(cudaFuncGetAttributes(&a, mask_assembly_kernel<FORMAT>));
+    return a.sharedSizeBytes;
+  }();
+  return bytes;
 }
 
-void launch_mask_assembly_list(const yb_post_item* d_items, const yb_post_item* h_items, int B, int ph, int pw, int k,
-                               int crop, int mask_format, cudaStream_t stream, LaunchCounter* lc) {
+}  // namespace
+
+PostSrc dense_post_src(const yb_post_item& first, int ph, int pw, int k, int mask_format) {
+  PostSrc s{};
+  s.base = first;
+  const long long n = first.n;
+  const long long plane = (long long)first.out_h * first.out_w;
+  s.proto_step = (long long)ph * pw * k;
+  s.coef_step = n * k;
+  s.box_step = n * 4;
+  s.masks_step_bytes = n * (mask_format == YB_MASK_F32 ? plane * 4
+                            : mask_format == YB_MASK_U8 ? plane
+                                                        : (long long)first.out_h * ((first.out_w + 31) / 32) * 4);
+  s.boxes_px_step = n * 4;
+  s.pm_step = n * ph * pw;
+  // a null output stays null in every image, so the kernels' "not wanted" checks hold for the whole batch
+  if (!first.masks) s.masks_step_bytes = 0;
+  if (!first.boxes_px) s.boxes_px_step = 0;
+  if (!first.proto_masks) s.pm_step = 0;
+  return s;
+}
+
+void launch_mask_assembly(const PostSrc& src, const yb_post_item* h_items, int B, int ph, int pw, int k, int crop,
+                          int mask_format, cudaStream_t stream, LaunchCounter* lc) {
   YB_REQUIRE(k % 4 == 0 && k <= 128, "mask_assembly: mask_dim must be a multiple of 4 and <= 128");
   YB_REQUIRE(ph > 0 && pw > 0, "mask_assembly: bad sizes");
-  YB_REQUIRE(mask_format == YB_MASK_F32 || mask_format == YB_MASK_U8 || mask_format == YB_MASK_BITS,
-             "mask_assembly: unknown mask format");
   // the grid covers the most rows of any image; the masks' grid and shared-memory tables also the tallest and widest
   // output and the largest vertical scale (the smallest out_h) among the images that want masks
   int max_n = 0, mask_n = 0, max_h = 0, max_w = 0, min_h = 0;
   bool any_boxes = false, any_pm = false;
-  for (int b = 0; b < B; ++b) {
+  for (int b = 0; b < (src.table ? B : 1); ++b) {
     const yb_post_item& it = h_items[b];
     YB_REQUIRE(it.n >= 0 && it.out_h > 0 && it.out_w > 0, "mask_assembly: bad sizes");
     if (it.n == 0) continue;
@@ -455,12 +423,12 @@ void launch_mask_assembly_list(const yb_post_item* d_items, const yb_post_item* 
     }
   }
   if (any_boxes) {
-    boxes_px_list_kernel<<<dim3(ceil_div(max_n, 128), B), 128, 0, stream>>>(d_items);
+    boxes_px_kernel<<<dim3(ceil_div(max_n, 128), B), 128, 0, stream>>>(src);
     YB_CHECK_LAUNCH();
     if (lc) lc->n++;
   }
   if (any_pm) {
-    proto_masks_list_kernel<<<dim3(ph, max_n, B), MT, 0, stream>>>(d_items, ph, pw, k, crop);
+    proto_masks_kernel<<<dim3(ph, max_n, B), MT, 0, stream>>>(src, ph, pw, k, crop);
     YB_CHECK_LAUNCH();
     if (lc) lc->n++;
   }
@@ -471,21 +439,20 @@ void launch_mask_assembly_list(const yb_post_item* d_items, const yb_post_item* 
     const int bands = ceil_div(max_h, band);
     const int group = mask_group(bands, mask_n, B);
     const dim3 grid(bands, ceil_div(mask_n, group), B);
-#define YB_LAUNCH_MASK_LIST(FMT)                                                                            \
-  do {                                                                                                      \
-    if (smem > 48 * 1024)                                                                                   \
-      YB_CHECK_CUDA(cudaFuncSetAttribute(mask_assembly_kernel<FMT, true>,                                   \
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));          \
-    mask_assembly_kernel<FMT, true><<<grid, MT, smem, stream>>>(nullptr, ph, pw, k, nullptr, nullptr, 0, 0, \
-                                                                0, crop, band, group, max_rows, 0.f, 0.f,  \
-                                                                nullptr, 0, d_items);                      \
+#define YB_LAUNCH_MASK(FMT)                                                                                  \
+  do {                                                                                                       \
+    if (smem + mask_static_smem<FMT>() > 48 * 1024)                                                         \
+      YB_CHECK_CUDA(cudaFuncSetAttribute(mask_assembly_kernel<FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                         (int)smem));                                                        \
+    mask_assembly_kernel<FMT><<<grid, MT, smem, stream>>>(src, ph, pw, k, crop, band, group, max_rows);      \
   } while (0)
     switch (mask_format) {
-      case YB_MASK_F32: YB_LAUNCH_MASK_LIST(YB_MASK_F32); break;
-      case YB_MASK_U8: YB_LAUNCH_MASK_LIST(YB_MASK_U8); break;
-      default: YB_LAUNCH_MASK_LIST(YB_MASK_BITS); break;
+      case YB_MASK_F32: YB_LAUNCH_MASK(YB_MASK_F32); break;
+      case YB_MASK_U8: YB_LAUNCH_MASK(YB_MASK_U8); break;
+      case YB_MASK_BITS: YB_LAUNCH_MASK(YB_MASK_BITS); break;
+      default: YB_REQUIRE(false, "mask_assembly: unknown mask format");
     }
-#undef YB_LAUNCH_MASK_LIST
+#undef YB_LAUNCH_MASK
     YB_CHECK_LAUNCH();
     if (lc) lc->n++;
   }

@@ -66,14 +66,7 @@ def assemble_masks(proto, coef, boxes, h, w, crop_masks=True, mask_format="f32",
     coef = coef.contiguous().float()
     boxes = boxes.contiguous().float()
     fmt = _FORMATS[mask_format]
-    if masks_out is not None:
-        masks = masks_out
-    elif fmt == _lib.YB_MASK_F32:
-        masks = torch.empty(n, h, w, dtype=torch.float32, device=dev)
-    elif fmt == _lib.YB_MASK_U8:
-        masks = torch.empty(n, h, w, dtype=torch.uint8, device=dev)
-    else:
-        masks = torch.empty(n, h, (w + 31) // 32, dtype=torch.int32, device=dev)
+    masks = masks_out if masks_out is not None else _empty_masks((n,), h, w, fmt, dev)
     boxes_px = torch.empty(n, 4, dtype=torch.int64, device=dev)
     pm = torch.empty(n, ph, pw, dtype=torch.float32, device=dev) if want_proto_masks else None
     if n > 0:
@@ -95,14 +88,7 @@ def assemble_masks_batch(proto, coef, boxes, h, w, crop_masks=True, mask_format=
     n = int(coef.shape[1])
     proto, coef, boxes = proto.contiguous().float(), coef.contiguous().float(), boxes.contiguous().float()
     fmt = _FORMATS[mask_format]
-    if masks_out is not None:
-        masks = masks_out
-    elif fmt == _lib.YB_MASK_F32:
-        masks = torch.empty(B, n, h, w, dtype=torch.float32, device=dev)
-    elif fmt == _lib.YB_MASK_U8:
-        masks = torch.empty(B, n, h, w, dtype=torch.uint8, device=dev)
-    else:
-        masks = torch.empty(B, n, h, (w + 31) // 32, dtype=torch.int32, device=dev)
+    masks = masks_out if masks_out is not None else _empty_masks((B, n), h, w, fmt, dev)
     boxes_px = boxes_out if boxes_out is not None else torch.empty(B, n, 4, dtype=torch.int64, device=dev)
     if n > 0 and B > 0:
         _lib.check(lib.yb_postprocess_batch(_ops_handle(dev, k), _lib.ptr(proto), ph, pw, k, _lib.ptr(coef),
@@ -142,22 +128,13 @@ def postprocess(det_output, w, h, batch_idx=0, interpolation_mode='bilinear', vi
         out_masks, boxes_px, pm = assemble_masks(dets['proto'], masks, boxes, h, w, crop_masks, mask_format,
                                                  want_proto_masks=use_maskiou)
         if use_maskiou:
-            # output_utils.py:79-88: maskiou on the cropped prototype-resolution masks, gathered at class
-            lib = _lib.load()
-            n, ph, pw = pm.shape
-            miou = torch.empty(n, dtype=torch.float32, device=pm.device)
-            cls64 = classes.contiguous().long()
-            _lib.check(lib.yb_maskiou(net._handle_for(pm.device), _lib.ptr(pm), int(n), int(ph), int(pw),
-                                      _lib.ptr(cls64), _lib.ptr(miou), _lib.current_stream(pm.device)), "yb_maskiou")
-            if getattr(ncfg, "rescore_mask", False):
-                if getattr(cfg, "rescore_bbox", False) or getattr(ncfg, "rescore_bbox", False):
-                    scores = scores * miou
-                else:
-                    scores = [scores, scores * miou]
+            rescored = _maskiou_rescore(net, ncfg, pm, classes, scores)
+            if rescored is not None:
+                scores = rescored[0] if rescored[1] else [scores, rescored[0]]
         masks = out_masks
     else:
         # cfg.eval_mask_branch == False (--detect): boxes only, masks are the raw coefficients (Appendix D.15)
-        _, boxes_px, _ = _boxes_only(boxes, h, w)
+        boxes_px = _boxes_only(boxes, h, w)
 
     return classes, scores, boxes_px, masks
 
@@ -242,12 +219,7 @@ def postprocess_list(det_output, sizes, interpolation_mode='bilinear', visualize
     for j, (i, d, n) in enumerate(zip(live, dets, ns)):
         h, w = hw[i]
         proto, coef, box = d['proto'].contiguous().float(), d['mask'].contiguous().float(), d['box'].contiguous().float()
-        if fmt == _lib.YB_MASK_F32:
-            masks = torch.empty(n, h, w, dtype=torch.float32, device=dev)
-        elif fmt == _lib.YB_MASK_U8:
-            masks = torch.empty(n, h, w, dtype=torch.uint8, device=dev)
-        else:
-            masks = torch.empty(n, h, (w + 31) // 32, dtype=torch.int32, device=dev)
+        masks = _empty_masks((n,), h, w, fmt, dev)
         boxes_px = torch.empty(n, 4, dtype=torch.int64, device=dev)
         keep_alive += [proto, coef, box]
         items[j] = _lib.YbPostItem(proto.data_ptr(), coef.data_ptr(), box.data_ptr(), masks.data_ptr() or None,
@@ -259,21 +231,39 @@ def postprocess_list(det_output, sizes, interpolation_mode='bilinear', visualize
                                        stream), "yb_postprocess_list")
 
     if use_maskiou and off > 0:
-        # output_utils.py:79-88 over the rows of every image at once: maskiou_net and the gather are per row
+        # maskiou_net and the gather are per row: one call over the rows of every image at once
         cat = (lambda ts: torch.cat(ts)) if len(dets) > 1 else (lambda ts: ts[0])
-        cls64 = cat([d['class'] for d in dets]).contiguous().long()
-        miou = torch.empty(off, dtype=torch.float32, device=dev)
-        _lib.check(lib.yb_maskiou(net._handle_for(dev), _lib.ptr(pm), off, ph, pw, _lib.ptr(cls64), _lib.ptr(miou),
-                                  stream), "yb_maskiou")
-        if getattr(ncfg, "rescore_mask", False):
-            rescored = cat([d['score'] for d in dets]) * miou
-            bbox = getattr(cfg, "rescore_bbox", False) or getattr(ncfg, "rescore_bbox", False)
+        rescored = _maskiou_rescore(net, ncfg, pm, cat([d['class'] for d in dets]), cat([d['score'] for d in dets]))
+        if rescored is not None:
             off = 0
             for i, d, n in zip(live, dets, ns):
-                r = rescored[off:off + n]
-                out[i] = (d['class'], r if bbox else [d['score'], r]) + out[i][2:]
+                r = rescored[0][off:off + n]
+                out[i] = (d['class'], r if rescored[1] else [d['score'], r]) + out[i][2:]
                 off += n
     return out
+
+
+def _empty_masks(lead, h, w, fmt, dev):
+    """Uninitialised masks [*lead, h, w] in yb_mask_format fmt: fp32, uint8, or int32 words of 32 pixels per row."""
+    if fmt == _lib.YB_MASK_F32:
+        return torch.empty(*lead, h, w, dtype=torch.float32, device=dev)
+    if fmt == _lib.YB_MASK_U8:
+        return torch.empty(*lead, h, w, dtype=torch.uint8, device=dev)
+    return torch.empty(*lead, h, (w + 31) // 32, dtype=torch.int32, device=dev)
+
+
+def _maskiou_rescore(net, ncfg, pm, classes, scores):
+    """output_utils.py:79-88: maskiou_net on the cropped prototype-resolution masks pm [n,ph,pw], gathered at each row's
+    class.  None unless cfg.rescore_mask; else (scores * maskiou, rescore_bbox): with rescore_bbox the rescored scores
+    replace the scores, without it the reference returns [scores, scores * maskiou]."""
+    lib = _lib.load()
+    n, ph, pw = (int(s) for s in pm.shape)
+    miou = torch.empty(n, dtype=torch.float32, device=pm.device)
+    _lib.check(lib.yb_maskiou(net._handle_for(pm.device), _lib.ptr(pm), n, ph, pw, _lib.ptr(classes.contiguous().long()),
+                              _lib.ptr(miou), _lib.current_stream(pm.device)), "yb_maskiou")
+    if not getattr(ncfg, "rescore_mask", False):
+        return None
+    return scores * miou, getattr(_config.cfg, "rescore_bbox", False) or getattr(ncfg, "rescore_bbox", False)
 
 
 def _keep_leading_rows(det_output, live, score_threshold, dev):
@@ -303,18 +293,17 @@ def _keep_leading_rows(det_output, live, score_threshold, dev):
 
 
 def _boxes_only(boxes, h, w):
+    """boxes [n,4] relative -> int64 [n,4] pixels: yb_postprocess without masks (its proto and coef are never read)."""
     lib = _lib.load()
     dev = boxes.device
     n = int(boxes.shape[0])
     boxes = boxes.contiguous().float()
     boxes_px = torch.empty(n, 4, dtype=torch.int64, device=dev)
-    dummy = torch.zeros(1, 1, 4, device=dev)
-    coef = torch.zeros(max(n, 1), 4, device=dev)
-    if n > 0:
-        _lib.check(lib.yb_postprocess(_ops_handle(dev, 4), _lib.ptr(dummy), 1, 1, 4, _lib.ptr(coef), _lib.ptr(boxes), n,
-                                      h, w, 0, _lib.YB_MASK_F32, None, _lib.ptr(boxes_px), None,
-                                      _lib.current_stream(dev)), "yb_postprocess(boxes)")
-    return None, boxes_px, None
+    dummy = torch.zeros(4, device=dev)
+    _lib.check(lib.yb_postprocess(_ops_handle(dev, 4), _lib.ptr(dummy), 1, 1, 4, _lib.ptr(dummy), _lib.ptr(boxes), n, h,
+                                  w, 0, _lib.YB_MASK_F32, None, _lib.ptr(boxes_px), None, _lib.current_stream(dev)),
+               "yb_postprocess(boxes)")
+    return boxes_px
 
 
 def unpack_bits(words, w):
