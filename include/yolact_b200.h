@@ -37,6 +37,9 @@
  *                         eval.py:435-445 (_mask_iou, _bbox_iou)
  *   yb_mask_rle        <- pycocotools.mask.encode in Detections.add_mask (eval.py:320-330)
  *   yb_display_blend   <- the GPU mask blend of prep_display (eval.py:186-209,226)
+ *   yb_render_list     <- the GPU part of prep_display with undo_transform=False (eval.py:147-226): postprocess with
+ *                         rescore_bbox, top-k selection, score cut, palette, mask blend and .byte(), for a list of
+ *                         frames, without materialising masks
  *   yb_dcn_forward     <- dcn_v2_forward (external/DCNv2/src/dcn_v2.h:9-39,
  *                         src/cuda/dcn_v2_cuda.cu:42-172, src/cuda/dcn_v2_im2col_cuda.cu:125-195)
  *   yb_conv2d          <- nn.Conv2d + folded BatchNorm2d + activation (+ residual), op-level test hook
@@ -314,6 +317,46 @@ YB_API int yb_pack_detections(yb_handle* h, const float* d_box, const float* d_c
 YB_API int yb_display_blend(yb_handle* h, const float* d_img, int img_is_255, const void* d_masks,
                             int mask_format, int n, int img_h, int img_w, const float* d_colors, float alpha,
                             uint8_t* d_out, void* stream);
+
+/* One frame of a yb_render_list call (all pointers device memory):
+ *   frame [h,w,3] BGR, uint8 or fp32 0..255 (the call's frame_is_u8); out [h,w,3] uint8;
+ *   proto [ph,pw,k], coef [n,k], box [n,4] relative, cls int64 [n]: as yb_postprocess's; proto NULL draws no masks
+ *   (cfg.eval_mask_branch off) but still selects the rows;
+ *   score [n]: the ranking scores (maskiou-rescored for YOLACT++), det_score [n]: Detect's scores, which the
+ *   score_threshold filter reads (may equal score);
+ *   sel_n int32 [1], sel_cls int64 [top_k], sel_score fp32 [top_k], sel_box int64 [top_k,4] (each nullable): the drawn
+ *   rows in drawing order (pixel boxes at h x w), zero past sel_n. */
+typedef struct {
+  const void* frame;
+  uint8_t* out;
+  const float* proto;
+  const float* coef;
+  const float* box;
+  const int64_t* cls;
+  const float* score;
+  const float* det_score;
+  int32_t* sel_n;
+  int64_t* sel_cls;
+  float* sel_score;
+  int64_t* sel_box;
+  int32_t n;
+  int32_t h;
+  int32_t w;
+} yb_render_item;
+
+/* prep_display(undo_transform=False) without text or boxes, for a list of B frames of any sizes, in two launches for
+ * the whole list.  Per frame: rows with det_score > score_threshold (all rows when score_threshold <= 0), in stable
+ * descending order of score (ties to the lower row), the first top_k, cut at the first score < score_threshold; drawn
+ * slot j gets palette colour (class_color ? cls : j) * 5 % P (d_palette [P,3] fp32 0..1, BGR); out =
+ * (frame / 255 blended with the drawn masks at mask_alpha) * 255, .byte().  The masks are postprocess's
+ * (crop_masks, bilinear, > 0.5) and are never written: out equals yb_postprocess + the selection + yb_display_blend,
+ * bit for bit.  n == 0 or proto == NULL gives the frame's round trip (frame / 255 * 255).byte().  The item table is
+ * uploaded into a table the handle owns (stream-ordered behind the handle's previous call); h_items may be reused as
+ * soon as the call returns.  YB_ERR_INVALID for a null frame or out, h or w <= 0, n < 0, a null coef, box, cls, score
+ * or det_score with n > 0, top_k < 1, P < 1, or a pointer that is not device memory of the handle's device. */
+YB_API int yb_render_list(yb_handle* h, const yb_render_item* h_items, int B, int frame_is_u8, int ph, int pw, int k,
+                          int crop_masks, int top_k, float score_threshold, int class_color, float mask_alpha,
+                          const float* d_palette, int P, void* stream);
 
 /* ---- op-level entry points --------------------------------------------------------------------- */
 /* Mirrors dcn_v2_forward's argument list (src/dcn_v2.h:9-23); all tensors NCHW fp32 contiguous.

@@ -2,7 +2,8 @@
 Yolact.forward() / Detect() / postprocess() surface.  See DESIGN.md and INTEGRATION.md."""
 from .config import cfg, set_cfg, CONFIGS, MEANS, STD  # noqa: F401
 
-__all__ = ["cfg", "set_cfg", "CONFIGS", "Yolact", "Detect", "postprocess", "postprocess_list", "FastBaseTransform"]
+__all__ = ["cfg", "set_cfg", "CONFIGS", "Yolact", "Detect", "postprocess", "postprocess_list", "FastBaseTransform",
+           "render_masks"]
 
 
 def __getattr__(name):  # lazy: importing the package must not require torch/CUDA
@@ -18,6 +19,9 @@ def __getattr__(name):  # lazy: importing the package must not require torch/CUD
     if name == "postprocess_list":
         from .output_utils import postprocess_list
         return postprocess_list
+    if name == "render_masks":
+        from .display import render_masks
+        return render_masks
     if name == "FastBaseTransform":
         from .augmentations import FastBaseTransform
         return FastBaseTransform

@@ -55,6 +55,27 @@ class YbPostItem(ctypes.Structure):
     ]
 
 
+class YbRenderItem(ctypes.Structure):
+    """Mirror of yb_render_item (one frame of yb_render_list)."""
+    _fields_ = [
+        ("frame", c_void_p),
+        ("out", c_void_p),
+        ("proto", c_void_p),
+        ("coef", c_void_p),
+        ("box", c_void_p),
+        ("cls", c_void_p),
+        ("score", c_void_p),
+        ("det_score", c_void_p),
+        ("sel_n", c_void_p),
+        ("sel_cls", c_void_p),
+        ("sel_score", c_void_p),
+        ("sel_box", c_void_p),
+        ("n", c_int32),
+        ("h", c_int32),
+        ("w", c_int32),
+    ]
+
+
 YB_BACKBONE_NONE, YB_BACKBONE_RESNET, YB_BACKBONE_DARKNET = -1, 0, 1
 YB_PREC_F32, YB_PREC_F16TC, YB_PREC_F16X3 = 0, 1, 2
 PRECISIONS = {"f32": YB_PREC_F32, "f16tc": YB_PREC_F16TC, "f16x3": YB_PREC_F16X3}
@@ -107,6 +128,8 @@ SIGNATURES = {
                                    c_void_p, c_void_p]),
     "yb_display_blend": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float,
                                  c_void_p, c_void_p]),
+    "yb_render_list": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_int,
+                               c_float, c_void_p, c_int, c_void_p]),
     "yb_dcn_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 14 +
                        [c_void_p]),
     "yb_conv2d": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 12 +

@@ -17,8 +17,8 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "csrc", "build")
 LIB = os.path.join(HERE, "libyolact_b200.so")
 
-SOURCES = ["capi.cu", "engine.cu", "tc_conv.cu", "stem_tc.cu", "simt_conv.cu", "pointwise.cu", "detect.cu", "mask.cu", "dcn.cu", "dcn_tc.cu", "evalops.cu"]
-HEADERS = ["common.cuh", "kernels.cuh", "engine.cuh", "tc_common.cuh", os.path.join(ROOT, "include", "yolact_b200.h")]
+SOURCES = ["capi.cu", "engine.cu", "tc_conv.cu", "stem_tc.cu", "simt_conv.cu", "pointwise.cu", "detect.cu", "mask.cu", "dcn.cu", "dcn_tc.cu", "evalops.cu", "render.cu"]
+HEADERS = ["common.cuh", "kernels.cuh", "engine.cuh", "tc_common.cuh", "mask_math.cuh", os.path.join(ROOT, "include", "yolact_b200.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -127,6 +127,15 @@ void require_device_frame(const yb_handle* h, const void* frame, const char* msg
   YB_REQUIRE(found && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == h->device, msg);
 }
 
+// The list entry points' pointer check: NULL, or device (or managed) memory of the handle's device.
+bool on_handle_device(const yb_handle* h, const void* p) {
+  if (!p) return true;
+  cudaPointerAttributes a;
+  const bool found = cudaPointerGetAttributes(&a, p) == cudaSuccess;
+  if (!found) cudaGetLastError();   // not a pointer CUDA knows: clear the error, then reject
+  return found && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == h->device;
+}
+
 }  // namespace
 
 extern "C" {
@@ -438,13 +447,7 @@ int yb_postprocess_list(yb_handle* h, const yb_post_item* h_items, int B, int ph
                         int mask_format, void* stream) {
   YB_API_BEGIN
   YB_REQUIRE(h && B >= 0 && (B == 0 || h_items), "yb_postprocess_list: bad argument");
-  auto on_device = [h](const void* p) {
-    if (!p) return true;
-    cudaPointerAttributes a;
-    const bool found = cudaPointerGetAttributes(&a, p) == cudaSuccess;
-    if (!found) cudaGetLastError();   // not a pointer CUDA knows: clear the error, then reject
-    return found && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == h->device;
-  };
+  auto on_device = [h](const void* p) { return on_handle_device(h, p); };
   for (int b = 0; b < B; ++b) {
     const yb_post_item& it = h_items[b];
     YB_REQUIRE(it.n >= 0 && it.out_h > 0 && it.out_w > 0, "yb_postprocess_list: n must be >= 0 and out_h, out_w > 0");
@@ -466,6 +469,39 @@ int yb_postprocess_list(yb_handle* h, const yb_post_item* h_items, int B, int ph
   PostSrc src{};
   src.table = table;
   launch_mask_assembly(src, h_items, B, ph, pw, k, crop_masks, mask_format, (cudaStream_t)stream, &h->lc);
+  YB_API_END
+}
+
+int yb_render_list(yb_handle* h, const yb_render_item* h_items, int B, int frame_is_u8, int ph, int pw, int k,
+                   int crop_masks, int top_k, float score_threshold, int class_color, float mask_alpha,
+                   const float* d_palette, int P, void* stream) {
+  YB_API_BEGIN
+  YB_REQUIRE(h && B >= 0 && (B == 0 || h_items), "yb_render_list: bad argument");
+  YB_REQUIRE(top_k >= 1, "yb_render_list: top_k must be >= 1");
+  YB_REQUIRE(P >= 1 && d_palette, "yb_render_list: the palette needs at least one colour");
+  YB_REQUIRE(on_handle_device(h, d_palette), "yb_render_list: the palette is not device memory of the handle's device");
+  auto on_device = [h](const void* p) { return on_handle_device(h, p); };
+  for (int b = 0; b < B; ++b) {
+    const yb_render_item& it = h_items[b];
+    YB_REQUIRE(it.frame && it.out, "yb_render_list: null frame or out");
+    YB_REQUIRE(it.n >= 0 && it.h > 0 && it.w > 0, "yb_render_list: n must be >= 0 and h, w > 0");
+    YB_REQUIRE(it.n == 0 || (it.box && it.cls && it.score && it.det_score && (!it.proto || it.coef)),
+               "yb_render_list: null coef, box, cls, score or det_score");
+    YB_REQUIRE(on_device(it.frame) && on_device(it.out) && on_device(it.proto) && on_device(it.coef) &&
+                   on_device(it.box) && on_device(it.cls) && on_device(it.score) && on_device(it.det_score) &&
+                   on_device(it.sel_n) && on_device(it.sel_cls) && on_device(it.sel_score) && on_device(it.sel_box),
+               "yb_render_list: a pointer is not device memory of the handle's device");
+  }
+  if (B == 0) return YB_OK;
+  CallGuard g(h, (cudaStream_t)stream);   // shared item and work tables: ordered behind the previous call
+  const size_t items_bytes = ((size_t)B * sizeof(yb_render_item) + 255) / 256 * 256;
+  char* ws = (char*)h->get_render_ws(items_bytes + render_work_bytes(B, top_k));
+  // pageable source: staged before the call returns, so the caller may reuse h_items at once.  Stream-ordered after
+  // the previous call (CallGuard), so its launches have read the tables before they are overwritten.
+  YB_CHECK_CUDA(cudaMemcpyAsync(ws, h_items, (size_t)B * sizeof(yb_render_item), cudaMemcpyHostToDevice,
+                                (cudaStream_t)stream));
+  launch_render(reinterpret_cast<const yb_render_item*>(ws), h_items, B, frame_is_u8, ph, pw, k, crop_masks, top_k,
+                score_threshold, class_color, mask_alpha, d_palette, P, ws + items_bytes, (cudaStream_t)stream, &h->lc);
   YB_API_END
 }
 

@@ -864,6 +864,7 @@ yb_handle::~yb_handle() {
   if (detect_ws) cudaFree(detect_ws);
   if (scratch) cudaFree(scratch);
   if (post_table) cudaFree(post_table);
+  if (render_ws) cudaFree(render_ws);
   if (cap_stream) cudaStreamDestroy(cap_stream);
   if (tune_stream) cudaStreamDestroy(tune_stream);
   for (auto s : lane_streams)
@@ -906,6 +907,21 @@ yb_post_item* yb_handle::get_post_table(int entries) {
     post_table_cap = cap;
   }
   return post_table;
+}
+
+void* yb_handle::get_render_ws(size_t bytes) {
+  if (bytes > render_ws_bytes) {
+    const size_t cap = std::max(bytes, std::max<size_t>(64 * 1024, 2 * render_ws_bytes));
+    if (render_ws) {
+      YB_CHECK_CUDA(cudaDeviceSynchronize());
+      cudaFree(render_ws);
+      render_ws = nullptr;
+      render_ws_bytes = 0;
+    }
+    YB_CHECK_CUDA(cudaMalloc(&render_ws, cap));
+    render_ws_bytes = cap;
+  }
+  return render_ws;
 }
 
 void* yb_handle::get_detect_ws(size_t bytes) {

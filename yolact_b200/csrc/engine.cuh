@@ -160,6 +160,8 @@ struct yb_handle {
   size_t scratch_bytes = 0;
   yb_post_item* post_table = nullptr;   // yb_postprocess_list's device item table
   int post_table_cap = 0;
+  void* render_ws = nullptr;            // yb_render_list's device item table and work table
+  size_t render_ws_bytes = 0;
   cudaStream_t cap_stream = nullptr;  // private stream used only for CUDA-graph capture
   cudaStream_t lane_streams[8] = {};  // branch streams joined into the capture (parallel graph branches)
   cudaEvent_t ev_fork = nullptr, ev_join[8] = {};
@@ -195,6 +197,7 @@ struct yb_handle {
   void* get_scratch(size_t bytes);
   void* get_detect_ws(size_t bytes);
   yb_post_item* get_post_table(int entries);
+  void* get_render_ws(size_t bytes);
 };
 
 namespace yb {

@@ -13,6 +13,7 @@
 //                         replaces pycocotools.mask.encode in Detections.add_mask (eval.py:320-330).
 //   display_blend       : the mask alpha-blend of prep_display (eval.py:186-209) + (img*255).byte().
 #include "kernels.cuh"
+#include "mask_math.cuh"
 
 namespace yb {
 
@@ -262,16 +263,7 @@ display_blend_kernel(const float* __restrict__ img, int img_is_255, const void* 
   const float inv = __fadd_rn(-alpha, 1.f);   // m * (-alpha) + 1 for m == 1
   for (int j = 0; j < n; ++j) {
     MaskReader<FORMAT> px{reinterpret_cast<const uint8_t*>(masks) + (size_t)j * plane_bytes, w, wpr};
-    if (px(y, x)) {
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        if (j == 0)
-          first[c] = s_col[c];
-        else
-          rest[c] = __fadd_rn(rest[c], __fmul_rn(s_col[j * 3 + c], prod));
-      }
-      prod = __fmul_rn(prod, inv);
-    }
+    if (px(y, x)) blend_step(j, s_col, inv, prod, first, rest);
   }
   float sum[3];
 #pragma unroll
@@ -280,10 +272,7 @@ display_blend_kernel(const float* __restrict__ img, int img_is_255, const void* 
   uint8_t* o = out + ((size_t)y * w + x) * 3;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    float v = img_is_255 ? __fdiv_rn(p[c], 255.f) : p[c];
-    v = __fadd_rn(__fmul_rn(v, prod), sum[c]);
-    v = __fmul_rn(v, 255.f);
-    o[c] = (uint8_t)(int)fminf(fmaxf(v, 0.f), 255.f);   // .byte(): truncation
+    o[c] = blend_out(img_is_255 ? __fdiv_rn(p[c], 255.f) : p[c], prod, sum[c]);
   }
 }
 

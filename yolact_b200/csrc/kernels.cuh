@@ -206,6 +206,15 @@ void launch_pack_detections(const float* box, const float* coef, const int64_t* 
 void launch_display_blend(const float* img, int img_is_255, const void* masks, int mask_format, int n, int h, int w,
                           const float* colors, float alpha, uint8_t* out, cudaStream_t stream, LaunchCounter* lc);
 
+// ---- prep_display's mask overlay from the detections (render.cu) ---------------------------------------------------
+// Device bytes of the work table launch_render needs for B images and top_k slots.
+size_t render_work_bytes(int B, int top_k);
+// Two launches for the B images of d_items (device; h_items is its host view): the selection, then the render of
+// every image's drawn masks over its frame.  work: render_work_bytes(B, top_k) bytes of device memory.
+void launch_render(const yb_render_item* d_items, const yb_render_item* h_items, int B, int frame_is_u8, int ph, int pw,
+                   int k, int crop, int top_k, float score_threshold, int class_color, float alpha,
+                   const float* palette, int P, void* work, cudaStream_t stream, LaunchCounter* lc);
+
 // ---- DCNv2 -------------------------------------------------------------------------------------
 // x NHWC (T) [B,H,W,C]; om = offset/mask conv output NHWC fp32 [B,Ho,Wo,27] (18 offsets
 // interleaved (dh,dw) per tap, then 9 masks: logits when mask_logits, dcn_v2.py:118-124); w: [9*C][Cout] (T);

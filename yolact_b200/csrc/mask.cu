@@ -19,37 +19,13 @@
 #include <stdlib.h>
 #include <algorithm>
 #include "kernels.cuh"
+#include "mask_math.cuh"
 
 namespace yb {
 
 namespace {
 
 constexpr int MT = 256;  // threads
-
-struct ColTab {  // per output column / row interpolation entry
-  int i0, i1;
-  float l0, l1;
-};
-
-__device__ __forceinline__ ColTab interp_entry(int dst, float scale, int in_size) {
-  // ATen area_pixel_compute_source_index, align_corners=False
-  float s = fmaxf(__fsub_rn(__fmul_rn(scale, (float)dst + 0.5f), 0.5f), 0.f);
-  ColTab t;
-  t.i0 = (int)s;
-  if (t.i0 > in_size - 1) t.i0 = in_size - 1;
-  t.i1 = t.i0 + (t.i0 < in_size - 1 ? 1 : 0);
-  t.l1 = __fsub_rn(s, (float)t.i0);
-  t.l0 = __fsub_rn(1.f, t.l1);
-  return t;
-}
-
-// sanitize_coordinates(cast=False) (box_utils.py:327-346)
-__device__ __forceinline__ void sanitize(float a, float b, int size, int padding, float* lo, float* hi) {
-  float x1 = __fmul_rn(a, (float)size), x2 = __fmul_rn(b, (float)size);
-  float mn = fminf(x1, x2), mx = fmaxf(x1, x2);
-  *lo = fmaxf(__fsub_rn(mn, (float)padding), 0.f);
-  *hi = fminf(__fadd_rn(mx, (float)padding), (float)size);
-}
 
 // Image z of a call: the list's table entry, or the dense batch's first image advanced by z strides.
 __device__ __forceinline__ yb_post_item post_item(const PostSrc& s, int z) {
@@ -141,12 +117,8 @@ mask_assembly_kernel(const PostSrc src, int ph, int pw, int k, int crop, int ban
 
   for (int d = d0; d < d1; ++d) {
     // crop window in prototype coordinates (box_utils.py:359-371)
-    float cx1 = 0.f, cx2 = (float)pw, cy1 = 0.f, cy2 = (float)ph;
-    if (crop) {
-      const float* bx = box + (size_t)d * 4;
-      sanitize(bx[0], bx[2], pw, 1, &cx1, &cx2);
-      sanitize(bx[1], bx[3], ph, 1, &cy1, &cy2);
-    }
+    float cx1, cx2, cy1, cy2;
+    crop_window(box, d, crop, ph, pw, cx1, cx2, cy1, cy2);
     // does any prototype row of this band survive the crop?
     bool any = false;
     for (int r = r_lo; r <= r_hi; ++r) any |= ((float)r >= cy1 && (float)r < cy2);
@@ -168,19 +140,7 @@ mask_assembly_kernel(const PostSrc src, int ph, int pw, int k, int crop, int ban
         const int rr = idx / cw;
         const int c = c_lo + (idx - rr * cw);
         const int pr = q_lo + rr;
-        const float4* pp = reinterpret_cast<const float4*>(proto + ((size_t)pr * pw + c) * k);
-        float acc = 0.f;
-        // not unrolled: an unrolled body keeps more loads in flight than the 40 registers that leave 6 CTAs per SM
-#pragma unroll 1
-        for (int j = 0; j < k / 4; ++j) {
-          const float4 q = __ldg(pp + j);
-          const float4 w4 = __ldg(reinterpret_cast<const float4*>(cf) + j);   // same address in every lane: one L1 broadcast
-          acc = fmaf(q.x, w4.x, acc);
-          acc = fmaf(q.y, w4.y, acc);
-          acc = fmaf(q.z, w4.z, acc);
-          acc = fmaf(q.w, w4.w, acc);
-        }
-        mrows[(size_t)(pr - r_lo) * pw + c] = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-acc)));  // torch.sigmoid
+        mrows[(size_t)(pr - r_lo) * pw + c] = lincomb_sigmoid(proto + ((size_t)pr * pw + c) * k, cf, k);
       }
       __syncthreads();
     }
@@ -195,8 +155,8 @@ mask_assembly_kernel(const PostSrc src, int ph, int pw, int k, int crop, int ban
       } else {
         // output columns whose interpolation sources can fall inside the crop window (conservative superset,
         // same bounds as the fp32 / uint8 path below): words entirely outside are zero without evaluation
-        const int xa = max((int)floorf(__fdiv_rn(cx1 - 0.5f, scale_w) - 0.5f) - 1, 0);
-        const int xb = min((int)ceilf(__fdiv_rn(ceilf(cx2) + 0.5f, scale_w) - 0.5f) + 1, out_w);
+        int xa, xb;
+        window_out_bounds(cx1, cx2, scale_w, out_w, &xa, &xb);
         const int wrp = tid >> 5, lane = tid & 31;
         for (int wi = wrp; wi < words; wi += MT / 32) {
           const int yy = wi / wpr, wx = wi - yy * wpr;
@@ -214,10 +174,7 @@ mask_assembly_kernel(const PostSrc src, int ph, int pw, int k, int crop, int ban
             const float* ra = mrows + (size_t)(rt.i0 - r_lo) * pw;
             const float* rb = mrows + (size_t)(rt.i1 - r_lo) * pw;
             const ColTab ct = coltab[x];
-            float top = __fadd_rn(__fmul_rn(ct.l0, ra[ct.i0]), __fmul_rn(ct.l1, ra[ct.i1]));
-            float bot = __fadd_rn(__fmul_rn(ct.l0, rb[ct.i0]), __fmul_rn(ct.l1, rb[ct.i1]));
-            float v = __fadd_rn(__fmul_rn(rt.l0, top), __fmul_rn(rt.l1, bot));
-            bit = v > 0.5f;
+            bit = bilinear4(rt, ct, ra, rb, ct.i0, ct.i1) > 0.5f;
           }
           const uint32_t word = __ballot_sync(0xffffffffu, bit);
           if (lane == 0) out[(size_t)y * wpr + wx] = word;
@@ -225,14 +182,9 @@ mask_assembly_kernel(const PostSrc src, int ph, int pw, int k, int crop, int ban
       }
     } else if (any) {
       // ---- phase B: only the output columns whose interpolation sources can fall inside the crop window
-      //      (a conservative superset: pixels outside interpolate zeros), only the ones are stored.
-      // A pixel x reads source columns i0 = floor(s), i1 = i0 + 1 with s = scale*(x+0.5)-0.5; the columns inside the
-      // window are the integers in [ceil(cx1), ceil(cx2)).  i1 >= ceil(cx1) needs s >= ceil(cx1) - 1 (cx1 - 0.5 below is
-      // smaller still), i0 < ceil(cx2) needs s < ceil(cx2): x < (ceil(cx2) + 0.5) / scale - 0.5.
-      int xa = (int)floorf(__fdiv_rn(cx1 - 0.5f, scale_w) - 0.5f) - 1;
-      int xb = (int)ceilf(__fdiv_rn(ceilf(cx2) + 0.5f, scale_w) - 0.5f) + 1;
-      xa = max(xa, 0);
-      xb = min(xb, out_w);
+      //      (window_out_bounds), only the ones are stored.
+      int xa, xb;
+      window_out_bounds(cx1, cx2, scale_w, out_w, &xa, &xb);
       const size_t band_off = (size_t)d * plane + (size_t)y0 * out_w;
       for (int yy = 0; yy < y1 - y0; ++yy) {
         const ColTab rt = interp_entry(y0 + yy, scale_h, ph);   // uniform
@@ -243,10 +195,7 @@ mask_assembly_kernel(const PostSrc src, int ph, int pw, int k, int crop, int ban
         for (int x = xa + tid; x < xb; x += MT) {
           const ColTab ct = coltab[x];
           if (!(((float)ct.i0 >= cx1 && (float)ct.i0 < cx2) || ((float)ct.i1 >= cx1 && (float)ct.i1 < cx2))) continue;
-          float top = __fadd_rn(__fmul_rn(ct.l0, ra[ct.i0]), __fmul_rn(ct.l1, ra[ct.i1]));
-          float bot = __fadd_rn(__fmul_rn(ct.l0, rb[ct.i0]), __fmul_rn(ct.l1, rb[ct.i1]));
-          float v = __fadd_rn(__fmul_rn(rt.l0, top), __fmul_rn(rt.l1, bot));
-          if (v > 0.5f) {
+          if (bilinear4(rt, ct, ra, rb, ct.i0, ct.i1) > 0.5f) {
             if (FORMAT == YB_MASK_F32)
               reinterpret_cast<float*>(masks_v())[band_off + (size_t)yy * out_w + x] = 1.f;
             else
@@ -286,12 +235,8 @@ __device__ __forceinline__ void proto_masks_row(const float* __restrict__ proto,
   __shared__ float s_coef[128];
   for (int j = threadIdx.x; j < k; j += MT) s_coef[j] = coef[(size_t)d * k + j];
   __syncthreads();
-  float cx1 = 0.f, cx2 = (float)pw, cy1 = 0.f, cy2 = (float)ph;
-  if (crop) {
-    const float* bx = box + (size_t)d * 4;
-    sanitize(bx[0], bx[2], pw, 1, &cx1, &cx2);
-    sanitize(bx[1], bx[3], ph, 1, &cy1, &cy2);
-  }
+  float cx1, cx2, cy1, cy2;
+  crop_window(box, d, crop, ph, pw, cx1, cx2, cy1, cy2);
   for (int c = threadIdx.x; c < pw; c += MT) {
     float v = 0.f;
     if ((float)c >= cx1 && (float)c < cx2 && (float)r >= cy1 && (float)r < cy2) {
@@ -304,7 +249,7 @@ __device__ __forceinline__ void proto_masks_row(const float* __restrict__ proto,
         acc = fmaf(q.z, s_coef[4 * j + 2], acc);
         acc = fmaf(q.w, s_coef[4 * j + 3], acc);
       }
-      v = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-acc)));
+      v = sigmoid_rn(acc);
     }
     out[((size_t)d * ph + r) * pw + c] = v;
   }

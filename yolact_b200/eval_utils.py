@@ -6,8 +6,9 @@
     display_blend(img, masks, colors, alpha)       <- the GPU mask blend inside prep_display (eval.py:186-209,226)
     get_color(j, classes, class_color)             <- prep_display's palette lookup (eval.py:169-183)
 
-prep_display itself (top-k selection, OpenCV text and boxes, eval.py:135-262) is caller code and is NOT rebuilt: the
-caller keeps its own loop and replaces the ten ATen ops of the blend by `display_blend` (INTEGRATION.md section 1).
+prep_display itself (eval.py:135-262) is caller code and is NOT rebuilt here: a caller that keeps its own loop replaces
+the ten ATen ops of the blend by `display_blend`; yolact_b200.display.render_masks does the whole GPU part (postprocess
+to .byte()) for a list of frames and leaves only the OpenCV text and boxes to the caller (INTEGRATION.md section 1).
 
 The reference multiplies two dense float matrices for the mask IoU and ships fp32 masks over PCIe for the RLE;
 here masks are 1 bit per pixel on the GPU (32x fewer bytes), the IoU is AND + popcount, and only the run
