@@ -43,6 +43,8 @@
  *   yb_dcn_forward     <- dcn_v2_forward (external/DCNv2/src/dcn_v2.h:9-39,
  *                         src/cuda/dcn_v2_cuda.cu:42-172, src/cuda/dcn_v2_im2col_cuda.cu:125-195)
  *   yb_conv2d          <- nn.Conv2d + folded BatchNorm2d + activation (+ residual), op-level test hook
+ *   yb_conv2d_ex       <- the same with the network's other epilogues (residual after the activation, fp32 output,
+ *                         zero-padded channels, the fused prediction head) and the tensor-core stem, op-level test hook
  */
 #ifndef YOLACT_B200_H_
 #define YOLACT_B200_H_
@@ -378,6 +380,33 @@ YB_API int yb_conv2d(yb_handle* h, const float* d_x, const float* h_w, const flo
               const float* d_residual, float* d_y, int B, int Ci, int H, int W, int Co,
               int kh, int kw, int stride, int pad, int act, int precision, int iters,
               float* ms, void* stream);
+
+/* The cases of the network's convolutions yb_conv2d cannot express (a zeroed struct = none of them). */
+typedef struct {
+  int32_t res_after_act;         /* y = act(conv) + residual (Darknet blocks) instead of act(conv + residual) */
+  int32_t y_f32;                 /* precision 1, 2 or 3: fp32 output straight from the epilogue */
+  int32_t cin_pad;               /* x has max(Ci, cin_pad) channels; the weights get zero rows for the extra ones */
+  int32_t cout_pad;              /* precision 1 or 3: the output has max(Co, cout_pad) channels, zeros beyond Co */
+  int32_t y_pix_stride;          /* fp32 output: elements from one output pixel to the next (>= Co; 0 = Co) */
+  int32_t poison;                /* fill d_y with 0xff bytes (fp16 and fp32 NaN) before the launch */
+  int32_t nseg;                  /* precision 1 or 3, 0..3: fused prediction head.  Output channels */
+  int32_t seg_begin[3];          /*   [seg_begin[i], seg_end[i]) (ascending, disjoint, within Co) go to the fp32 */
+  int32_t seg_end[3];            /*   device tensor seg_y[i] at b * seg_batch_stride[i] + pixel * seg_pix_stride[i] */
+  int32_t seg_act[3];            /*   + channel - seg_begin[i], with activation seg_act[i]; other channels are not */
+  int32_t seg_pix_stride[3];     /*   stored; act and d_y are ignored */
+  int64_t seg_batch_stride[3];
+  float* seg_y[3];
+} yb_conv_opts;
+
+/* yb_conv2d with options, and the output in the kernel's own layout: d_y is NHWC [B,Ho,Wo,Cp] (Cp = max(Co, cout_pad);
+ * device, 16-byte aligned) of fp32 (precision 0, or y_f32; [B,Ho,Wo,y_pix_stride] when that is set), fp16 (precision
+ * 1 and 2) or, in precision 3, hi / lo fp16 pairs [B,Ho,Wo,hi(Cp) | lo(Cp)] whose value is hi + lo * 2^-11.  The residual is
+ * NCHW fp32 [B,Co,Ho,Wo] as in yb_conv2d.  Precision 1 and 3 with Ci == 3 and the network's stem shapes
+ * (7x7/2 pad 3 -> 64, 3x3/1 pad 1 -> 32) run the tensor-core stem kernel, cout_pad its zero-padded channels.  The
+ * YB_CONV2D_* tiling switches apply as in yb_conv2d.  opts is nullable. */
+YB_API int yb_conv2d_ex(yb_handle* h, const float* d_x, const float* h_w, const float* h_bias,
+                        const float* d_residual, void* d_y, int B, int Ci, int H, int W, int Co, int kh, int kw,
+                        int stride, int pad, int act, int precision, const yb_conv_opts* opts, void* stream);
 
 /* ---- introspection ----------------------------------------------------------------------------- */
 /* Kernel launches issued by this handle since creation (bench.py's gpu_launches). */

@@ -50,6 +50,19 @@ def test_config_struct_matches_header_layout(tmp_path):
                    _lib.YbConfig.ars_f64.offset]
 
 
+def test_conv_opts_struct_matches_header_layout(tmp_path):
+    fields = ("cout_pad", "nseg", "seg_begin", "seg_pix_stride", "seg_batch_stride", "seg_y")
+    src = tmp_path / "layout.c"
+    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "yolact_b200.h"\n'
+                   'int main(void) { printf("%zu' + ' %zu' * len(fields) + '\\n", sizeof(yb_conv_opts)' +
+                   "".join(", offsetof(yb_conv_opts, %s)" % f for f in fields) + '); return 0; }\n')
+    exe = tmp_path / "layout"
+    import subprocess
+    subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
+    got = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
+    assert got == [ctypes.sizeof(_lib.YbConvOpts)] + [getattr(_lib.YbConvOpts, f).offset for f in fields]
+
+
 @pytest.mark.parametrize("name", sorted(CONFIGS))
 def test_state_dict_keys_match_reference(name):
     ref = json.load(open(os.path.join(GOLDEN, "state_keys.json")))[name]

@@ -15,14 +15,13 @@ import torch
 
 from oracle import yolact_oracle as O
 from tests.dcn_probe import GEOMETRIES, build_probe_case, out_hw, selected_columns
+from tests.error_bounds import UNIT, worst
 from yolact_b200 import _lib
 from yolact_b200.dcn_v2 import _handle, dcn_v2_conv
 
 pytestmark = pytest.mark.gpu
 
 YB_ERR_INVALID = -1       # include/yolact_b200.h
-U16, U22, U24 = 2.0 ** -11, 2.0 ** -22, 2.0 ** -24   # unit roundoff of fp16, of the hi+lo pair, of fp32
-UNIT = {"f32": U24, "f16tc": U16, "f16x3": U22}
 # Whole-output bound, per element: |y - ref| <= K * unit * scale, scale = sum_k |w_k| * mag_k + |bias|, where
 # mag = sum over corners |weight * mask * x| is what a rounding error of one sample is proportional to.
 #  f16tc  1 for the fp16 rounding of the output (coherent: |y| <= scale) + 1 for the roundings of the operands -- x,
@@ -45,14 +44,6 @@ def t(a):
 
 def run(x, off, msk, w, bias, stride, pad, dil, precision):
     return dcn_v2_conv(t(x), t(off), t(msk), t(w), t(bias), stride, pad, dil, 1, precision=precision).cpu().numpy()
-
-
-def worst(err, tol):
-    """Index and values of the element that exceeds its tolerance the most (for the assertion message)."""
-    bad = ~(err <= tol)
-    ratio = np.where(bad, np.where(np.isfinite(err), err, np.inf) / np.maximum(tol, 1e-300), 0)
-    at = np.unravel_index(np.argmax(ratio), err.shape)
-    return "%d elements over; worst at %s: err %.4g tol %.4g" % (bad.sum(), at, err[at], tol[at])
 
 
 def random_inputs(r, B, C, Co, H, W, stride, pad=1, dil=1):

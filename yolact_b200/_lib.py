@@ -76,6 +76,25 @@ class YbRenderItem(ctypes.Structure):
     ]
 
 
+class YbConvOpts(ctypes.Structure):
+    """Mirror of yb_conv_opts (yb_conv2d_ex)."""
+    _fields_ = [
+        ("res_after_act", c_int32),
+        ("y_f32", c_int32),
+        ("cin_pad", c_int32),
+        ("cout_pad", c_int32),
+        ("y_pix_stride", c_int32),
+        ("poison", c_int32),
+        ("nseg", c_int32),
+        ("seg_begin", c_int32 * 3),
+        ("seg_end", c_int32 * 3),
+        ("seg_act", c_int32 * 3),
+        ("seg_pix_stride", c_int32 * 3),
+        ("seg_batch_stride", c_int64 * 3),
+        ("seg_y", c_void_p * 3),
+    ]
+
+
 YB_BACKBONE_NONE, YB_BACKBONE_RESNET, YB_BACKBONE_DARKNET = -1, 0, 1
 YB_PREC_F32, YB_PREC_F16TC, YB_PREC_F16X3 = 0, 1, 2
 PRECISIONS = {"f32": YB_PREC_F32, "f16tc": YB_PREC_F16TC, "f16x3": YB_PREC_F16X3}
@@ -134,6 +153,8 @@ SIGNATURES = {
                        [c_void_p]),
     "yb_conv2d": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 12 +
                   [POINTER(c_float), c_void_p]),
+    "yb_conv2d_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 11 +
+                     [POINTER(YbConvOpts), c_void_p]),
     "yb_launch_count": (c_int64, [c_void_p]),
     "yb_set_profiling": (c_int, [c_void_p, c_int]),
     "yb_last_forward_ms": (c_int, [c_void_p, POINTER(c_float), POINTER(c_float)]),

@@ -112,6 +112,35 @@ struct TempPool {  // RAII device temporaries for the op-level hooks
   }
 };
 
+// The tensor-core plan of an op-level conv hook, tiled as the YB_CONV2D_* switches ask (unset = the heuristic), with
+// its stream-K workspace (zeroed on s) from tp.
+TcConvPlan* hook_tc_plan(const ConvProblem& p, const __half* w, TempPool& tp, cudaStream_t s) {
+  auto env = [](const char* name) {
+    const char* v = getenv(name);
+    return v ? atoi(v) : 0;
+  };
+  TcTiling want;
+  want.bn = env("YB_CONV2D_BN");
+  want.grid = env("YB_CONV2D_GRID");
+  want.pair = env("YB_CONV2D_PAIR");
+  want.mma_groups = env("YB_CONV2D_EPI");
+  want.pdl_friendly = env("YB_CONV2D_PDL");   // PDL-friendly plan + programmatic dependent launch
+  want.stream_k = env("YB_CONV2D_SK");
+  TcConvPlan* plan = tc_conv_plan_create(p, w, want);
+  if (want.pdl_friendly) tc_conv_plan_set_pdl(plan, 1);
+  if (tc_conv_plan_tiling(plan).stream_k) {
+    try {
+      void* ws = tp.get(tc_conv_sk_workspace_bytes());
+      YB_CHECK_CUDA(cudaMemsetAsync(ws, 0, tc_conv_sk_workspace_bytes(), s));
+      tc_conv_plan_set_sk_workspace(plan, ws);
+    } catch (...) {
+      tc_conv_plan_destroy(plan);
+      throw;
+    }
+  }
+  return plan;
+}
+
 // data/config.py:28-29 (BGR order): the transform's mean / std when the caller passes NULL
 const float kMeans[3] = {103.94f, 116.78f, 123.68f};
 const float kStd[3] = {57.38f, 57.12f, 58.40f};
@@ -774,26 +803,7 @@ int yb_conv2d(yb_handle* h, const float* d_x, const float* h_w, const float* h_b
   const void* wd = tp.put(pw);
   p.out_scale = pw.out_scale;
   if (tc) {
-    {
-      auto env = [](const char* name) {
-        const char* v = getenv(name);
-        return v ? atoi(v) : 0;
-      };
-      TcTiling want;
-      want.bn = env("YB_CONV2D_BN");
-      want.grid = env("YB_CONV2D_GRID");
-      want.pair = env("YB_CONV2D_PAIR");
-      want.mma_groups = env("YB_CONV2D_EPI");
-      want.pdl_friendly = env("YB_CONV2D_PDL");   // PDL-friendly plan + programmatic dependent launch
-      want.stream_k = env("YB_CONV2D_SK");
-      plan = tc_conv_plan_create(p, (const __half*)wd, want);
-      if (want.pdl_friendly) tc_conv_plan_set_pdl(plan, 1);
-      if (tc_conv_plan_tiling(plan).stream_k) {
-        void* ws = tp.get(tc_conv_sk_workspace_bytes());
-        YB_CHECK_CUDA(cudaMemsetAsync(ws, 0, tc_conv_sk_workspace_bytes(), s));
-        tc_conv_plan_set_sk_workspace(plan, ws);
-      }
-    }
+    plan = hook_tc_plan(p, (const __half*)wd, tp, s);
     run = [&]() { launch_tc_conv(plan, s, &h->lc); };
   } else {
     run = [&]() { launch_simt_conv(p, wd, precision == 2 ? SIMT_F16 : SIMT_F32, s, &h->lc); };
@@ -825,6 +835,137 @@ int yb_conv2d(yb_handle* h, const float* d_x, const float* h_w, const float* h_b
   else
     launch_nhwc_to_nchw_f32<__half>((const __half*)y, d_y, B, Ho, Wo, Co, s, &h->lc, sp);
   YB_CHECK_CUDA(cudaStreamSynchronize(s));
+  YB_API_END
+}
+
+int yb_conv2d_ex(yb_handle* h, const float* d_x, const float* h_w, const float* h_bias, const float* d_residual,
+                 void* d_y, int B, int Ci, int H, int W, int Co, int kh, int kw, int stride, int pad, int act,
+                 int precision, const yb_conv_opts* opts, void* stream) {
+  YB_API_BEGIN
+  yb_conv_opts o;
+  memset(&o, 0, sizeof(o));
+  if (opts) o = *opts;
+  YB_REQUIRE(h && d_x && h_w && (d_y || o.nseg > 0), "yb_conv2d_ex: null argument");
+  YB_REQUIRE(precision >= 0 && precision <= 3, "yb_conv2d_ex: precision must be 0, 1, 2 or 3 (as yb_conv2d's)");
+  YB_REQUIRE(o.nseg >= 0 && o.nseg <= 3, "yb_conv2d_ex: nseg must be 0..3");
+  const bool tc = precision == 1 || precision == 3, f16 = precision != 0;
+  const int sp = (precision == 3) ? 1 : 0;
+  const int CiP = std::max(Ci, o.cin_pad), CoP = std::max(Co, o.cout_pad);
+  YB_REQUIRE(tc || (CoP == Co && o.nseg == 0), "yb_conv2d_ex: cout_pad and nseg need the tensor cores (precision 1 or 3)");
+  YB_REQUIRE(CoP == Co || (!d_residual && !o.y_f32 && o.nseg == 0),
+             "yb_conv2d_ex: cout_pad does not combine with a residual, y_f32 or nseg");
+  for (int i = 0; i < o.nseg; ++i)
+    YB_REQUIRE(o.seg_y[i] && o.seg_begin[i] >= (i ? o.seg_end[i - 1] : 0) && o.seg_end[i] > o.seg_begin[i] &&
+                   o.seg_end[i] <= Co && o.seg_pix_stride[i] >= o.seg_end[i] - o.seg_begin[i] && o.seg_batch_stride[i] >= 0,
+               "yb_conv2d_ex: the segments need outputs, ascending disjoint channel ranges within Co and strides");
+  const bool y_f32 = !f16 || o.y_f32;
+  const int ps = o.y_pix_stride > 0 ? o.y_pix_stride : CoP;   // fp32 output pixel stride
+  YB_REQUIRE(ps == CoP || (y_f32 && ps > Co && o.nseg == 0), "yb_conv2d_ex: y_pix_stride needs an fp32 output and >= Co");
+  CallGuard g(h);
+  cudaStream_t s = (cudaStream_t)stream;
+  const int Ho = (H + 2 * pad - kh) / stride + 1, Wo = (W + 2 * pad - kw) / stride + 1;
+  YB_REQUIRE(Ho >= 1 && Wo >= 1, "yb_conv2d_ex: empty output");
+  if (o.poison && o.nseg == 0)
+    YB_CHECK_CUDA(cudaMemsetAsync(d_y, 0xff, (size_t)B * Ho * Wo * (y_f32 ? 4 * ps : sp ? 4 * CoP : 2 * CoP), s));
+  TempPool tp;
+  float* bias = nullptr;
+  if (h_bias) {   // zeros for the padding channels, as the network's packer writes them
+    bias = (float*)tp.get((size_t)CoP * 4);
+    YB_CHECK_CUDA(cudaMemsetAsync(bias, 0, (size_t)CoP * 4, s));
+    YB_CHECK_CUDA(cudaMemcpyAsync(bias, h_bias, (size_t)Co * 4, cudaMemcpyHostToDevice, s));
+  }
+  const WFormat fmt = sp ? WFormat::Split : f16 ? WFormat::F16 : WFormat::F32;
+  if (tc && kh == kw && stem_tc_supported(kh, stride, pad, Ci, Co)) {
+    YB_REQUIRE(!d_residual && !o.y_f32 && !o.res_after_act && o.nseg == 0 && CiP == Ci,
+               "yb_conv2d_ex: the tensor-core stem takes no residual, y_f32, res_after_act, nseg or cin_pad");
+    const PackedWeights pw = pack_weights(h_w, Co, Ci, kh, kw, nullptr, WLayout::Stem, fmt);
+    StemTcPlan* plan = stem_tc_plan_create(d_x, (const __half*)tp.put(pw), bias, (__half*)d_y, B, H, W, kh, stride, pad,
+                                           Co, act, sp, pw.out_scale, CoP);
+    try {
+      launch_stem_tc(plan, s, &h->lc);
+    } catch (...) {
+      stem_tc_plan_destroy(plan);
+      throw;
+    }
+    stem_tc_plan_destroy(plan);
+    YB_CHECK_CUDA(cudaStreamSynchronize(s));  // temporaries are freed on return
+    return YB_OK;
+  }
+  const size_t es = (f16 && !sp) ? 2 : 4;   // split: two halfs per element
+  void* x = tp.get((size_t)B * H * W * CiP * es);
+  void* res = d_residual ? tp.get((size_t)B * Ho * Wo * Co * es) : nullptr;
+  if (!f16) {
+    launch_nchw_f32_to_nhwc<float>(d_x, (float*)x, B, CiP, H, W, s, &h->lc);
+    if (res) launch_nchw_f32_to_nhwc<float>(d_residual, (float*)res, B, Co, Ho, Wo, s, &h->lc);
+  } else {
+    launch_nchw_f32_to_nhwc<__half>(d_x, (__half*)x, B, CiP, H, W, s, &h->lc, sp);
+    if (res) launch_nchw_f32_to_nhwc<__half>(d_residual, (__half*)res, B, Co, Ho, Wo, s, &h->lc, sp);
+  }
+  ConvProblem p;
+  p.B = B;
+  p.H = H;
+  p.W = W;
+  p.Cin = CiP;
+  p.Ho = Ho;
+  p.Wo = Wo;
+  p.Cout = CoP;
+  p.KH = kh;
+  p.KW = kw;
+  p.stride = stride;
+  p.pad = pad;
+  p.act = act;
+  p.x = x;
+  p.split = sp;
+  p.bias = bias;
+  p.residual = res;
+  p.res_after_act = o.res_after_act ? 1 : 0;
+  p.y = d_y;
+  p.y_f32 = (f16 && o.y_f32) ? 1 : 0;
+  p.y_pix_stride = y_f32 ? ps : sp ? 2 * CoP : CoP;
+  p.y_batch_stride = (int64_t)Ho * Wo * p.y_pix_stride;
+  p.nseg = o.nseg;
+  for (int i = 0; i < o.nseg; ++i) {   // as the network's fused head sets them up (engine.cu fused_head)
+    p.seg_begin[i] = o.seg_begin[i];
+    p.seg_end[i] = o.seg_end[i];
+    p.seg_act[i] = o.seg_act[i];
+    p.seg_ps[i] = o.seg_pix_stride[i];
+    p.seg_bs[i] = o.seg_batch_stride[i];
+    p.seg_y[i] = o.seg_y[i];
+  }
+  if (o.nseg > 0) {
+    p.y = o.seg_y[0];
+    p.y_f32 = 1;
+    p.y_pix_stride = o.seg_pix_stride[0];
+    p.y_batch_stride = o.seg_batch_stride[0];
+  }
+  // input channels beyond Ci are zeros that meet zero weights: the tensor-core packer pads its rows, the CUDA-core
+  // kernel gets zero-padded OIHW weights
+  std::vector<float> wpad;
+  const float* w = h_w;
+  if (!tc && CiP > Ci) {
+    const size_t taps = (size_t)kh * kw;
+    wpad.assign((size_t)Co * CiP * taps, 0.f);
+    for (int c = 0; c < Co; ++c) memcpy(&wpad[(size_t)c * CiP * taps], h_w + (size_t)c * Ci * taps, Ci * taps * 4);
+    w = wpad.data();
+  }
+  YB_REQUIRE(!tc || tc_conv_supported(p), "yb_conv2d_ex: shape not supported by the tensor-core kernel (Cin % 64, taps <= 9)");
+  const PackedWeights pw = tc ? pack_weights(w, Co, Ci, kh, kw, nullptr, WLayout::Conv, fmt, CiP, CoP)
+                              : pack_weights(w, Co, CiP, kh, kw, nullptr, WLayout::Simt, fmt);
+  const void* wd = tp.put(pw);
+  p.out_scale = pw.out_scale;
+  if (tc) {
+    TcConvPlan* plan = hook_tc_plan(p, (const __half*)wd, tp, s);
+    try {
+      launch_tc_conv(plan, s, &h->lc);
+    } catch (...) {
+      tc_conv_plan_destroy(plan);
+      throw;
+    }
+    tc_conv_plan_destroy(plan);
+  } else {
+    launch_simt_conv(p, wd, precision == 2 ? SIMT_F16 : SIMT_F32, s, &h->lc);
+  }
+  YB_CHECK_CUDA(cudaStreamSynchronize(s));  // temporaries are freed on return
   YB_API_END
 }
 

@@ -1136,6 +1136,9 @@ TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, co
   q.epi_tma = (!p.y_f32 && vec_ok && p.Cout % 8 == 0 && p.nseg == 0) ? 1 : 0;
   // split: a 64-channel hi box must not run into the lo plane of the same pixel (nothing clips it there)
   if (split && q.epi_tma && p.Cout % 64 != 0) q.epi_tma = 0;
+  // the staged epilogue has an act-then-add instance for LeakyReLU (Darknet blocks) only (epi_staged_act)
+  YB_REQUIRE(!q.epi_tma || !p.res_after_act || p.act == ACT_LEAKY || p.act == ACT_NONE,
+             "tc_conv: a residual after the activation needs LeakyReLU (or none) with a half-precision output");
   // the staged epilogue moves 64-channel boxes: a CTA must own at least 64 output channels
   const int bn_min = q.epi_tma ? 64 : 32;
 
