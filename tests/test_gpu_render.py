@@ -112,6 +112,23 @@ def test_render_matches_the_composition(top_k, thr):
     check(dets, frames_for(SIZES, 1 + top_k, torch.float32), top_k, thr)
 
 
+def test_render_nan_boxes_match_the_composition():
+    """A box with a NaN coordinate crops its mask to nothing (box_utils.crop: every comparison with NaN is false), so
+    the row is drawn nowhere; its pixel box is postprocess's .long() of the NaN."""
+    ybcfg.set_cfg("yolact_base_config")
+    dets = [make_dets(12, 138, 138, 21), make_dets(9, 138, 138, 22)]
+    nan, inf = float("nan"), float("inf")
+    for d in dets:
+        box = d["box"].clone()
+        box[1, 0] = box[3, 2] = box[4, 1] = box[6, 3] = nan
+        box[5] = nan
+        box[7] = torch.tensor([-inf, 0.2, inf, 0.9])
+        box[8] = torch.tensor([0.1, -3e38, 0.6, 3e38])
+        d["box"] = box
+    for crop in (True, False):
+        check(dets, frames_for([(203, 277), (550, 550)], 23, torch.uint8), 15, 0, crop_masks=crop)
+
+
 def test_render_im700_prototypes_and_a_batch_tensor():
     ybcfg.set_cfg("yolact_im700_config")
     dets = [make_dets(n, 176, 176, 300 + n) for n in (100, 31)]

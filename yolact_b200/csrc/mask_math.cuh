@@ -23,12 +23,15 @@ __device__ __forceinline__ ColTab interp_entry(int dst, float scale, int in_size
   return t;
 }
 
-// sanitize_coordinates(cast=False) (box_utils.py:327-346)
+// sanitize_coordinates(cast=False) (box_utils.py:327-346).  torch.min, torch.max and clamp propagate NaN where
+// fminf / fmaxf drop it: a NaN coordinate makes both ends NaN, so every crop comparison fails (an empty mask) and the
+// pixel box converts NaN exactly as Tensor.long() does.
 __device__ __forceinline__ void sanitize(float a, float b, int size, int padding, float* lo, float* hi) {
   float x1 = __fmul_rn(a, (float)size), x2 = __fmul_rn(b, (float)size);
   float mn = fminf(x1, x2), mx = fmaxf(x1, x2);
   *lo = fmaxf(__fsub_rn(mn, (float)padding), 0.f);
   *hi = fminf(__fadd_rn(mx, (float)padding), (float)size);
+  if (isnan(x1) || isnan(x2)) *lo = *hi = __int_as_float(0x7fffffff);
 }
 
 // crop window of one detection in prototype coordinates (box_utils.py:359-371); the whole map without crop.  A position
@@ -47,8 +50,13 @@ __device__ __forceinline__ void crop_window(const float* box, int d, int crop, i
 // superset: pixels outside interpolate zeros).  A pixel x reads source columns i0 = floor(s), i1 = i0 + 1 with
 // s = scale*(x+0.5)-0.5; the columns inside the window are the integers in [ceil(cx1), ceil(cx2)).  i1 >= ceil(cx1)
 // needs s >= ceil(cx1) - 1 (cx1 - 0.5 below is smaller still), i0 < ceil(cx2) needs s < ceil(cx2):
-// x < (ceil(cx2) + 0.5) / scale - 0.5.  Rows are the same with the vertical window and scale.
+// x < (ceil(cx2) + 0.5) / scale - 0.5.  Rows are the same with the vertical window and scale.  An empty or NaN window
+// (!(c1 < c2)) reaches no pixel.
 __device__ __forceinline__ void window_out_bounds(float c1, float c2, float scale, int out_size, int* a, int* b) {
+  if (!(c1 < c2)) {
+    *a = *b = 0;
+    return;
+  }
   *a = max((int)floorf(__fdiv_rn(c1 - 0.5f, scale) - 0.5f) - 1, 0);
   *b = min((int)ceilf(__fdiv_rn(ceilf(c2) + 0.5f, scale) - 0.5f) + 1, out_size);
 }
