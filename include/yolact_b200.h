@@ -28,6 +28,8 @@
  *                         sanitize_coordinates (layers/box_utils.py:327-373), F.interpolate bilinear
  *   yb_postprocess_list <- the same, called once per image of a batch of differently sized images (evalimages over a
  *                         folder, eval.py:612-625)
+ *   yb_coco_rle_list   <- postprocess + pycocotools.mask.encode + rleToString in prep_metrics' --output_coco_json path
+ *                         (eval.py:320-330, :414-429), for a list of images, without materialising masks
  *   yb_maskiou         <- FastMaskIoUNet.forward (yolact.py:363-375) + gather (output_utils.py:79-83)
  *   yb_fast_base_transform <- FastBaseTransform.forward (utils/augmentations.py:616-658)
  *   yb_infer_frames    <- FastBaseTransform()(frames) followed by Yolact.forward in eval mode, as evalimage /
@@ -271,6 +273,25 @@ typedef struct {
  * of the handle's device. */
 YB_API int yb_postprocess_list(yb_handle* h, const yb_post_item* h_items, int B, int ph, int pw, int k,
                                int crop_masks, int mask_format, void* stream);
+
+/* eval.py's --output_coco_json masks for a list of B images, in ONE launch, without materialising them: for every row of
+ * every image (rows numbered image by image, n rows each), the pycocotools rleToString string of the mask
+ * yb_postprocess_list would produce for that row at out_h x out_w with crop_masks (bilinear, > 0.5), zero-area boxes
+ * included: its runs are yb_mask_rle's on yb_postprocess's masks, bit for bit.  h_items as for yb_postprocess_list
+ * (proto, coef, box, n, out_h, out_w are read; masks, boxes_px and proto_masks are ignored).
+ *   d_runs uint32 [runs_cap]: scratch for the rows' run lengths;  d_chars [chars_cap]: the strings (not
+ *   NUL-terminated), row r's at d_chars + d_row_off[r], d_row_len[r] characters (int64 / int32 [rows]).  Rows reserve
+ *   their space by atomic add, so the strings need not be in row order.
+ *   d_need int64 [2]: the runs and characters the rows asked for.  When either exceeds its cap, the rows that did not
+ *   fit have d_row_len -1; calling again with caps of at least d_need[0] and d_need[1] then fits every row (a row whose
+ *   runs did not fit asks for 7 characters per run, the most rleToString writes for one).
+ * The item table is uploaded into a table the handle owns (stream-ordered behind the handle's previous call); h_items
+ * may be reused as soon as the call returns.  B == 0 and n == 0 are allowed.  YB_ERR_INVALID, with nothing written, for
+ * a null proto, coef or box with n > 0, n < 0, out_h <= 0 or out_w <= 0, a null output, a negative cap, or a pointer
+ * that is not device memory of the handle's device. */
+YB_API int yb_coco_rle_list(yb_handle* h, const yb_post_item* h_items, int B, int ph, int pw, int k, int crop_masks,
+                            uint32_t* d_runs, int64_t runs_cap, char* d_chars, int64_t chars_cap, int64_t* d_row_off,
+                            int32_t* d_row_len, int64_t* d_need, void* stream);
 
 /* maskiou_net on [n,1,ph,pw] fp32 masks -> d_maskiou [n] = net(mask)[i, cls[i]];
  * d_cls == NULL: d_maskiou [n, num_classes-1] = net(mask) (FastMaskIoUNet.forward itself). */

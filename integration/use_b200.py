@@ -8,7 +8,7 @@
 or, from the shell:   python -m integration.use_b200 /path/to/yolact --trained_model=... --benchmark
 
 For the mAP mode, `install_metrics(E)` after `import eval as E` also moves prep_metrics' matching loop and calc_map to
-the GPU (yolact_b200.metrics).  The shell route runs eval.py as a fresh `__main__` module that cannot be patched, so it
+the GPU (yolact_b200.metrics); `install_coco_json(E)` does the same for --output_coco_json's records.  The shell route runs eval.py as a fresh `__main__` module that cannot be patched, so it
 keeps the reference's own loop.
 
 `install` puts the reference on sys.path, imports its modules and rebinds the names eval.py pulls from them
@@ -97,6 +97,35 @@ def install_metrics(E):
     prep_metrics.__doc__, calc_map.__doc__ = metrics.prep_metrics.__doc__, metrics.calc_map.__doc__
     E.prep_metrics, E.calc_map = prep_metrics, calc_map
     return {"prep_metrics": prep_metrics, "calc_map": calc_map}
+
+
+def install_coco_json(E):
+    """Wrap whatever E.prep_metrics is bound to now (the reference's, or install_metrics'; either install order works)
+    so that with --output_coco_json its records come from yolact_b200.metrics.Detections' GPU route: one
+    yb_coco_rle_list launch per image instead of full-size fp32 masks and pycocotools on the host.  The records are
+    appended to the reference's own `detections` object (bbox_data / mask_data, categories from E.get_coco_cat), so
+    evaluate()'s detections.dump() and dump_web() run unchanged.  Without the flag the call goes to the previous
+    binding."""
+    import yolact_b200
+    from yolact_b200 import metrics
+
+    prev = E.prep_metrics
+    live_keys = ("rescore_bbox", "rescore_mask", "eval_mask_branch")   # as install()'s postprocess re-reads them
+
+    def prep_metrics(ap_data, dets, img, gt, gt_masks, h, w, num_crowd, image_id, detections=None):
+        if not E.args.output_coco_json:
+            return prev(ap_data, dets, img, gt, gt_masks, h, w, num_crowd, image_id, detections)
+        ref_cfg = getattr(E, "cfg", None)
+        for key in live_keys:
+            if hasattr(ref_cfg, key):
+                setattr(yolact_b200.cfg, key, getattr(ref_cfg, key))
+        sink = metrics.Detections(E.get_coco_cat)
+        sink.bbox_data, sink.mask_data = detections.bbox_data, detections.mask_data
+        sink.add(dets[:1], [(h, w)], [image_id], crop_masks=E.args.crop, score_threshold=E.args.score_threshold)
+
+    prep_metrics.__doc__ = install_coco_json.__doc__
+    E.prep_metrics = prep_metrics
+    return {"prep_metrics": prep_metrics}
 
 
 if __name__ == "__main__":

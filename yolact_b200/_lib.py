@@ -136,6 +136,8 @@ SIGNATURES = {
     "yb_postprocess_batch": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                      c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "yb_postprocess_list": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "yb_coco_rle_list": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p,
+                                 c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "yb_maskiou": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "yb_fast_base_transform": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                        POINTER(c_float), POINTER(c_float), c_void_p, c_void_p]),

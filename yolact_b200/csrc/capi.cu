@@ -501,6 +501,36 @@ int yb_postprocess_list(yb_handle* h, const yb_post_item* h_items, int B, int ph
   YB_API_END
 }
 
+int yb_coco_rle_list(yb_handle* h, const yb_post_item* h_items, int B, int ph, int pw, int k, int crop_masks,
+                     uint32_t* d_runs, int64_t runs_cap, char* d_chars, int64_t chars_cap, int64_t* d_row_off,
+                     int32_t* d_row_len, int64_t* d_need, void* stream) {
+  YB_API_BEGIN
+  YB_REQUIRE(h && B >= 0 && (B == 0 || h_items), "yb_coco_rle_list: bad argument");
+  YB_REQUIRE(d_runs && d_chars && d_row_off && d_row_len && d_need, "yb_coco_rle_list: null output");
+  YB_REQUIRE(runs_cap >= 0 && chars_cap >= 0, "yb_coco_rle_list: negative capacity");
+  auto on_device = [h](const void* p) { return on_handle_device(h, p); };
+  YB_REQUIRE(on_device(d_runs) && on_device(d_chars) && on_device(d_row_off) && on_device(d_row_len) &&
+                 on_device(d_need),
+             "yb_coco_rle_list: an output is not device memory of the handle's device");
+  for (int b = 0; b < B; ++b) {
+    const yb_post_item& it = h_items[b];
+    YB_REQUIRE(it.n >= 0 && it.out_h > 0 && it.out_w > 0, "yb_coco_rle_list: n must be >= 0 and out_h, out_w > 0");
+    YB_REQUIRE(it.n == 0 || (it.proto && it.coef && it.box), "yb_coco_rle_list: null proto, coef or box");
+    YB_REQUIRE(on_device(it.proto) && on_device(it.coef) && on_device(it.box),
+               "yb_coco_rle_list: a pointer is not device memory of the handle's device");
+  }
+  CallGuard g(h, (cudaStream_t)stream);   // shared item table: ordered behind the previous call
+  yb_post_item* table = h->get_post_table(std::max(B, 1));
+  // pageable source: staged before the call returns, so the caller may reuse h_items at once.  Stream-ordered after
+  // the previous call (CallGuard), so its launches have read the table before it is overwritten.
+  if (B > 0)
+    YB_CHECK_CUDA(cudaMemcpyAsync(table, h_items, (size_t)B * sizeof(yb_post_item), cudaMemcpyHostToDevice,
+                                  (cudaStream_t)stream));
+  launch_coco_rle(table, h_items, B, ph, pw, k, crop_masks, d_runs, runs_cap, d_chars, chars_cap, d_row_off, d_row_len,
+                  d_need, (cudaStream_t)stream, &h->lc);
+  YB_API_END
+}
+
 int yb_render_list(yb_handle* h, const yb_render_item* h_items, int B, int frame_is_u8, int ph, int pw, int k,
                    int crop_masks, int top_k, float score_threshold, int class_color, float mask_alpha,
                    const float* d_palette, int P, void* stream) {

@@ -14,6 +14,7 @@
 //   display_blend       : the mask alpha-blend of prep_display (eval.py:186-209) + (img*255).byte().
 #include "kernels.cuh"
 #include "mask_math.cuh"
+#include "rle_walk.cuh"
 
 namespace yb {
 
@@ -148,97 +149,27 @@ struct MaskReader {
     if (FORMAT == YB_MASK_U8) return reinterpret_cast<const uint8_t*>(base)[(size_t)y * w + x] != 0;
     return reinterpret_cast<const float*>(base)[(size_t)y * w + x] != 0.f;
   }
+  __device__ __forceinline__ void chunk(int, int) const {}   // read in place: nothing to stage
 };
 
-__device__ __forceinline__ int rle_block_scan(int v, int* s_warp, int* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  int inc = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int n = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += n;
-  }
-  __syncthreads();
-  if (lane == 31) s_warp[wid] = inc;
-  __syncthreads();
-  int woff = 0, tot = 0;
-  const int nwarps = (int)(blockDim.x >> 5);
-  for (int w = 0; w < nwarps; ++w) {
-    int c = s_warp[w];
-    if (w < wid) woff += c;
-    tot += c;
-  }
-  *total = tot;
-  return woff + inc - v;
-}
-
-// One CTA per mask, one thread per column (up to 1024 per pass).  Thread t walks column c0+t top to bottom (reads are coalesced across the CTA),
-// once to count value changes and once to emit their column-major positions; a final in-place pass
-// turns positions into run lengths.  counts[0] is the number of leading zeros (0 when the mask starts
-// with a one), exactly maskApi.c's rleEncode.
+// One CTA per mask, one thread per column (up to 1024 per pass): the walk of rle_walk.cuh over the whole mask, then the
+// positions -> lengths pass.  counts[0] is the number of leading zeros (0 when the mask starts with a one), exactly
+// maskApi.c's rleEncode.
 template <int FORMAT>
 __global__ void __launch_bounds__(RLE_MAX_THREADS)
 mask_rle_kernel(const void* __restrict__ masks, size_t mask_stride_bytes, int h, int w, int wpr,
                 uint32_t* __restrict__ counts, int64_t cap, int32_t* __restrict__ nruns) {
   __shared__ int s_warp[RLE_MAX_THREADS / 32];
-  const int NT = (int)blockDim.x;
   const int d = blockIdx.x, tid = threadIdx.x;
   MaskReader<FORMAT> px{reinterpret_cast<const uint8_t*>(masks) + (size_t)d * mask_stride_bytes, w, wpr};
   uint32_t* out = counts + (int64_t)d * cap;
-  int64_t base = 0;   // transitions emitted by previous column chunks
-  for (int c0 = 0; c0 < w; c0 += NT) {
-    const int x = c0 + tid;
-    const bool active = x < w;
-    const int first_prev = (active && x > 0) ? px(h - 1, x - 1) : 0;
-    int cnt = 0;
-    if (active) {
-      int prev = first_prev;
-      for (int y = 0; y < h; ++y) {
-        const int v = px(y, x);
-        cnt += (v != prev);
-        prev = v;
-      }
-    }
-    int total;
-    int off = rle_block_scan(cnt, s_warp, &total);
-    if (active && cnt) {
-      int prev = first_prev;
-      int64_t o = base + off;
-      for (int y = 0; y < h; ++y) {
-        const int v = px(y, x);
-        if (v != prev) {
-          if (o < cap) out[o] = (uint32_t)x * (uint32_t)h + (uint32_t)y;
-          ++o;
-        }
-        prev = v;
-      }
-    }
-    base += total;
-  }
-  __syncthreads();
-  const int64_t T = base;   // number of value changes; runs = T + 1
+  const int64_t T = rle_walk(px, h, w, 0, w, 0, h, out, cap, s_warp);   // number of value changes; runs = T + 1
   if (T + 1 > cap) {
     if (tid == 0) nruns[d] = -(int32_t)(T + 1 < 0x7fffffffll ? T + 1 : 0x7fffffffll);   // overflow: caller must grow cap
     return;
   }
-  const uint32_t hw = (uint32_t)h * (uint32_t)w;
-  if (tid == 0) {
-    out[T] = T ? hw - out[T - 1] : hw;
-    nruns[d] = (int32_t)(T + 1);
-  }
-  __syncthreads();
-  // positions -> lengths, in place, from the back (a chunk only reads entries at or below itself)
-  for (int64_t hi = T; hi > 0; hi -= NT) {
-    const int64_t i = hi - 1 - tid;
-    uint32_t cur = 0, prv = 0;
-    if (i >= 0) {
-      cur = out[i];
-      prv = i > 0 ? out[i - 1] : 0u;
-    }
-    __syncthreads();
-    if (i >= 0) out[i] = cur - prv;
-    __syncthreads();
-  }
+  if (tid == 0) nruns[d] = (int32_t)(T + 1);
+  rle_positions_to_lengths(out, T, (uint32_t)h * (uint32_t)w);
 }
 
 // -------------------------------------------------------------------------------------------------

@@ -237,6 +237,14 @@ void launch_render(const yb_render_item* d_items, const yb_render_item* h_items,
                    int k, int crop, int top_k, float score_threshold, int class_color, float alpha,
                    const float* palette, int P, void* work, cudaStream_t stream, LaunchCounter* lc);
 
+// ---- eval.py's COCO results masks from the detections (cocorle.cu) --------------------------------------------------
+// One launch for the B images of d_items (device; h_items is its host view): every row's rleToString string of the mask
+// launch_mask_assembly would produce, in the chars arena at row_off[row] (row_len[row] characters, or -1 when an arena
+// was too small); need[0] / need[1] = the runs / characters all rows asked for.  Zeroes need first.
+void launch_coco_rle(const yb_post_item* d_items, const yb_post_item* h_items, int B, int ph, int pw, int k, int crop,
+                     uint32_t* runs, int64_t runs_cap, char* chars, int64_t chars_cap, int64_t* row_off,
+                     int32_t* row_len, int64_t* need, cudaStream_t stream, LaunchCounter* lc);
+
 // ---- DCNv2 -------------------------------------------------------------------------------------
 // x NHWC (T) [B,H,W,C]; om = offset/mask conv output NHWC fp32 [B,Ho,Wo,27] (18 offsets
 // interleaved (dh,dw) per tap, then 9 masks: logits when mask_logits, dcn_v2.py:118-124); w: [9*C][Cout] (T);

@@ -255,3 +255,146 @@ def print_maps(all_maps):
         print(cell(t) + "".join(cell("%.2f" % v if v < 100 else "%.1f" % v) for v in all_maps[t].values()))
     print(sep)
     print()
+
+
+# ---- --output_coco_json (eval.py:300-371, :414-429) -----------------------------------------------------------------
+def _category_fn(category_of):
+    """category_of: a sequence (or mapping) indexed by class, or a callable (eval.py's get_coco_cat)."""
+    return category_of if callable(category_of) else category_of.__getitem__
+
+
+def append_coco_records(bbox_data, mask_data, category_of, image_id, classes, boxes, box_scores, mask_scores, counts,
+                        h, w):
+    """prep_metrics' --output_coco_json records of one image (eval.py:420-429, Detections.add_bbox / add_mask), from host
+    arrays: classes [n], boxes int64 [n,4] pixels, box / mask scores [n] (fp32 values), counts: n RLE strings (str).
+    Rows with (y2-y1)*(x2-x1) > 0 on the int64 boxes append a bbox record to bbox_data and a mask record to mask_data,
+    in row order; the records are the reference's dicts, key for key."""
+    boxes = np.asarray(boxes, np.int64).reshape(-1, 4)
+    with np.errstate(over="ignore"):   # numpy int64 arithmetic wraps, as in eval.py
+        keep = (boxes[:, 3] - boxes[:, 1]) * (boxes[:, 2] - boxes[:, 0]) > 0
+        bbox = np.concatenate([boxes[:, :2], boxes[:, 2:] - boxes[:, :2]], 1)
+    cat = _category_fn(category_of)
+    image_id = int(image_id)
+    classes = np.asarray(classes).astype(int)
+    box_scores = np.asarray(box_scores).astype(float)
+    mask_scores = np.asarray(mask_scores).astype(float)
+    size = [int(h), int(w)]
+    for i in np.flatnonzero(keep).tolist():
+        bbox_data.append({"image_id": image_id, "category_id": cat(int(classes[i])),
+                          "bbox": [round(float(x) * 10) / 10 for x in bbox[i]], "score": float(box_scores[i])})
+        mask_data.append({"image_id": image_id, "category_id": cat(int(classes[i])),
+                          "segmentation": {"size": list(size), "counts": counts[i]}, "score": float(mask_scores[i])})
+
+
+def coco_rle_list(items, num_rows, ph, pw, k, crop_masks=True, extra=(), cap=None, device=None):
+    """yb_coco_rle_list over a yb_post_item table (ctypes array) -> (strings, host copies of `extra`, calls).
+    strings: one str per row, image by image; extra: device tensors (per-row arrays) copied back in the same D2H copy.
+    cap: the initial (runs, characters) arena capacities (an int for both); a too small arena costs exactly one more
+    call, with the sizes the first reported.  One host synchronisation, two when an arena was too small."""
+    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    B = len(items)
+    if cap is None:
+        runs_cap = sum(int(it.n) * (2 * int(it.out_w) + 8) for it in items)
+        chars_cap = 2 * runs_cap
+    elif isinstance(cap, (tuple, list)):
+        runs_cap, chars_cap = int(cap[0]), int(cap[1])
+    else:
+        runs_cap = chars_cap = int(cap)
+    extra = [t.contiguous().reshape(-1).view(torch.uint8) for t in extra]
+    lib = _lib.load()
+    calls = 0
+    while True:
+        calls += 1
+        runs = torch.empty(max(runs_cap, 1), dtype=torch.int32, device=dev)
+        chars = torch.empty(max(chars_cap, 1), dtype=torch.uint8, device=dev)
+        need = torch.empty(2, dtype=torch.int64, device=dev)
+        row_off = torch.empty(max(num_rows, 1), dtype=torch.int64, device=dev)
+        row_len = torch.empty(max(num_rows, 1), dtype=torch.int32, device=dev)
+        _lib.check(lib.yb_coco_rle_list(_ops_handle(dev, k), items, B, ph, pw, k, 1 if crop_masks else 0,
+                                        _lib.ptr(runs), runs_cap, _lib.ptr(chars), chars_cap, _lib.ptr(row_off),
+                                        _lib.ptr(row_len), _lib.ptr(need), _lib.current_stream(dev)),
+                   "yb_coco_rle_list")
+        parts = [need.view(torch.uint8), row_off[:num_rows].view(torch.uint8), row_len[:num_rows].view(torch.uint8)]
+        parts += extra + [chars[:chars_cap]]
+        host = torch.cat(parts).cpu().numpy()   # the one host synchronisation
+        need_h = host[:16].view(np.int64)
+        if need_h[0] <= runs_cap and need_h[1] <= chars_cap:
+            break
+        runs_cap, chars_cap = max(runs_cap, int(need_h[0])), max(chars_cap, int(need_h[1]))
+    pos = 16
+    off = host[pos:pos + 8 * num_rows].view(np.int64)
+    pos += 8 * num_rows
+    ln = host[pos:pos + 4 * num_rows].view(np.int32)
+    pos += 4 * num_rows
+    got = []
+    for t in extra:
+        got.append(host[pos:pos + t.numel()])
+        pos += t.numel()
+    text = host[pos:].tobytes()
+    strings = [text[o:o + n].decode("ascii") for o, n in zip(off.tolist(), ln.tolist())]
+    return strings, got, calls
+
+
+class Detections:
+    """eval.py's Detections (eval.py:300-371) for --output_coco_json: bbox_data / mask_data lists of the reference's
+    records, filled from the detections on the GPU.
+
+        dets = Detections(category_of)      # class index -> dataset category id: a sequence or a callable
+        dets.add(preds, sizes, image_ids)   # a list of images: Yolact outputs, (h, w) each, their ids
+        dets.dump(bbox_det_file, mask_det_file)
+
+    add() takes the pixel boxes, classes and scores (YOLACT++'s [box, mask] scores included) from postprocess_list
+    without assembling masks, then ONE yb_coco_rle_list launch writes every row's RLE string, and one D2H copy brings
+    the strings and the per-row arrays back."""
+
+    def __init__(self, category_of):
+        self.bbox_data = []
+        self.mask_data = []
+        self.category_of = category_of
+
+    def add(self, preds, sizes, image_ids, crop_masks=True, score_threshold=0, cap=None):
+        """prep_metrics' --output_coco_json branch (eval.py:414-429) for every image of preds (postprocess_list's
+        det_output: one {'net', 'detection'} per image), image i at sizes[i] = (h, w) with id image_ids[i].  One host
+        synchronisation (two when the string arena overflows, plus postprocess_list's one when score_threshold > 0);
+        returns the number of yb_coco_rle_list calls."""
+        from .output_utils import _postprocess_list
+        if len(image_ids) != len(preds):
+            raise ValueError("Detections.add: %d image ids for %d images" % (len(image_ids), len(preds)))
+        for d in preds:
+            if d['detection'] is not None:
+                _require_cuda(d['detection']['box'], "metrics.Detections.add")
+        from . import config as _config
+        if not getattr(_config.cfg, "eval_mask_branch", True) or any(
+                d['detection'] is not None and 'proto' not in d['detection'] for d in preds):
+            raise ValueError("Detections.add: --output_coco_json needs masks; with cfg.eval_mask_branch off (--detect) "
+                             "the detections carry no prototypes to encode")
+        out, items, shape, live, keep_alive = _postprocess_list(preds, sizes, crop_masks=crop_masks,
+                                                                score_threshold=score_threshold, mask_format=None)
+        if items is None:   # no image has detections (eval.py:410-411)
+            return 0
+        ph, pw, k = shape
+        cls = [out[i][0].long() for i in live]
+        box_s = [(out[i][1][0] if isinstance(out[i][1], list) else out[i][1]).float() for i in live]
+        mask_s = [(out[i][1][1] if isinstance(out[i][1], list) else out[i][1]).float() for i in live]
+        boxes = [out[i][2] for i in live]
+        ns = [int(b.shape[0]) for b in boxes]
+        extra = [torch.cat(t) for t in (cls, boxes, box_s, mask_s)]
+        strings, (cls_h, box_h, bs_h, ms_h), calls = coco_rle_list(items, sum(ns), ph, pw, k, crop_masks, extra, cap,
+                                                                   extra[0].device)
+        del keep_alive
+        cls_h, box_h = cls_h.view(np.int64), box_h.view(np.int64).reshape(-1, 4)
+        bs_h, ms_h = bs_h.view(np.float32), ms_h.view(np.float32)
+        r = 0
+        for i, n in zip(live, ns):
+            h, w = (int(v) for v in sizes[i])
+            append_coco_records(self.bbox_data, self.mask_data, self.category_of, image_ids[i], cls_h[r:r + n],
+                                box_h[r:r + n], bs_h[r:r + n], ms_h[r:r + n], strings[r:r + n], h, w)
+            r += n
+        return calls
+
+    def dump(self, bbox_det_file, mask_det_file):
+        """Detections.dump (eval.py:332-340): json.dump of bbox_data and mask_data, the same bytes."""
+        import json
+        for data, path in ((self.bbox_data, bbox_det_file), (self.mask_data, mask_det_file)):
+            with open(path, "w") as f:
+                json.dump(data, f)

@@ -151,6 +151,15 @@ def postprocess_list(det_output, sizes, interpolation_mode='bilinear', visualize
     list.  With score_threshold == 0 there is no host sync; with score_threshold > 0 there is one, for the kept-row
     counts of all images together.  The threshold keeps each image's leading rows (Detect's scores are descending):
     rows that are not a prefix raise ValueError rather than silently differ from postprocess."""
+    return _postprocess_list(det_output, sizes, interpolation_mode, visualize_lincomb, crop_masks, score_threshold,
+                             mask_format)[0]
+
+
+def _postprocess_list(det_output, sizes, interpolation_mode='bilinear', visualize_lincomb=False, crop_masks=True,
+                      score_threshold=0, mask_format="f32"):
+    """postprocess_list's work -> (its result, the yb_post_item table it ran with (one item per image of `live`) or
+    None, (ph, pw, k) or None, live, the tensors the table points at).  mask_format=None: no masks are assembled (masks in the result are None); the pixel
+    boxes and YOLACT++'s maskiou rescoring are as with masks, so the table can drive yb_coco_rle_list."""
     if len(sizes) != len(det_output):
         raise ValueError("postprocess_list: %d sizes for %d images" % (len(sizes), len(det_output)))
     hw = []
@@ -171,7 +180,7 @@ def postprocess_list(det_output, sizes, interpolation_mode='bilinear', visualize
         live = [i for i in live if det_output[i]['detection']['score'].size(0) > 0]
     out = [empty] * len(det_output)
     if not live:
-        return out
+        return out, None, None, live, []
 
     cfg = _config.cfg
     dets = [det_output[i]['detection'] for i in live]
@@ -197,7 +206,7 @@ def postprocess_list(det_output, sizes, interpolation_mode='bilinear', visualize
             out[i] = (d['class'], d['score'], boxes_px, d['mask'])
         _lib.check(lib.yb_postprocess_list(_ops_handle(dev, 4), items, len(dets), 1, 1, 4, 0, _lib.YB_MASK_F32, stream),
                    "yb_postprocess_list(boxes)")
-        return out
+        return out, None, None, live, keep_alive
 
     if interpolation_mode != 'bilinear':
         raise NotImplementedError("yolact_b200.postprocess implements bilinear upsampling only "
@@ -213,16 +222,17 @@ def postprocess_list(det_output, sizes, interpolation_mode='bilinear', visualize
     use_maskiou = bool(getattr(ncfg, "use_maskiou", False))
     if use_maskiou and any(det_output[i]['net'] is not net for i in live):
         raise ValueError("postprocess_list: maskiou rescoring needs every image to come from the same net")
-    fmt = _FORMATS[mask_format]
+    fmt = _FORMATS[mask_format] if mask_format is not None else _lib.YB_MASK_F32
     pm = torch.empty(sum(ns), ph, pw, dtype=torch.float32, device=dev) if use_maskiou else None
     off = 0
     for j, (i, d, n) in enumerate(zip(live, dets, ns)):
         h, w = hw[i]
         proto, coef, box = d['proto'].contiguous().float(), d['mask'].contiguous().float(), d['box'].contiguous().float()
-        masks = _empty_masks((n,), h, w, fmt, dev)
+        masks = _empty_masks((n,), h, w, fmt, dev) if mask_format is not None else None
         boxes_px = torch.empty(n, 4, dtype=torch.int64, device=dev)
         keep_alive += [proto, coef, box]
-        items[j] = _lib.YbPostItem(proto.data_ptr(), coef.data_ptr(), box.data_ptr(), masks.data_ptr() or None,
+        items[j] = _lib.YbPostItem(proto.data_ptr(), coef.data_ptr(), box.data_ptr(),
+                                   (masks.data_ptr() or None) if masks is not None else None,
                                    boxes_px.data_ptr() or None, pm[off:off + n].data_ptr() if use_maskiou else None,
                                    n, h, w)
         out[i] = (d['class'], d['score'], boxes_px, masks)
@@ -240,7 +250,7 @@ def postprocess_list(det_output, sizes, interpolation_mode='bilinear', visualize
                 r = rescored[0][off:off + n]
                 out[i] = (d['class'], r if rescored[1] else [d['score'], r]) + out[i][2:]
                 off += n
-    return out
+    return out, items, (ph, pw, k), live, keep_alive
 
 
 def _empty_masks(lead, h, w, fmt, dev):
