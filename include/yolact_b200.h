@@ -44,6 +44,8 @@
  *   yb_render_list     <- the GPU part of prep_display with undo_transform=False (eval.py:147-226): postprocess with
  *                         rescore_bbox, top-k selection, score cut, palette, mask blend and .byte(), for a list of
  *                         frames, without materialising masks
+ *   yb_render_list_ex  <- the same with device row counts (yb_infer_frames' padded outputs, no host sync), the
+ *                         --display_fps box (eval.py:211-219) and --display_masks=False
  *   yb_dcn_forward     <- dcn_v2_forward (external/DCNv2/src/dcn_v2.h:9-39,
  *                         src/cuda/dcn_v2_cuda.cu:42-172, src/cuda/dcn_v2_im2col_cuda.cu:125-195)
  *   yb_conv2d          <- nn.Conv2d + folded BatchNorm2d + activation (+ residual), op-level test hook
@@ -410,6 +412,28 @@ typedef struct {
 YB_API int yb_render_list(yb_handle* h, const yb_render_item* h_items, int B, int frame_is_u8, int ph, int pw, int k,
                           int crop_masks, int top_k, float score_threshold, int class_color, float mask_alpha,
                           const float* d_palette, int P, void* stream);
+
+/* Options of yb_render_list_ex; all zero except draw_masks = 1 is yb_render_list.
+ *   d_counts int32 [B] (nullable, device memory): frame b's row count, read on the device; each item's n is then only
+ *     the capacity (the padded rows of yb_infer_frames' outputs, which the item's pointers address) and rows at or
+ *     past d_counts[b] are never read.  No count is read on the host, so the call needs no host sync;
+ *   fps_w, fps_h (>= 0): the --display_fps box of eval.py:211-219 (cv2.getTextSize of the fps string): pixel rows
+ *     [0, min(h, fps_h + 8)) and columns [0, min(w, fps_w + 8)) are scaled by 0.6 after the mask blend and before
+ *     * 255; 0, 0 draws no box;
+ *   draw_masks: 0 is --display_masks=False: the rows are selected and the sel_* outputs written, no mask is blended. */
+typedef struct {
+  const int32_t* d_counts;
+  int32_t fps_w;
+  int32_t fps_h;
+  int32_t draw_masks;
+} yb_render_opts;
+
+/* yb_render_list with options (opts NULL: the defaults above).  YB_ERR_INVALID, with nothing written, for everything
+ * yb_render_list refuses, a negative fps_w or fps_h, or d_counts that is not device memory of the handle's device. */
+YB_API int yb_render_list_ex(yb_handle* h, const yb_render_item* h_items, int B, int frame_is_u8, int ph, int pw,
+                             int k, int crop_masks, int top_k, float score_threshold, int class_color,
+                             float mask_alpha, const float* d_palette, int P, const yb_render_opts* opts,
+                             void* stream);
 
 /* ---- op-level entry points --------------------------------------------------------------------- */
 /* Mirrors dcn_v2_forward's argument list (src/dcn_v2.h:9-23); all tensors NCHW fp32 contiguous.

@@ -8,8 +8,9 @@
 or, from the shell:   python -m integration.use_b200 /path/to/yolact --trained_model=... --benchmark
 
 For the mAP mode, `install_metrics(E)` after `import eval as E` also moves prep_metrics' matching loop and calc_map to
-the GPU (yolact_b200.metrics); `install_coco_json(E)` does the same for --output_coco_json's records.  The shell route runs eval.py as a fresh `__main__` module that cannot be patched, so it
-keeps the reference's own loop.
+the GPU (yolact_b200.metrics); `install_coco_json(E)` does the same for --output_coco_json's records, and
+`install_display(E)` routes --image, --images and --video frames' prep_display through yolact_b200.display.  The shell
+route runs eval.py as a fresh `__main__` module that cannot be patched, so it keeps the reference's own loop.
 
 `install` puts the reference on sys.path, imports its modules and rebinds the names eval.py pulls from them
 (`from yolact import Yolact`, `from layers.output_utils import postprocess`, `from utils.augmentations import
@@ -126,6 +127,73 @@ def install_coco_json(E):
     prep_metrics.__doc__ = install_coco_json.__doc__
     E.prep_metrics = prep_metrics
     return {"prep_metrics": prep_metrics}
+
+
+def install_display(E):
+    """Rebind E.prep_display (eval.py:135-262) so that --image, --images and --video frames, the calls with
+    undo_transform=False, take yolact_b200.display.render_masks: the rows are selected and the masks blended straight
+    from the detections in two launches, with the --display_fps box and --display_masks, instead of postprocess writing
+    fp32 masks for every row at frame size.  The image and the drawn rows come to the host in one copy, and the fps
+    text, rectangles and labels are drawn on it with OpenCV from the drawn rows, as eval.py:226-259 draws them.
+    undo_transform=True (evaluate --display) and --display_lincomb go to the original prep_display."""
+    import torch
+    import yolact_b200
+    from yolact_b200 import display
+    from yolact_b200.eval_utils import get_color
+
+    orig = E.prep_display
+    live_keys = ("rescore_bbox", "rescore_mask", "eval_mask_branch")   # as install()'s postprocess re-reads them
+
+    def prep_display(dets_out, img, h, w, undo_transform=True, class_color=False, mask_alpha=0.45, fps_str=''):
+        args = E.args
+        if undo_transform or args.display_lincomb:
+            return orig(dets_out, img, h, w, undo_transform=undo_transform, class_color=class_color,
+                        mask_alpha=mask_alpha, fps_str=fps_str)
+        import cv2
+        ref_cfg = getattr(E, "cfg", None)
+        for key in live_keys:
+            if hasattr(ref_cfg, key):
+                setattr(yolact_b200.cfg, key, getattr(ref_cfg, key))
+        font_face, font_scale, font_thickness = cv2.FONT_HERSHEY_DUPLEX, 0.6, 1
+        text_w = text_h = 0
+        if args.display_fps:
+            text_w, text_h = cv2.getTextSize(fps_str, font_face, font_scale, font_thickness)[0]
+        images, drawn = display.render_masks(dets_out[:1], [img], top_k=args.top_k,
+                                             score_threshold=args.score_threshold, class_color=class_color,
+                                             mask_alpha=mask_alpha, crop_masks=args.crop,
+                                             fps_box=(text_w, text_h) if args.display_fps else None,
+                                             draw_masks=args.display_masks)
+        # one copy to the host: the image and the drawn rows, enqueued together, then one wait
+        dev = images[0].device
+        host = [t.to("cpu", non_blocking=True) for t in (images[0], drawn["num"][0], drawn["classes"][0],
+                                                            drawn["scores"][0], drawn["boxes"][0])]
+        if dev.type == "cuda":
+            torch.cuda.current_stream(dev).synchronize()
+        img_numpy, num, classes, scores, boxes = (t.numpy() for t in host)
+
+        if args.display_fps:
+            cv2.putText(img_numpy, fps_str, (4, text_h + 2), font_face, font_scale, [255, 255, 255], font_thickness,
+                        cv2.LINE_AA)
+        num = int(num)
+        if num == 0 or not (args.display_text or args.display_bboxes):
+            return img_numpy
+        for j in reversed(range(num)):
+            x1, y1, x2, y2 = (int(v) for v in boxes[j])
+            color = get_color(j, classes, class_color, bgr=True)
+            if args.display_bboxes:
+                cv2.rectangle(img_numpy, (x1, y1), (x2, y2), color, 1)
+            if args.display_text:
+                _class = E.cfg.dataset.class_names[classes[j]]
+                text_str = '%s: %.2f' % (_class, scores[j]) if args.display_scores else _class
+                tw, th = cv2.getTextSize(text_str, font_face, font_scale, font_thickness)[0]
+                cv2.rectangle(img_numpy, (x1, y1), (x1 + tw, y1 - th - 4), color, -1)
+                cv2.putText(img_numpy, text_str, (x1, y1 - 3), font_face, font_scale, [255, 255, 255], font_thickness,
+                            cv2.LINE_AA)
+        return img_numpy
+
+    prep_display.__doc__ = install_display.__doc__
+    E.prep_display = prep_display
+    return {"prep_display": prep_display}
 
 
 if __name__ == "__main__":

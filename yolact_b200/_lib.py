@@ -76,6 +76,16 @@ class YbRenderItem(ctypes.Structure):
     ]
 
 
+class YbRenderOpts(ctypes.Structure):
+    """Mirror of yb_render_opts (yb_render_list_ex)."""
+    _fields_ = [
+        ("d_counts", c_void_p),
+        ("fps_w", c_int32),
+        ("fps_h", c_int32),
+        ("draw_masks", c_int32),
+    ]
+
+
 class YbConvOpts(ctypes.Structure):
     """Mirror of yb_conv_opts (yb_conv2d_ex)."""
     _fields_ = [
@@ -156,6 +166,8 @@ SIGNATURES = {
                                  c_void_p, c_void_p]),
     "yb_render_list": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_int,
                                c_float, c_void_p, c_int, c_void_p]),
+    "yb_render_list_ex": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_int,
+                                  c_float, c_void_p, c_int, POINTER(YbRenderOpts), c_void_p]),
     "yb_dcn_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 14 +
                        [c_void_p]),
     "yb_conv2d": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 12 +

@@ -531,14 +531,18 @@ int yb_coco_rle_list(yb_handle* h, const yb_post_item* h_items, int B, int ph, i
   YB_API_END
 }
 
-int yb_render_list(yb_handle* h, const yb_render_item* h_items, int B, int frame_is_u8, int ph, int pw, int k,
-                   int crop_masks, int top_k, float score_threshold, int class_color, float mask_alpha,
-                   const float* d_palette, int P, void* stream) {
+int yb_render_list_ex(yb_handle* h, const yb_render_item* h_items, int B, int frame_is_u8, int ph, int pw, int k,
+                      int crop_masks, int top_k, float score_threshold, int class_color, float mask_alpha,
+                      const float* d_palette, int P, const yb_render_opts* opts, void* stream) {
   YB_API_BEGIN
+  yb_render_opts o{nullptr, 0, 0, 1};
+  if (opts) o = *opts;
   YB_REQUIRE(h && B >= 0 && (B == 0 || h_items), "yb_render_list: bad argument");
   YB_REQUIRE(top_k >= 1, "yb_render_list: top_k must be >= 1");
   YB_REQUIRE(P >= 1 && d_palette, "yb_render_list: the palette needs at least one colour");
   YB_REQUIRE(on_handle_device(h, d_palette), "yb_render_list: the palette is not device memory of the handle's device");
+  YB_REQUIRE(o.fps_w >= 0 && o.fps_h >= 0, "yb_render_list_ex: fps_w and fps_h must be >= 0");
+  YB_REQUIRE(on_handle_device(h, o.d_counts), "yb_render_list_ex: d_counts is not device memory of the handle's device");
   auto on_device = [h](const void* p) { return on_handle_device(h, p); };
   for (int b = 0; b < B; ++b) {
     const yb_render_item& it = h_items[b];
@@ -560,8 +564,16 @@ int yb_render_list(yb_handle* h, const yb_render_item* h_items, int B, int frame
   YB_CHECK_CUDA(cudaMemcpyAsync(ws, h_items, (size_t)B * sizeof(yb_render_item), cudaMemcpyHostToDevice,
                                 (cudaStream_t)stream));
   launch_render(reinterpret_cast<const yb_render_item*>(ws), h_items, B, frame_is_u8, ph, pw, k, crop_masks, top_k,
-                score_threshold, class_color, mask_alpha, d_palette, P, ws + items_bytes, (cudaStream_t)stream, &h->lc);
+                score_threshold, class_color, mask_alpha, d_palette, P, o, ws + items_bytes, (cudaStream_t)stream,
+                &h->lc);
   YB_API_END
+}
+
+int yb_render_list(yb_handle* h, const yb_render_item* h_items, int B, int frame_is_u8, int ph, int pw, int k,
+                   int crop_masks, int top_k, float score_threshold, int class_color, float mask_alpha,
+                   const float* d_palette, int P, void* stream) {
+  return yb_render_list_ex(h, h_items, B, frame_is_u8, ph, pw, k, crop_masks, top_k, score_threshold, class_color,
+                           mask_alpha, d_palette, P, nullptr, stream);
 }
 
 int yb_maskiou(yb_handle* h, const float* d_proto_masks, int n, int ph, int pw, const int64_t* d_cls,

@@ -232,10 +232,12 @@ void launch_eval_ap(const float* rec_score, const int32_t* rec_tag, int64_t R, c
 // Device bytes of the work table launch_render needs for B images and top_k slots.
 size_t render_work_bytes(int B, int top_k);
 // Two launches for the B images of d_items (device; h_items is its host view): the selection, then the render of
-// every image's drawn masks over its frame.  work: render_work_bytes(B, top_k) bytes of device memory.
+// every image's drawn masks over its frame.  opts: device row counts (items' n is then the capacity), the fps box and
+// draw_masks, as yb_render_list_ex documents them.  work: render_work_bytes(B, top_k) bytes of device memory.
 void launch_render(const yb_render_item* d_items, const yb_render_item* h_items, int B, int frame_is_u8, int ph, int pw,
                    int k, int crop, int top_k, float score_threshold, int class_color, float alpha,
-                   const float* palette, int P, void* work, cudaStream_t stream, LaunchCounter* lc);
+                   const float* palette, int P, const yb_render_opts& opts, void* work, cudaStream_t stream,
+                   LaunchCounter* lc);
 
 // ---- eval.py's COCO results masks from the detections (cocorle.cu) --------------------------------------------------
 // One launch for the B images of d_items (device; h_items is its host view): every row's rleToString string of the mask

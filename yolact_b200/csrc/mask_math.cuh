@@ -108,9 +108,11 @@ __device__ __forceinline__ void blend_step(int j, const float* cols, float inv, 
   prod = __fmul_rn(prod, inv);
 }
 
-// (v * prod + first + rest) * 255, .byte() (truncation); v = the frame's value scaled to 0..1
-__device__ __forceinline__ uint8_t blend_out(float v, float prod, float sum) {
+// (v * prod + first + rest) * 255, .byte() (truncation); v = the frame's value scaled to 0..1.  dim: the value is first
+// scaled by the fps box's 0.6 (eval.py:219, `*= 0.6` on an fp32 tensor: torch rounds the scalar to fp32)
+__device__ __forceinline__ uint8_t blend_out(float v, float prod, float sum, bool dim = false) {
   v = __fadd_rn(__fmul_rn(v, prod), sum);
+  if (dim) v = __fmul_rn(v, 0.6f);
   v = __fmul_rn(v, 255.f);
   return (uint8_t)(int)fminf(fmaxf(v, 0.f), 255.f);
 }

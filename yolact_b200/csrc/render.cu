@@ -1,7 +1,8 @@
 // prep_display's mask overlay straight from the detections (eval.py:147-226 with display_text / display_bboxes off):
 // no [n,h,w] masks are written.
 //
-//   render_select_kernel : one CTA per image.  postprocess's score filter (det_score > score_threshold when the threshold
+//   render_select_kernel : one CTA per image, over the item's n rows or, with device row counts, its first counts[b]
+//                          (n is then the padded capacity and the rows past the count are never read).  postprocess's score filter (det_score > score_threshold when the threshold
 //                          is > 0, output_utils.py:42-50), a stable descending order of the ranking scores (ties to the
 //                          lower row), the first top_k rows and the cut at the first score < score_threshold
 //                          (eval.py:155-166).  Per drawn slot: palette colour * alpha (eval.py:169-183), crop window and
@@ -10,7 +11,8 @@
 //                          keeps the blend state of PPT pixels in registers; the CTA streams the drawn detections whose
 //                          window meets the tile through shared memory in groups, each holding the cropped sigmoid
 //                          values on the prototype rows and columns the tile interpolates from, then blends them in
-//                          drawing order.  The frame is read once and the uint8 result written once.
+//                          drawing order.  The frame is read once and the uint8 result written once.  The --display_fps
+//                          box (eval.py:211-219) scales the blended value by 0.6 before * 255 in the pixels it covers.
 //
 // Mask pixels and blend steps go through mask_math.cuh, the functions mask_assembly_kernel and display_blend_kernel use,
 // so the image equals postprocess(mask_format='u8') + display_blend on the same rows, bit for bit.
@@ -56,11 +58,12 @@ __device__ __forceinline__ bool candidate(const float* det_score, int i, float t
 }
 
 __global__ void __launch_bounds__(RT)
-render_select_kernel(const yb_render_item* __restrict__ items, int ph, int pw, int crop, int top_k, float thr,
-                     int class_color, float alpha, const float* __restrict__ palette, int P, RenderWork work) {
+render_select_kernel(const yb_render_item* __restrict__ items, const int* __restrict__ row_counts, int ph, int pw,
+                     int crop, int top_k, float thr, int class_color, float alpha, const float* __restrict__ palette,
+                     int P, int draw_masks, RenderWork work) {
   const int b = blockIdx.x;
   const yb_render_item& it = items[b];
-  const int n = it.n;
+  const int n = row_counts ? min(max(row_counts[b], 0), it.n) : it.n;
   RenderSlot* sl = work.slots + (size_t)b * top_k;
   __shared__ int s_cand, s_cut;
   if (threadIdx.x == 0) {
@@ -123,7 +126,8 @@ render_select_kernel(const yb_render_item* __restrict__ items, int ph, int pw, i
       for (int c = 0; c < 4; ++c) it.sel_box[j * 4 + c] = bx[c];
   }
   if (threadIdx.x == 0) {
-    work.counts[b] = it.proto ? m : 0;   // no prototypes (cfg.eval_mask_branch off): rows are selected, nothing drawn
+    // no prototypes (cfg.eval_mask_branch off) or --display_masks=False: rows are selected, nothing is blended
+    work.counts[b] = it.proto && draw_masks ? m : 0;
     if (it.sel_n) *it.sel_n = m;
   }
 }
@@ -137,7 +141,7 @@ __device__ __forceinline__ int src_entry(const ColTab* tab, bool contiguous, int
 template <typename T>
 __global__ void __launch_bounds__(RT)
 render_kernel(const yb_render_item* __restrict__ items, RenderWork work, int top_k, int ph, int pw, int k, float alpha,
-              int sig_cap) {
+              int sig_cap, int fps_w, int fps_h) {
   __shared__ yb_render_item it;
   __shared__ float scale_h, scale_w;
   __shared__ int s_m;
@@ -225,18 +229,22 @@ render_kernel(const yb_render_item* __restrict__ items, RenderWork work, int top
     }
   }
 
-  // out = (frame / 255 * prod + first + rest) * 255, .byte()
+  // out = (frame / 255 * prod + first + rest) [* 0.6 inside the fps box] * 255, .byte(); the box is
+  // img_gpu[0:fps_h+8, 0:fps_w+8] *= 0.6, which slicing clips to the frame; fps_w == fps_h == 0 is no box
   const int x = x0 + tx;
   if (x >= x1) return;
   const T* frame = static_cast<const T*>(it.frame);
+  const bool box_x = (fps_w > 0 || fps_h > 0) && x < fps_w + 8;
 #pragma unroll
   for (int p = 0; p < PPT; ++p) {
     const int y = y0 + ty + p * YSTEP;
     if (y >= y1) break;
+    const bool dim = box_x && y < fps_h + 8;
     const size_t o = ((size_t)y * it.w + x) * 3;
 #pragma unroll
     for (int c = 0; c < 3; ++c)
-      it.out[o + c] = blend_out(__fdiv_rn((float)frame[o + c], 255.f), prod[p], __fadd_rn(first[p][c], rest[p][c]));
+      it.out[o + c] =
+          blend_out(__fdiv_rn((float)frame[o + c], 255.f), prod[p], __fadd_rn(first[p][c], rest[p][c]), dim);
   }
 }
 
@@ -259,10 +267,13 @@ size_t render_work_bytes(int B, int top_k) {
 
 void launch_render(const yb_render_item* d_items, const yb_render_item* h_items, int B, int frame_is_u8, int ph, int pw,
                    int k, int crop, int top_k, float score_threshold, int class_color, float alpha,
-                   const float* palette, int P, void* work, cudaStream_t stream, LaunchCounter* lc) {
+                   const float* palette, int P, const yb_render_opts& opts, void* work, cudaStream_t stream,
+                   LaunchCounter* lc) {
   YB_REQUIRE(B > 0 && B <= 65535 && top_k >= 1 && P >= 1, "render: bad sizes");
+  YB_REQUIRE(opts.fps_w >= 0 && opts.fps_h >= 0, "render: negative fps box size");
   // the grid covers the tallest and widest frame; the group buffer holds at least one detection on any tile, and up to
-  // top_k detections on the tiles of the frame that interpolates from the most prototype positions per tile
+  // top_k detections on the tiles of the frame that interpolates from the most prototype positions per tile.  With
+  // device row counts an item's n is its capacity, so the buffer is sized without reading a count on the host.
   int max_h = 0, max_w = 0;
   int64_t per_det = 0;
   for (int b = 0; b < B; ++b) {
@@ -280,8 +291,8 @@ void launch_render(const yb_render_item* d_items, const yb_render_item* h_items,
   const int sig_cap = (int)std::min<int64_t>(std::max<int64_t>(MIN_SIG, per_det * top_k), 6 * MIN_SIG);
   const size_t smem = (size_t)sig_cap * sizeof(float);
   const RenderWork w = bind_work(work, B, top_k);
-  render_select_kernel<<<B, RT, 0, stream>>>(d_items, ph, pw, crop, top_k, score_threshold, class_color, alpha, palette,
-                                             P, w);
+  render_select_kernel<<<B, RT, 0, stream>>>(d_items, opts.d_counts, ph, pw, crop, top_k, score_threshold, class_color,
+                                             alpha, palette, P, opts.draw_masks ? 1 : 0, w);
   YB_CHECK_LAUNCH();
   if (lc) lc->n++;
   const dim3 grid(ceil_div(max_w, TW), ceil_div(max_h, TH), B);
@@ -289,7 +300,8 @@ void launch_render(const yb_render_item* d_items, const yb_render_item* h_items,
   do {                                                                                                         \
     if (smem + render_static_smem<T>() > 48 * 1024)                                                            \
       YB_CHECK_CUDA(cudaFuncSetAttribute(render_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    render_kernel<T><<<grid, RT, smem, stream>>>(d_items, w, top_k, ph, pw, k, alpha, sig_cap);                \
+    render_kernel<T><<<grid, RT, smem, stream>>>(d_items, w, top_k, ph, pw, k, alpha, sig_cap, opts.fps_w,      \
+                                                 opts.fps_h);                                                  \
   } while (0)
   if (frame_is_u8)
     YB_LAUNCH_RENDER(uint8_t);

@@ -406,6 +406,15 @@ class Yolact(nn.Module):
         _config.cfg._tmp_img_h, _config.cfg._tmp_img_w = oh, ow   # the network input size, as forward sets it
         return self._detection_list(out)
 
+    def render_frames(self, frames, top_k=5, score_threshold=0, class_color=False, mask_alpha=0.45, crop_masks=True,
+                      fps_box=None, draw_masks=True):
+        """prep_display's GPU part straight from uint8 frames: render_masks(self.forward_frames(frames), frames, ...)
+        bit for bit -> (images, drawn), with no host sync (yolact_b200.display.render_frames), so a video loop can keep
+        several batches in flight."""
+        from .display import render_frames
+        return render_frames(self, frames, top_k=top_k, score_threshold=score_threshold, class_color=class_color,
+                             mask_alpha=mask_alpha, crop_masks=crop_masks, fps_box=fps_box, draw_masks=draw_masks)
+
     def _infer_frames(self, frames, cross_class):
         if isinstance(frames, (list, tuple)):
             return self._infer_frame_list(frames, cross_class)
