@@ -20,6 +20,19 @@ stays the object eval.py mutates; it is snapshotted into yolact_b200.cfg each ti
 """
 import sys
 
+# cfg keys the reference's callers flip on the GLOBAL cfg between calls (prep_display sets rescore_bbox = True around
+# postprocess, eval.py:147-151; --detect clears eval_mask_branch, eval.py:1074): the package snapshot would go stale,
+# so every routed call re-reads them from the live reference cfg.
+LIVE_CFG_KEYS = ("rescore_bbox", "rescore_mask", "eval_mask_branch", "mask_proto_debug")
+
+
+def _refresh_cfg(ref_cfg):
+    """Copies LIVE_CFG_KEYS that ref_cfg (a reference cfg object) has into yolact_b200.cfg."""
+    import yolact_b200
+    for key in LIVE_CFG_KEYS:
+        if hasattr(ref_cfg, key):
+            setattr(yolact_b200.cfg, key, getattr(ref_cfg, key))
+
 
 def install(reference_root, mask_iou_on_gpu=True):
     if reference_root not in sys.path:
@@ -46,15 +59,8 @@ def install(reference_root, mask_iou_on_gpu=True):
         def __init__(self):
             super().__init__(from_reference_cfg(ref_data.cfg))
 
-    # cfg keys the reference's callers flip on the GLOBAL cfg between calls (prep_display sets rescore_bbox = True around
-    # postprocess, eval.py:147-151; --detect clears eval_mask_branch, eval.py:1074): the package snapshot would go stale,
-    # so they are re-read from the live reference cfg on every postprocess call.
-    live_keys = ("rescore_bbox", "rescore_mask", "eval_mask_branch", "mask_proto_debug")
-
     def postprocess(*args, **kwargs):
-        for key in live_keys:
-            if hasattr(ref_data.cfg, key):
-                setattr(yolact_b200.cfg, key, getattr(ref_data.cfg, key))
+        _refresh_cfg(ref_data.cfg)
         return yolact_b200.postprocess(*args, **kwargs)
     postprocess.__doc__ = yolact_b200.postprocess.__doc__
 
@@ -107,19 +113,14 @@ def install_coco_json(E):
     appended to the reference's own `detections` object (bbox_data / mask_data, categories from E.get_coco_cat), so
     evaluate()'s detections.dump() and dump_web() run unchanged.  Without the flag the call goes to the previous
     binding."""
-    import yolact_b200
     from yolact_b200 import metrics
 
     prev = E.prep_metrics
-    live_keys = ("rescore_bbox", "rescore_mask", "eval_mask_branch")   # as install()'s postprocess re-reads them
 
     def prep_metrics(ap_data, dets, img, gt, gt_masks, h, w, num_crowd, image_id, detections=None):
         if not E.args.output_coco_json:
             return prev(ap_data, dets, img, gt, gt_masks, h, w, num_crowd, image_id, detections)
-        ref_cfg = getattr(E, "cfg", None)
-        for key in live_keys:
-            if hasattr(ref_cfg, key):
-                setattr(yolact_b200.cfg, key, getattr(ref_cfg, key))
+        _refresh_cfg(getattr(E, "cfg", None))
         sink = metrics.Detections(E.get_coco_cat)
         sink.bbox_data, sink.mask_data = detections.bbox_data, detections.mask_data
         sink.add(dets[:1], [(h, w)], [image_id], crop_masks=E.args.crop, score_threshold=E.args.score_threshold)
@@ -137,12 +138,10 @@ def install_display(E):
     text, rectangles and labels are drawn on it with OpenCV from the drawn rows, as eval.py:226-259 draws them.
     undo_transform=True (evaluate --display) and --display_lincomb go to the original prep_display."""
     import torch
-    import yolact_b200
     from yolact_b200 import display
     from yolact_b200.eval_utils import get_color
 
     orig = E.prep_display
-    live_keys = ("rescore_bbox", "rescore_mask", "eval_mask_branch")   # as install()'s postprocess re-reads them
 
     def prep_display(dets_out, img, h, w, undo_transform=True, class_color=False, mask_alpha=0.45, fps_str=''):
         args = E.args
@@ -150,10 +149,7 @@ def install_display(E):
             return orig(dets_out, img, h, w, undo_transform=undo_transform, class_color=class_color,
                         mask_alpha=mask_alpha, fps_str=fps_str)
         import cv2
-        ref_cfg = getattr(E, "cfg", None)
-        for key in live_keys:
-            if hasattr(ref_cfg, key):
-                setattr(yolact_b200.cfg, key, getattr(ref_cfg, key))
+        _refresh_cfg(getattr(E, "cfg", None))
         font_face, font_scale, font_thickness = cv2.FONT_HERSHEY_DUPLEX, 0.6, 1
         text_w = text_h = 0
         if args.display_fps:

@@ -165,6 +165,35 @@ bool on_handle_device(const yb_handle* h, const void* p) {
   return found && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == h->device;
 }
 
+// A yb_post_item table's refusals, named after the entry point `where`, before anything is written or launched.
+// with_outputs: the caller writes the items' outputs, so masks must also be 16-byte aligned and masks, boxes_px and
+// proto_masks on the handle's device.
+void check_post_items(const yb_handle* h, const yb_post_item* h_items, int B, const char* where, bool with_outputs) {
+  const std::string w(where);
+  auto on_device = [h](const void* p) { return on_handle_device(h, p); };
+  for (int b = 0; b < B; ++b) {
+    const yb_post_item& it = h_items[b];
+    YB_REQUIRE(it.n >= 0 && it.out_h > 0 && it.out_w > 0, w + ": n must be >= 0 and out_h, out_w > 0");
+    YB_REQUIRE(it.n == 0 || (it.proto && it.coef && it.box), w + ": null proto, coef or box");
+    YB_REQUIRE(!with_outputs || (reinterpret_cast<uintptr_t>(it.masks) & 15) == 0, w + ": masks must be 16-byte aligned");
+    YB_REQUIRE(on_device(it.proto) && on_device(it.coef) && on_device(it.box) &&
+                   (!with_outputs || (on_device(it.masks) && on_device(it.boxes_px) && on_device(it.proto_masks))),
+               w + ": a pointer is not device memory of the handle's device");
+  }
+}
+
+// Copies a host item table of B entries to the front of buf (at least `bytes` long) on `stream` and returns it.  The
+// source is pageable, so the copy is staged before the call returns and the caller may reuse h_items at once.  The
+// caller holds a CallGuard on `stream`, so the copy is ordered after the previous call's launches, which have read the
+// table before it is overwritten.
+template <class T>
+T* stage_items(yb::DeviceBuffer& buf, size_t bytes, const T* h_items, int B, void* stream) {
+  T* table = static_cast<T*>(buf.get(bytes));
+  if (B > 0)
+    YB_CHECK_CUDA(cudaMemcpyAsync(table, h_items, (size_t)B * sizeof(T), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  return table;
+}
+
 }  // namespace
 
 extern "C" {
@@ -436,7 +465,7 @@ int yb_detect(yb_handle* h, const float* d_loc, const float* d_conf, const float
   dp.max_size = (float)h->cfg.max_size;
   dp.max_out = max_out;
   YB_REQUIRE(dp.nms_thresh > 0.f, "nms_threshold must be non negative.");  // detection.py:25-26
-  void* ws = h->get_detect_ws(detect_workspace_bytes(B, P, dp.num_classes, dp.top_k));
+  void* ws = h->detect_ws.get(detect_workspace_bytes(B, P, dp.num_classes, dp.top_k));
   DetectWorkspace dws;
   detect_workspace_bind(&dws, ws, B, P, dp.num_classes, dp.top_k);
   launch_detect(dp, d_loc, d_conf, d_coef, d_priors, dws, d_box, d_coef_out, d_cls, d_score, d_count,
@@ -476,27 +505,13 @@ int yb_postprocess_list(yb_handle* h, const yb_post_item* h_items, int B, int ph
                         int mask_format, void* stream) {
   YB_API_BEGIN
   YB_REQUIRE(h && B >= 0 && (B == 0 || h_items), "yb_postprocess_list: bad argument");
-  auto on_device = [h](const void* p) { return on_handle_device(h, p); };
-  for (int b = 0; b < B; ++b) {
-    const yb_post_item& it = h_items[b];
-    YB_REQUIRE(it.n >= 0 && it.out_h > 0 && it.out_w > 0, "yb_postprocess_list: n must be >= 0 and out_h, out_w > 0");
-    YB_REQUIRE(it.n == 0 || (it.proto && it.coef && it.box), "yb_postprocess_list: null proto, coef or box");
-    YB_REQUIRE((reinterpret_cast<uintptr_t>(it.masks) & 15) == 0, "yb_postprocess_list: masks must be 16-byte aligned");
-    YB_REQUIRE(on_device(it.proto) && on_device(it.coef) && on_device(it.box) && on_device(it.masks) &&
-                   on_device(it.boxes_px) && on_device(it.proto_masks),
-               "yb_postprocess_list: a pointer is not device memory of the handle's device");
-  }
+  check_post_items(h, h_items, B, "yb_postprocess_list", true);
   if (B == 0) return YB_OK;
   YB_REQUIRE(mask_format == YB_MASK_F32 || mask_format == YB_MASK_U8 || mask_format == YB_MASK_BITS,
              "mask_assembly: unknown mask format");
   CallGuard g(h, (cudaStream_t)stream);   // shared item table: ordered behind the previous call
-  yb_post_item* table = h->get_post_table(B);
-  // pageable source: staged before the call returns, so the caller may reuse h_items at once.  Stream-ordered after
-  // the previous call (CallGuard), so its launches have read the table before it is overwritten.
-  YB_CHECK_CUDA(cudaMemcpyAsync(table, h_items, (size_t)B * sizeof(yb_post_item), cudaMemcpyHostToDevice,
-                                (cudaStream_t)stream));
   PostSrc src{};
-  src.table = table;
+  src.table = stage_items(h->post_table, (size_t)B * sizeof(yb_post_item), h_items, B, stream);
   launch_mask_assembly(src, h_items, B, ph, pw, k, crop_masks, mask_format, (cudaStream_t)stream, &h->lc);
   YB_API_END
 }
@@ -512,20 +527,10 @@ int yb_coco_rle_list(yb_handle* h, const yb_post_item* h_items, int B, int ph, i
   YB_REQUIRE(on_device(d_runs) && on_device(d_chars) && on_device(d_row_off) && on_device(d_row_len) &&
                  on_device(d_need),
              "yb_coco_rle_list: an output is not device memory of the handle's device");
-  for (int b = 0; b < B; ++b) {
-    const yb_post_item& it = h_items[b];
-    YB_REQUIRE(it.n >= 0 && it.out_h > 0 && it.out_w > 0, "yb_coco_rle_list: n must be >= 0 and out_h, out_w > 0");
-    YB_REQUIRE(it.n == 0 || (it.proto && it.coef && it.box), "yb_coco_rle_list: null proto, coef or box");
-    YB_REQUIRE(on_device(it.proto) && on_device(it.coef) && on_device(it.box),
-               "yb_coco_rle_list: a pointer is not device memory of the handle's device");
-  }
+  check_post_items(h, h_items, B, "yb_coco_rle_list", false);
   CallGuard g(h, (cudaStream_t)stream);   // shared item table: ordered behind the previous call
-  yb_post_item* table = h->get_post_table(std::max(B, 1));
-  // pageable source: staged before the call returns, so the caller may reuse h_items at once.  Stream-ordered after
-  // the previous call (CallGuard), so its launches have read the table before it is overwritten.
-  if (B > 0)
-    YB_CHECK_CUDA(cudaMemcpyAsync(table, h_items, (size_t)B * sizeof(yb_post_item), cudaMemcpyHostToDevice,
-                                  (cudaStream_t)stream));
+  const yb_post_item* table =
+      stage_items(h->post_table, (size_t)std::max(B, 1) * sizeof(yb_post_item), h_items, B, stream);
   launch_coco_rle(table, h_items, B, ph, pw, k, crop_masks, d_runs, runs_cap, d_chars, chars_cap, d_row_off, d_row_len,
                   d_need, (cudaStream_t)stream, &h->lc);
   YB_API_END
@@ -558,14 +563,9 @@ int yb_render_list_ex(yb_handle* h, const yb_render_item* h_items, int B, int fr
   if (B == 0) return YB_OK;
   CallGuard g(h, (cudaStream_t)stream);   // shared item and work tables: ordered behind the previous call
   const size_t items_bytes = ((size_t)B * sizeof(yb_render_item) + 255) / 256 * 256;
-  char* ws = (char*)h->get_render_ws(items_bytes + render_work_bytes(B, top_k));
-  // pageable source: staged before the call returns, so the caller may reuse h_items at once.  Stream-ordered after
-  // the previous call (CallGuard), so its launches have read the tables before they are overwritten.
-  YB_CHECK_CUDA(cudaMemcpyAsync(ws, h_items, (size_t)B * sizeof(yb_render_item), cudaMemcpyHostToDevice,
-                                (cudaStream_t)stream));
-  launch_render(reinterpret_cast<const yb_render_item*>(ws), h_items, B, frame_is_u8, ph, pw, k, crop_masks, top_k,
-                score_threshold, class_color, mask_alpha, d_palette, P, o, ws + items_bytes, (cudaStream_t)stream,
-                &h->lc);
+  yb_render_item* table = stage_items(h->render_ws, items_bytes + render_work_bytes(B, top_k), h_items, B, stream);
+  launch_render(table, h_items, B, frame_is_u8, ph, pw, k, crop_masks, top_k, score_threshold, class_color, mask_alpha,
+                d_palette, P, o, reinterpret_cast<char*>(table) + items_bytes, (cudaStream_t)stream, &h->lc);
   YB_API_END
 }
 
@@ -599,7 +599,7 @@ int yb_maskiou(yb_handle* h, const float* d_proto_masks, int n, int ph, int pw, 
     }
   }
   const size_t half = (need + 255) / 256 * 256;
-  char* scratch = (char*)h->get_scratch(2 * half);
+  char* scratch = (char*)h->scratch.get(2 * half);
   const float* cur = d_proto_masks;
   for (int i = 0; i < 6; ++i) {
     ConvW& cw = h->convs[std::string("maskiou_net.maskiou_net.") + idx[i]];

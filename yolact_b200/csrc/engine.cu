@@ -861,10 +861,6 @@ using namespace yb;
 yb_handle::~yb_handle() {
   execs.clear();
   for (void* p : weight_allocs) cudaFree(p);
-  if (detect_ws) cudaFree(detect_ws);
-  if (scratch) cudaFree(scratch);
-  if (post_table) cudaFree(post_table);
-  if (render_ws) cudaFree(render_ws);
   if (cap_stream) cudaStreamDestroy(cap_stream);
   if (tune_stream) cudaStreamDestroy(tune_stream);
   for (auto s : lane_streams)
@@ -880,61 +876,19 @@ cudaStream_t yb_handle::capture_stream() {
   return cap_stream;
 }
 
-void* yb_handle::get_scratch(size_t bytes) {
-  if (bytes > scratch_bytes) {
-    if (scratch) {
+void* yb::DeviceBuffer::get(size_t bytes) {
+  if (bytes > bytes_) {
+    const size_t cap = floor_ ? std::max(bytes, std::max(floor_, 2 * bytes_)) : bytes;
+    if (ptr_) {
       YB_CHECK_CUDA(cudaDeviceSynchronize());
-      cudaFree(scratch);
-      scratch = nullptr;
+      cudaFree(ptr_);
+      ptr_ = nullptr;
+      bytes_ = 0;
     }
-    YB_CHECK_CUDA(cudaMalloc(&scratch, bytes));
-    scratch_bytes = bytes;
+    YB_CHECK_CUDA(cudaMalloc(&ptr_, cap));
+    bytes_ = cap;
   }
-  return scratch;
-}
-
-// Grows by doubling; the old table is freed only after the device has drained, since a queued launch may still read it
-yb_post_item* yb_handle::get_post_table(int entries) {
-  if (entries > post_table_cap) {
-    const int cap = std::max(entries, std::max(16, 2 * post_table_cap));
-    if (post_table) {
-      YB_CHECK_CUDA(cudaDeviceSynchronize());
-      cudaFree(post_table);
-      post_table = nullptr;
-      post_table_cap = 0;
-    }
-    YB_CHECK_CUDA(cudaMalloc(&post_table, (size_t)cap * sizeof(yb_post_item)));
-    post_table_cap = cap;
-  }
-  return post_table;
-}
-
-void* yb_handle::get_render_ws(size_t bytes) {
-  if (bytes > render_ws_bytes) {
-    const size_t cap = std::max(bytes, std::max<size_t>(64 * 1024, 2 * render_ws_bytes));
-    if (render_ws) {
-      YB_CHECK_CUDA(cudaDeviceSynchronize());
-      cudaFree(render_ws);
-      render_ws = nullptr;
-      render_ws_bytes = 0;
-    }
-    YB_CHECK_CUDA(cudaMalloc(&render_ws, cap));
-    render_ws_bytes = cap;
-  }
-  return render_ws;
-}
-
-void* yb_handle::get_detect_ws(size_t bytes) {
-  if (bytes > detect_ws_bytes) {
-    if (detect_ws) {
-      YB_CHECK_CUDA(cudaDeviceSynchronize());
-      cudaFree(detect_ws);
-      detect_ws = nullptr;
-    }
-    YB_CHECK_CUDA(cudaMalloc(&detect_ws, bytes));
-    detect_ws_bytes = bytes;
-  }
-  return detect_ws;
+  return ptr_;
 }
 
 int yb_handle::peek_cout(const std::string& conv_key) const {

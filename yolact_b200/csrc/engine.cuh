@@ -132,6 +132,25 @@ struct Executor {
   ~Executor();
 };
 
+// A grow-only device allocation of one of the handle's standalone ops.  get(bytes) grows it to exactly `bytes`, or,
+// with a doubling floor, to max(bytes, 2 * size, floor).  The old allocation is freed only after the device has
+// drained, since a queued launch may still read it.
+class DeviceBuffer {
+ public:
+  explicit DeviceBuffer(size_t doubling_floor = 0) : floor_(doubling_floor) {}
+  DeviceBuffer(const DeviceBuffer&) = delete;
+  DeviceBuffer& operator=(const DeviceBuffer&) = delete;
+  ~DeviceBuffer() {
+    if (ptr_) cudaFree(ptr_);
+  }
+  void* get(size_t bytes);
+
+ private:
+  void* ptr_ = nullptr;
+  size_t bytes_ = 0;
+  const size_t floor_;   // 0: exact growth
+};
+
 }  // namespace yb
 
 struct yb_handle {
@@ -154,14 +173,12 @@ struct yb_handle {
   cudaStream_t tune_stream = nullptr;   // private stream of the autotuner when PDL candidates are timed
   yb::Executor* last_exec = nullptr;
   // standalone op workspaces
-  void* detect_ws = nullptr;
-  size_t detect_ws_bytes = 0;
-  void* scratch = nullptr;   // maskiou / dcn / conv2d temporaries
-  size_t scratch_bytes = 0;
-  yb_post_item* post_table = nullptr;   // yb_postprocess_list's device item table
-  int post_table_cap = 0;
-  void* render_ws = nullptr;            // yb_render_list's device item table and work table
-  size_t render_ws_bytes = 0;
+  yb::DeviceBuffer detect_ws;
+  yb::DeviceBuffer scratch;   // maskiou temporaries
+  yb::DeviceBuffer post_table{16 * sizeof(yb_post_item)};   // yb_postprocess_list's and yb_coco_rle_list's item table
+  // yb_render_list's device item table and, after it, the work table that carries the selection from the call's first
+  // launch to its second
+  yb::DeviceBuffer render_ws{64 * 1024};
   cudaStream_t cap_stream = nullptr;  // private stream used only for CUDA-graph capture
   cudaStream_t lane_streams[8] = {};  // branch streams joined into the capture (parallel graph branches)
   cudaEvent_t ev_fork = nullptr, ev_join[8] = {};
@@ -194,10 +211,6 @@ struct yb_handle {
   void infer_on(yb::Executor* ex, yb::Executor::FrameInput* fin, const void* d_x, int cross_class, int max_out,
                 float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto,
                 cudaStream_t stream);
-  void* get_scratch(size_t bytes);
-  void* get_detect_ws(size_t bytes);
-  yb_post_item* get_post_table(int entries);
-  void* get_render_ws(size_t bytes);
 };
 
 namespace yb {

@@ -29,7 +29,7 @@ import torch
 
 from . import _lib
 from . import config as _config
-from .output_utils import _maskiou_rescore, _ops_handle
+from .output_utils import _gather, _ops_handle, _post_list, _rescore_list
 
 _palettes = {}
 
@@ -121,56 +121,20 @@ def render_masks(det_output, frames, top_k=5, score_threshold=0, class_color=Fal
     if B == 0:
         return [], drawn
 
-    cfg = _config.cfg
-    live = [i for i, d in enumerate(det_output) if d['detection'] is not None]
-    dets = {i: det_output[i]['detection'] for i in live}
-    for d in dets.values():
-        if not d['box'].is_cuda:
-            raise _lib.YbError("yolact_b200.render_masks runs on CUDA (H100) only; there is no CPU path.")
-    with_proto = ['proto' in d for d in dets.values()]
-    if any(with_proto) and not all(with_proto):
-        raise ValueError("render_masks: some detections carry 'proto' and some do not")
-    eval_mask_branch = bool(live) and getattr(cfg, "eval_mask_branch", True) and with_proto[0]
-    keep_alive = []   # the contiguous inputs, held until the calls have enqueued their reads of them
-    ph = pw = 1
-    k = 4
-    rank = {i: dets[i]['score'] for i in live}
-    if eval_mask_branch:
-        shapes = {tuple(int(s) for s in d['proto'].shape) for d in dets.values()}
-        if len(shapes) != 1:
-            raise ValueError("render_masks: the images' prototypes differ in (ph, pw, k): %s" % sorted(shapes))
-        ph, pw, k = shapes.pop()
-        net = det_output[live[0]]['net']
-        ncfg = getattr(net, "cfg", cfg)
-        if bool(getattr(ncfg, "use_maskiou", False)):
-            # YOLACT++ (output_utils.py:77-88 with rescore_bbox, eval.py:148-149): maskiou_net on the prototype-resolution
-            # masks of every row of every image at once; the rows are independent, so the score filter can follow
-            if any(det_output[i]['net'] is not net for i in live):
-                raise ValueError("render_masks: maskiou rescoring needs every image to come from the same net")
-            ns = [int(dets[i]['box'].shape[0]) for i in live]
-            pm = torch.empty(sum(ns), ph, pw, dtype=torch.float32, device=dev)
-            post = (_lib.YbPostItem * len(live))()
-            off = 0
-            for j, (i, n) in enumerate(zip(live, ns)):
-                d = dets[i]
-                proto, coef, box = d['proto'].contiguous().float(), d['mask'].contiguous().float(), d['box'].contiguous().float()
-                keep_alive += [proto, coef, box]
-                post[j] = _lib.YbPostItem(proto.data_ptr(), coef.data_ptr(), box.data_ptr(), None, None,
-                                           pm[off:off + n].data_ptr() if n else None, n, int(frames[i].shape[0]),
-                                           int(frames[i].shape[1]))
-                off += n
-            lib = _lib.load()
-            _lib.check(lib.yb_postprocess_list(_ops_handle(dev, k), post, len(live), ph, pw, k, 1 if crop_masks else 0,
-                                               _lib.YB_MASK_F32, _lib.current_stream(dev)), "yb_postprocess_list(proto)")
-            if off > 0:
-                cat = (lambda ts: torch.cat(ts)) if len(live) > 1 else (lambda ts: ts[0])
-                rescored = _maskiou_rescore(net, ncfg, pm, cat([dets[i]['class'] for i in live]),
-                                            cat([dets[i]['score'] for i in live]))
-                if rescored is not None:
-                    off = 0
-                    for i, n in zip(live, ns):
-                        rank[i] = rescored[0][off:off + n]
-                        off += n
+    g = _gather(det_output, "render_masks")
+    dets = dict(zip(g.live, g.dets))
+    keep_alive = []   # the contiguous inputs, held until the call has enqueued its reads of them
+    ph, pw, k = g.shape if g.eval_mask_branch else (1, 1, 4)
+    rank = {i: d['score'] for i, d in dets.items()}
+    if g.use_maskiou:
+        # YOLACT++ (output_utils.py:77-88 with rescore_bbox, eval.py:148-149): maskiou_net on the prototype-resolution
+        # masks of every row of every image at once; the rows are independent, so the score filter can follow
+        pm = torch.empty(sum(g.ns), ph, pw, dtype=torch.float32, device=dev)
+        _post_list(dev, [(d['proto'], d['mask'], d['box'], int(frames[i].shape[0]), int(frames[i].shape[1]))
+                         for i, d in dets.items()], ph, pw, k, crop_masks, pm=pm)
+        rescored = _rescore_list(g.net, g.ncfg, pm, [d['class'] for d in g.dets], [d['score'] for d in g.dets], g.ns)
+        if rescored is not None:
+            rank.update(zip(g.live, rescored[0]))
 
     for i in range(B):
         it = items[i]
@@ -183,7 +147,7 @@ def render_masks(det_output, frames, top_k=5, score_threshold=0, class_color=Fal
             score = rank[i].contiguous().float()
             keep_alive += [box, cls, det_score, score]
             it.box, it.cls, it.det_score, it.score = box.data_ptr(), cls.data_ptr(), det_score.data_ptr(), score.data_ptr()
-            if eval_mask_branch:
+            if g.eval_mask_branch:
                 proto, coef = d['proto'].contiguous().float(), d['mask'].contiguous().float()
                 keep_alive += [proto, coef]
                 it.proto, it.coef = proto.data_ptr(), coef.data_ptr()
@@ -220,7 +184,6 @@ def render_frames(net, frames, top_k=5, score_threshold=0, class_color=False, ma
     if not eval_mask_branch:
         k = 4
     rank = score
-    keep_alive = []
     ncfg = net.cfg
     if eval_mask_branch and bool(getattr(ncfg, "use_maskiou", False)) and M > 0:
         # YOLACT++: maskiou_net over all B*M padded rows at once (rows are independent and maskiou_net is bit-identical
@@ -233,18 +196,11 @@ def render_frames(net, frames, top_k=5, score_threshold=0, class_color=False, ma
         zcoef = torch.where(valid[..., None], coef, 0.0)
         zcls = torch.where(valid, cls, 0)
         pm = torch.empty(B * M, ph, pw, dtype=torch.float32, device=dev)
-        post = (_lib.YbPostItem * B)()
-        for b in range(B):
-            post[b] = _lib.YbPostItem(proto[b].data_ptr(), zcoef[b].data_ptr(), zbox[b].data_ptr(), None, None,
-                                      pm[b * M:(b + 1) * M].data_ptr(), M, int(flist[b].shape[0]),
-                                      int(flist[b].shape[1]))
-        lib = _lib.load()
-        _lib.check(lib.yb_postprocess_list(_ops_handle(dev, k), post, B, ph, pw, k, 1 if crop_masks else 0,
-                                           _lib.YB_MASK_F32, _lib.current_stream(dev)), "yb_postprocess_list(proto)")
-        rescored = _maskiou_rescore(net, ncfg, pm, zcls.reshape(-1), score.reshape(-1))
+        _post_list(dev, [(proto[b], zcoef[b], zbox[b], int(flist[b].shape[0]), int(flist[b].shape[1]))
+                         for b in range(B)], ph, pw, k, crop_masks, pm=pm)
+        rescored = _rescore_list(net, ncfg, pm, [zcls.reshape(-1)], [score.reshape(-1)], [B * M])
         if rescored is not None:
-            rank = rescored[0].reshape(B, M)
-        keep_alive += [zbox, zcoef, zcls, pm]
+            rank = rescored[0][0].reshape(B, M)
     for b in range(B):
         it = items[b]
         it.box, it.cls, it.det_score, it.score = (box[b].data_ptr(), cls[b].data_ptr(), score[b].data_ptr(),

@@ -368,24 +368,24 @@ class Detections:
                 d['detection'] is not None and 'proto' not in d['detection'] for d in preds):
             raise ValueError("Detections.add: --output_coco_json needs masks; with cfg.eval_mask_branch off (--detect) "
                              "the detections carry no prototypes to encode")
-        out, items, shape, live, keep_alive = _postprocess_list(preds, sizes, crop_masks=crop_masks,
-                                                                score_threshold=score_threshold, mask_format=None)
-        if items is None:   # no image has detections (eval.py:410-411)
+        res = _postprocess_list(preds, sizes, crop_masks=crop_masks, score_threshold=score_threshold, mask_format=None)
+        if not res.live:   # no image has detections (eval.py:410-411)
             return 0
-        ph, pw, k = shape
-        cls = [out[i][0].long() for i in live]
-        box_s = [(out[i][1][0] if isinstance(out[i][1], list) else out[i][1]).float() for i in live]
-        mask_s = [(out[i][1][1] if isinstance(out[i][1], list) else out[i][1]).float() for i in live]
-        boxes = [out[i][2] for i in live]
+        ph, pw, k = res.shape
+        out = [res.out[i] for i in res.live]
+        cls = [o[0].long() for o in out]
+        box_s = [(o[1][0] if isinstance(o[1], list) else o[1]).float() for o in out]
+        mask_s = [(o[1][1] if isinstance(o[1], list) else o[1]).float() for o in out]
+        boxes = [o[2] for o in out]
         ns = [int(b.shape[0]) for b in boxes]
         extra = [torch.cat(t) for t in (cls, boxes, box_s, mask_s)]
-        strings, (cls_h, box_h, bs_h, ms_h), calls = coco_rle_list(items, sum(ns), ph, pw, k, crop_masks, extra, cap,
-                                                                   extra[0].device)
-        del keep_alive
+        # res.keep_alive holds the inputs res.items points at until this call has read them
+        strings, (cls_h, box_h, bs_h, ms_h), calls = coco_rle_list(res.items, sum(ns), ph, pw, k, crop_masks, extra,
+                                                                   cap, extra[0].device)
         cls_h, box_h = cls_h.view(np.int64), box_h.view(np.int64).reshape(-1, 4)
         bs_h, ms_h = bs_h.view(np.float32), ms_h.view(np.float32)
         r = 0
-        for i, n in zip(live, ns):
+        for i, n in zip(res.live, ns):
             h, w = (int(v) for v in sizes[i])
             append_coco_records(self.bbox_data, self.mask_data, self.category_of, image_ids[i], cls_h[r:r + n],
                                 box_h[r:r + n], bs_h[r:r + n], ms_h[r:r + n], strings[r:r + n], h, w)

@@ -18,6 +18,7 @@ uint32 words, 1 bit per pixel, row pitch ceil(w/32) -- 32x less HBM/PCIe traffic
 postprocess_list(det_output, sizes, ...) is postprocess for every image of a list at its own size (a folder of images
 through Yolact.forward_frames), in one call with one launch per kernel for the whole list.
 """
+import collections
 import ctypes
 
 import torch
@@ -119,11 +120,7 @@ def postprocess(det_output, w, h, batch_idx=0, interpolation_mode='bilinear', vi
     eval_mask_branch = getattr(cfg, "eval_mask_branch", True) and 'proto' in dets
 
     if eval_mask_branch:
-        if interpolation_mode != 'bilinear':
-            raise NotImplementedError("yolact_b200.postprocess implements bilinear upsampling only "
-                                      "(the only mode eval.py uses)")
-        if visualize_lincomb:
-            raise NotImplementedError("display_lincomb (debug visualisation) is out of scope")
+        _refuse_unsupported(interpolation_mode, visualize_lincomb)
         use_maskiou = bool(getattr(ncfg, "use_maskiou", False))
         out_masks, boxes_px, pm = assemble_masks(dets['proto'], masks, boxes, h, w, crop_masks, mask_format,
                                                  want_proto_masks=use_maskiou)
@@ -152,14 +149,20 @@ def postprocess_list(det_output, sizes, interpolation_mode='bilinear', visualize
     counts of all images together.  The threshold keeps each image's leading rows (Detect's scores are descending):
     rows that are not a prefix raise ValueError rather than silently differ from postprocess."""
     return _postprocess_list(det_output, sizes, interpolation_mode, visualize_lincomb, crop_masks, score_threshold,
-                             mask_format)[0]
+                             mask_format).out
+
+
+# _postprocess_list's result: out, postprocess_list's result; items, the yb_post_item table it ran with (one item per
+# image of live) or None; shape, (ph, pw, k) or None without masks; live, the indices of the images with detections;
+# keep_alive, the tensors the table points at.
+_ListResult = collections.namedtuple("_ListResult", "out items shape live keep_alive")
 
 
 def _postprocess_list(det_output, sizes, interpolation_mode='bilinear', visualize_lincomb=False, crop_masks=True,
                       score_threshold=0, mask_format="f32"):
-    """postprocess_list's work -> (its result, the yb_post_item table it ran with (one item per image of `live`) or
-    None, (ph, pw, k) or None, live, the tensors the table points at).  mask_format=None: no masks are assembled (masks in the result are None); the pixel
-    boxes and YOLACT++'s maskiou rescoring are as with masks, so the table can drive yb_coco_rle_list."""
+    """postprocess_list's work -> _ListResult.  mask_format=None: no masks are assembled (masks in the result are
+    None); the pixel boxes and YOLACT++'s maskiou rescoring are as with masks, so the table can drive
+    yb_coco_rle_list."""
     if len(sizes) != len(det_output):
         raise ValueError("postprocess_list: %d sizes for %d images" % (len(sizes), len(det_output)))
     hw = []
@@ -168,89 +171,123 @@ def _postprocess_list(det_output, sizes, interpolation_mode='bilinear', visualiz
         if h <= 0 or w <= 0:
             raise ValueError("postprocess_list: image sizes must be positive, got %s" % (tuple(s),))
         hw.append((h, w))
-    empty = [torch.Tensor()] * 4   # output_utils.py:39-40,49-50
+    g = _gather(det_output, "postprocess_list", score_threshold)
+    out = [[torch.Tensor()] * 4] * len(det_output)   # output_utils.py:39-40,49-50
+    if not g.live:
+        return _ListResult(out, None, None, g.live, [])
+    boxes_px = [torch.empty(n, 4, dtype=torch.int64, device=g.dev) for n in g.ns]
+
+    if not g.eval_mask_branch:
+        # cfg.eval_mask_branch == False (--detect): boxes only, masks are the raw coefficients (Appendix D.15)
+        dummy = torch.empty(4, dtype=torch.float32, device=g.dev)   # never read without masks
+        items, keep_alive = _post_list(g.dev, [(dummy, dummy, d['box']) + hw[i] for i, d in zip(g.live, g.dets)],
+                                       1, 1, 4, crop_masks=False, boxes_px=boxes_px)
+        for i, d, px in zip(g.live, g.dets, boxes_px):
+            out[i] = (d['class'], d['score'], px, d['mask'])
+        return _ListResult(out, items, None, g.live, keep_alive)
+
+    _refuse_unsupported(interpolation_mode, visualize_lincomb)
+    ph, pw, k = g.shape
+    fmt = _FORMATS[mask_format] if mask_format is not None else _lib.YB_MASK_F32
+    masks = [_empty_masks((n,), *hw[i], fmt, g.dev) if mask_format is not None else None for i, n in zip(g.live, g.ns)]
+    pm = torch.empty(sum(g.ns), ph, pw, dtype=torch.float32, device=g.dev) if g.use_maskiou else None
+    items, keep_alive = _post_list(g.dev, [(d['proto'], d['mask'], d['box']) + hw[i] for i, d in zip(g.live, g.dets)],
+                                   ph, pw, k, crop_masks, fmt, masks, boxes_px, pm)
+    scores = [d['score'] for d in g.dets]
+    rescored = _rescore_list(g.net, g.ncfg, pm, [d['class'] for d in g.dets], scores, g.ns) if g.use_maskiou else None
+    if rescored is not None:
+        r, rescore_bbox = rescored
+        scores = r if rescore_bbox else [[s, x] for s, x in zip(scores, r)]
+    for i, d, s, px, m in zip(g.live, g.dets, scores, boxes_px, masks):
+        out[i] = (d['class'], s, px, m)
+    return _ListResult(out, items, g.shape, g.live, keep_alive)
+
+
+_Gathered = collections.namedtuple("_Gathered", "live dets dev eval_mask_branch shape net ncfg use_maskiou ns")
+
+
+def _gather(det_output, where, score_threshold=0):
+    """What one list call over det_output (Yolact's output list) needs -> _Gathered: live, the indices of the images
+    with detections, and dets, their detection dicts; dev, their device (None without live images); eval_mask_branch,
+    whether masks are evaluated (cfg.eval_mask_branch and 'proto' present), and with masks shape (ph, pw, k), the net,
+    its cfg ncfg and use_maskiou; ns, the images' row counts.  score_threshold > 0 first keeps each image's leading
+    rows above it (one host sync) and drops the images left empty.  Refuses CPU tensors with YbError, and with
+    ValueError a list where only some images carry 'proto', prototypes that differ in (ph, pw, k), and maskiou
+    rescoring over images of more than one net.  `where` names the caller in the messages."""
     live = [i for i, d in enumerate(det_output) if d['detection'] is not None]
     for i in live:
         if not det_output[i]['detection']['box'].is_cuda:
-            raise _lib.YbError("yolact_b200.postprocess runs on CUDA (H100) only; there is no CPU path.")
+            raise _lib.YbError("yolact_b200.%s runs on CUDA (H100) only; there is no CPU path." % where)
     dev = det_output[live[0]]['detection']['box'].device if live else None
-
     if score_threshold > 0 and live:
         _keep_leading_rows(det_output, live, score_threshold, dev)
         live = [i for i in live if det_output[i]['detection']['score'].size(0) > 0]
-    out = [empty] * len(det_output)
-    if not live:
-        return out, None, None, live, []
-
-    cfg = _config.cfg
     dets = [det_output[i]['detection'] for i in live]
     with_proto = ['proto' in d for d in dets]
     if any(with_proto) and not all(with_proto):
-        raise ValueError("postprocess_list: some detections carry 'proto' and some do not")
-    eval_mask_branch = getattr(cfg, "eval_mask_branch", True) and with_proto[0]
-    lib = _lib.load()
-    stream = _lib.current_stream(dev)
+        raise ValueError("%s: some detections carry 'proto' and some do not" % where)
+    eval_mask_branch = bool(live) and getattr(_config.cfg, "eval_mask_branch", True) and with_proto[0]
+    shape, net, ncfg, use_maskiou = None, None, None, False
+    if eval_mask_branch:
+        shapes = {tuple(int(s) for s in d['proto'].shape) for d in dets}
+        if len(shapes) != 1:
+            raise ValueError("%s: the images' prototypes differ in (ph, pw, k): %s" % (where, sorted(shapes)))
+        shape = shapes.pop()
+        net = det_output[live[0]]['net']
+        ncfg = getattr(net, "cfg", _config.cfg)
+        use_maskiou = bool(getattr(ncfg, "use_maskiou", False))
+        if use_maskiou and any(det_output[i]['net'] is not net for i in live):
+            raise ValueError("%s: maskiou rescoring needs every image to come from the same net" % where)
     ns = [int(d['box'].shape[0]) for d in dets]
-    keep_alive = []   # the contiguous inputs, held until the call has enqueued its reads of them
-    items = (_lib.YbPostItem * len(dets))()
+    return _Gathered(live, dets, dev, eval_mask_branch, shape, net, ncfg, use_maskiou, ns)
 
-    if not eval_mask_branch:
-        # cfg.eval_mask_branch == False (--detect): boxes only, masks are the raw coefficients (Appendix D.15)
-        dummy = torch.empty(4, dtype=torch.float32, device=dev)   # never read without masks
-        for j, (i, d, n) in enumerate(zip(live, dets, ns)):
-            box = d['box'].contiguous().float()
-            boxes_px = torch.empty(n, 4, dtype=torch.int64, device=dev)
-            keep_alive.append(box)
-            items[j] = _lib.YbPostItem(dummy.data_ptr(), dummy.data_ptr(), box.data_ptr(), None, boxes_px.data_ptr(),
-                                       None, n, hw[i][0], hw[i][1])
-            out[i] = (d['class'], d['score'], boxes_px, d['mask'])
-        _lib.check(lib.yb_postprocess_list(_ops_handle(dev, 4), items, len(dets), 1, 1, 4, 0, _lib.YB_MASK_F32, stream),
-                   "yb_postprocess_list(boxes)")
-        return out, None, None, live, keep_alive
 
+def _post_list(dev, entries, ph, pw, k, crop_masks=True, fmt=_lib.YB_MASK_F32, masks=None, boxes_px=None, pm=None):
+    """One yb_postprocess_list call on dev over entries [(proto, coef, box, h, w)], one per image, each image's rows
+    n = box.shape[0].  Image j writes masks[j] and boxes_px[j] when those lists are given (an entry may be None), and
+    its rows of pm, a [sum n, ph, pw] buffer, when pm is given.  -> (the yb_post_item table, the contiguous inputs it
+    points at: hold them for as long as the table is used)."""
+    def addr(t):
+        return (t.data_ptr() or None) if t is not None else None
+    items = (_lib.YbPostItem * len(entries))()
+    keep_alive = []
+    off = 0
+    for j, (proto, coef, box, h, w) in enumerate(entries):
+        proto, coef, box = proto.contiguous().float(), coef.contiguous().float(), box.contiguous().float()
+        n = int(box.shape[0])
+        keep_alive += [proto, coef, box]
+        items[j] = _lib.YbPostItem(proto.data_ptr(), coef.data_ptr(), box.data_ptr(),
+                                   addr(masks[j]) if masks is not None else None,
+                                   addr(boxes_px[j]) if boxes_px is not None else None,
+                                   addr(pm[off:off + n]) if pm is not None and n else None, n, h, w)
+        off += n
+    _lib.check(_lib.load().yb_postprocess_list(_ops_handle(dev, k), items, len(entries), ph, pw, k,
+                                               1 if crop_masks else 0, fmt, _lib.current_stream(dev)),
+               "yb_postprocess_list")
+    return items, keep_alive
+
+
+def _rescore_list(net, ncfg, pm, classes, scores, ns):
+    """YOLACT++'s rescoring (output_utils.py:79-88) of a list's rows: maskiou_net and the gather are per row, so one
+    _maskiou_rescore covers every image.  pm [sum ns, ph, pw]: the rows' prototype-resolution masks; classes, scores:
+    the rows' tensors, one per image (or one of all rows, with ns = [their count]).  -> (the rescored scores, one
+    tensor per image, and rescore_bbox), or None without rows or without cfg.rescore_mask."""
+    if sum(ns) == 0:
+        return None
+    cat = (lambda ts: torch.cat(ts)) if len(ns) > 1 else (lambda ts: ts[0])
+    rescored = _maskiou_rescore(net, ncfg, pm, cat(classes), cat(scores))
+    if rescored is None:
+        return None
+    return rescored[0].split(ns), rescored[1]
+
+
+def _refuse_unsupported(interpolation_mode, visualize_lincomb):
+    """postprocess' refusal of the modes eval.py never uses with masks."""
     if interpolation_mode != 'bilinear':
         raise NotImplementedError("yolact_b200.postprocess implements bilinear upsampling only "
                                   "(the only mode eval.py uses)")
     if visualize_lincomb:
         raise NotImplementedError("display_lincomb (debug visualisation) is out of scope")
-    shapes = {tuple(int(s) for s in d['proto'].shape) for d in dets}
-    if len(shapes) != 1:
-        raise ValueError("postprocess_list: the images' prototypes differ in (ph, pw, k): %s" % sorted(shapes))
-    ph, pw, k = shapes.pop()
-    net = det_output[live[0]]['net']
-    ncfg = getattr(net, "cfg", cfg)
-    use_maskiou = bool(getattr(ncfg, "use_maskiou", False))
-    if use_maskiou and any(det_output[i]['net'] is not net for i in live):
-        raise ValueError("postprocess_list: maskiou rescoring needs every image to come from the same net")
-    fmt = _FORMATS[mask_format] if mask_format is not None else _lib.YB_MASK_F32
-    pm = torch.empty(sum(ns), ph, pw, dtype=torch.float32, device=dev) if use_maskiou else None
-    off = 0
-    for j, (i, d, n) in enumerate(zip(live, dets, ns)):
-        h, w = hw[i]
-        proto, coef, box = d['proto'].contiguous().float(), d['mask'].contiguous().float(), d['box'].contiguous().float()
-        masks = _empty_masks((n,), h, w, fmt, dev) if mask_format is not None else None
-        boxes_px = torch.empty(n, 4, dtype=torch.int64, device=dev)
-        keep_alive += [proto, coef, box]
-        items[j] = _lib.YbPostItem(proto.data_ptr(), coef.data_ptr(), box.data_ptr(),
-                                   (masks.data_ptr() or None) if masks is not None else None,
-                                   boxes_px.data_ptr() or None, pm[off:off + n].data_ptr() if use_maskiou else None,
-                                   n, h, w)
-        out[i] = (d['class'], d['score'], boxes_px, masks)
-        off += n
-    _lib.check(lib.yb_postprocess_list(_ops_handle(dev, k), items, len(dets), ph, pw, k, 1 if crop_masks else 0, fmt,
-                                       stream), "yb_postprocess_list")
-
-    if use_maskiou and off > 0:
-        # maskiou_net and the gather are per row: one call over the rows of every image at once
-        cat = (lambda ts: torch.cat(ts)) if len(dets) > 1 else (lambda ts: ts[0])
-        rescored = _maskiou_rescore(net, ncfg, pm, cat([d['class'] for d in dets]), cat([d['score'] for d in dets]))
-        if rescored is not None:
-            off = 0
-            for i, d, n in zip(live, dets, ns):
-                r = rescored[0][off:off + n]
-                out[i] = (d['class'], r if rescored[1] else [d['score'], r]) + out[i][2:]
-                off += n
-    return out, items, (ph, pw, k), live, keep_alive
 
 
 def _empty_masks(lead, h, w, fmt, dev):
