@@ -349,6 +349,77 @@ YB_API int yb_eval_match(yb_handle* h, const float* d_box_iou, const float* d_ma
                          int num_crowd, const double* h_thresholds, int T, int C, float* d_rec_score,
                          int32_t* d_rec_tag, int64_t* d_counts, int32_t* d_err, void* stream);
 
+/* One image of a yb_eval_iou_list call (all pointers device memory):
+ *   proto [ph,pw,k], coef [n,k], box [n,4] relative, n, out_h, out_w: as yb_post_item's;
+ *   boxes_px int64 [n,4]: the pixel boxes yb_postprocess writes for these rows;
+ *   gt_bits [g_all, out_h, ceil(out_w/32)] uint32: the ground-truth masks in YB_MASK_BITS rows (padding bits zero);
+ *   gt_boxes fp32 [g_all,4]: the ground-truth boxes in pixels; the crowds are the last num_crowd of the g_all rows;
+ *   box_iou, mask_iou fp32 [n, g] and crowd_box_iou, crowd_mask_iou fp32 [n, num_crowd], g = g_all - num_crowd: the
+ *   outputs (each may be NULL when its side is empty). */
+typedef struct {
+  const float* proto;
+  const float* coef;
+  const float* box;
+  const int64_t* boxes_px;
+  const uint32_t* gt_bits;
+  const float* gt_boxes;
+  float* box_iou;
+  float* mask_iou;
+  float* crowd_box_iou;
+  float* crowd_mask_iou;
+  int32_t n;
+  int32_t out_h;
+  int32_t out_w;
+  int32_t g_all;
+  int32_t num_crowd;
+} yb_eval_iou_item;
+
+/* prep_metrics' four IoU caches (eval.py:431-445) for a list of B images in ONE launch, straight from the detections:
+ * per image, box_iou = jaccard(boxes_px, gt_boxes[:g]), mask_iou = mask_iou(masks, gt[:g]), crowd_box_iou and
+ * crowd_mask_iou the same against the crowds with iscrowd, where masks are the YB_MASK_BITS masks yb_postprocess would
+ * write for the rows at out_h x out_w with crop_masks (bilinear, > 0.5).  The masks are never written: every cache is
+ * yb_box_iou / yb_mask_iou's on yb_postprocess's outputs, bit for bit (0 / 0 = NaN).  Reads the items' proto, coef,
+ * box, boxes_px, gt_bits and gt_boxes; writes the four caches and nothing else.  The item table is uploaded into a table
+ * the handle owns (stream-ordered behind the handle's previous call); h_items may be reused as soon as the call
+ * returns.  No host sync.  B == 0, n == 0 and g_all == 0 are allowed.  YB_ERR_INVALID, with nothing written, for
+ * B < 0 or B > 65535, n < 0 or n > 1024, out_h or out_w <= 0, more than 2^28 pixels, num_crowd outside [0, g_all],
+ * g or num_crowd > 1024, k not a multiple of 4 or > 128, ph or pw <= 0, a null input or output a non-empty side needs,
+ * or a pointer that is not device memory of the handle's device. */
+YB_API int yb_eval_iou_list(yb_handle* h, const yb_eval_iou_item* h_items, int B, int ph, int pw, int k,
+                            int crop_masks, void* stream);
+
+/* One image of a yb_eval_match_list call (all pointers device memory): the arguments of yb_eval_match for that image
+ * (caches, classes, scores, ground-truth and crowd classes, n, g, num_crowd) and rec_offset, the index of the image's
+ * first record in the call's d_rec_score / d_rec_tag. */
+typedef struct {
+  const float* box_iou;
+  const float* mask_iou;
+  const float* crowd_box_iou;
+  const float* crowd_mask_iou;
+  const int64_t* cls;
+  const float* box_score;
+  const float* mask_score;
+  const int32_t* gt_cls;
+  const int32_t* crowd_cls;
+  int64_t rec_offset;
+  int32_t n;
+  int32_t g;
+  int32_t num_crowd;
+} yb_eval_match_item;
+
+/* yb_eval_match for a list of B images in ONE launch (one CTA per image): image b's 2*T*n records go to
+ * d_rec_score / d_rec_tag + rec_offset, exactly as yb_eval_match would write them at that address, and its non-crowd
+ * ground-truth counts are added to d_counts int64 [C]; a class outside [0, C) sets d_err as in yb_eval_match.  An image
+ * with n == 0 writes nothing and counts nothing (eval.py:405-406).  Reads the items' caches, classes, scores and
+ * ground-truth classes; writes only those records, d_counts and d_err.  The item table is uploaded into a table the
+ * handle owns (stream-ordered behind the handle's previous call); h_items and h_thresholds may be reused as soon as the
+ * call returns.  No host sync.  YB_ERR_INVALID, with nothing written, for B < 0, any image beyond n, g, num_crowd <=
+ * 1024, T outside [1, 32], C outside [1, 2048], a negative rec_offset, a null argument an image with n > 0 needs, or a
+ * pointer that is not device memory of the handle's device. */
+YB_API int yb_eval_match_list(yb_handle* h, const yb_eval_match_item* h_items, int B, const double* h_thresholds, int T,
+                              int C, float* d_rec_score, int32_t* d_rec_tag, int64_t* d_counts, int32_t* d_err,
+                              void* stream);
+
 /* Device bytes of the workspace yb_eval_ap needs for num_records records, T thresholds and C classes. */
 YB_API int yb_eval_ap_workspace(int64_t num_records, int T, int C, int64_t* bytes);
 

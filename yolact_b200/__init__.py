@@ -3,7 +3,7 @@ Yolact.forward() / Detect() / postprocess() surface.  See DESIGN.md and INTEGRAT
 from .config import cfg, set_cfg, CONFIGS, MEANS, STD  # noqa: F401
 
 __all__ = ["cfg", "set_cfg", "CONFIGS", "Yolact", "Detect", "postprocess", "postprocess_list", "FastBaseTransform",
-           "render_masks", "APData", "prep_metrics", "calc_map", "Detections"]
+           "render_masks", "APData", "prep_metrics", "prep_metrics_list", "calc_map", "Detections"]
 
 
 def __getattr__(name):  # lazy: importing the package must not require torch/CUDA
@@ -22,7 +22,7 @@ def __getattr__(name):  # lazy: importing the package must not require torch/CUD
     if name == "render_masks":
         from .display import render_masks
         return render_masks
-    if name in ("APData", "prep_metrics", "calc_map", "Detections"):
+    if name in ("APData", "prep_metrics", "prep_metrics_list", "calc_map", "Detections"):
         from . import metrics
         return getattr(metrics, name)
     if name == "FastBaseTransform":

@@ -55,6 +55,46 @@ class YbPostItem(ctypes.Structure):
     ]
 
 
+class YbEvalIouItem(ctypes.Structure):
+    """Mirror of yb_eval_iou_item (one image of yb_eval_iou_list)."""
+    _fields_ = [
+        ("proto", c_void_p),
+        ("coef", c_void_p),
+        ("box", c_void_p),
+        ("boxes_px", c_void_p),
+        ("gt_bits", c_void_p),
+        ("gt_boxes", c_void_p),
+        ("box_iou", c_void_p),
+        ("mask_iou", c_void_p),
+        ("crowd_box_iou", c_void_p),
+        ("crowd_mask_iou", c_void_p),
+        ("n", c_int32),
+        ("out_h", c_int32),
+        ("out_w", c_int32),
+        ("g_all", c_int32),
+        ("num_crowd", c_int32),
+    ]
+
+
+class YbEvalMatchItem(ctypes.Structure):
+    """Mirror of yb_eval_match_item (one image of yb_eval_match_list)."""
+    _fields_ = [
+        ("box_iou", c_void_p),
+        ("mask_iou", c_void_p),
+        ("crowd_box_iou", c_void_p),
+        ("crowd_mask_iou", c_void_p),
+        ("cls", c_void_p),
+        ("box_score", c_void_p),
+        ("mask_score", c_void_p),
+        ("gt_cls", c_void_p),
+        ("crowd_cls", c_void_p),
+        ("rec_offset", c_int64),
+        ("n", c_int32),
+        ("g", c_int32),
+        ("num_crowd", c_int32),
+    ]
+
+
 class YbRenderItem(ctypes.Structure):
     """Mirror of yb_render_item (one frame of yb_render_list)."""
     _fields_ = [
@@ -157,6 +197,8 @@ SIGNATURES = {
     "yb_mask_rle": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p]),
     "yb_eval_match": (c_int, [c_void_p] + [c_void_p] * 7 + [c_int, c_void_p, c_int, c_void_p, c_int,
                                                               POINTER(ctypes.c_double), c_int, c_int] + [c_void_p] * 5),
+    "yb_eval_iou_list": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "yb_eval_match_list": (c_int, [c_void_p, c_void_p, c_int, POINTER(ctypes.c_double), c_int, c_int] + [c_void_p] * 5),
     "yb_eval_ap_workspace": (c_int, [c_int64, c_int, c_int, POINTER(c_int64)]),
     "yb_eval_ap": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_int64, c_void_p,
                            c_void_p, c_void_p]),

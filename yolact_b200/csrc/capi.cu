@@ -699,7 +699,8 @@ int yb_eval_match(yb_handle* h, const float* d_box_iou, const float* d_mask_iou,
   YB_REQUIRE(n == 0 || g == 0 || (d_box_iou && d_mask_iou && d_gt_cls), "yb_eval_match: null ground-truth argument");
   YB_REQUIRE(n == 0 || num_crowd == 0 || (d_crowd_box_iou && d_crowd_mask_iou && d_crowd_cls),
              "yb_eval_match: null crowd argument");
-  EvalMatchArgs a{};
+  EvalMatchSrc src{};
+  yb_eval_match_item& a = src.one;
   a.box_iou = d_box_iou;
   a.mask_iou = d_mask_iou;
   a.crowd_box_iou = d_crowd_box_iou;
@@ -712,15 +713,88 @@ int yb_eval_match(yb_handle* h, const float* d_box_iou, const float* d_mask_iou,
   a.n = n;
   a.g = g;
   a.num_crowd = num_crowd;
-  a.T = T;
-  a.C = C;
-  for (int t = 0; t < T; ++t) a.thr[t] = h_thresholds[t];
-  a.rec_score = d_rec_score;
-  a.rec_tag = d_rec_tag;
-  a.counts = d_counts;
-  a.err = d_err;
+  src.T = T;
+  src.C = C;
+  for (int t = 0; t < T; ++t) src.thr[t] = h_thresholds[t];
+  src.rec_score = d_rec_score;
+  src.rec_tag = d_rec_tag;
+  src.counts = d_counts;
+  src.err = d_err;
   CallGuard gd(h);
-  launch_eval_match(a, (cudaStream_t)stream, &h->lc);
+  launch_eval_match(src, &src.one, 1, (cudaStream_t)stream, &h->lc);
+  YB_API_END
+}
+
+int yb_eval_match_list(yb_handle* h, const yb_eval_match_item* h_items, int B, const double* h_thresholds, int T, int C,
+                       float* d_rec_score, int32_t* d_rec_tag, int64_t* d_counts, int32_t* d_err, void* stream) {
+  YB_API_BEGIN
+  YB_REQUIRE(h && B >= 0 && (B == 0 || h_items) && h_thresholds && d_counts && d_err,
+             "yb_eval_match_list: null argument");
+  eval_check_limits(0, 0, 0, T, C);
+  auto on_device = [h](const void* p) { return on_handle_device(h, p); };
+  YB_REQUIRE(on_device(d_rec_score) && on_device(d_rec_tag) && on_device(d_counts) && on_device(d_err),
+             "yb_eval_match_list: an output is not device memory of the handle's device");
+  for (int b = 0; b < B; ++b) {
+    const yb_eval_match_item& it = h_items[b];
+    eval_check_limits(it.n, it.g, it.num_crowd, T, C);
+    YB_REQUIRE(it.rec_offset >= 0, "yb_eval_match_list: negative record offset");
+    if (it.n == 0) continue;
+    YB_REQUIRE(it.cls && it.box_score && it.mask_score && d_rec_score && d_rec_tag,
+               "yb_eval_match_list: null detection argument");
+    YB_REQUIRE(it.g == 0 || (it.box_iou && it.mask_iou && it.gt_cls), "yb_eval_match_list: null ground-truth argument");
+    YB_REQUIRE(it.num_crowd == 0 || (it.crowd_box_iou && it.crowd_mask_iou && it.crowd_cls),
+               "yb_eval_match_list: null crowd argument");
+    YB_REQUIRE(on_device(it.box_iou) && on_device(it.mask_iou) && on_device(it.crowd_box_iou) &&
+                   on_device(it.crowd_mask_iou) && on_device(it.cls) && on_device(it.box_score) &&
+                   on_device(it.mask_score) && on_device(it.gt_cls) && on_device(it.crowd_cls),
+               "yb_eval_match_list: a pointer is not device memory of the handle's device");
+  }
+  EvalMatchSrc src{};
+  src.T = T;
+  src.C = C;
+  for (int t = 0; t < T; ++t) src.thr[t] = h_thresholds[t];
+  src.rec_score = d_rec_score;
+  src.rec_tag = d_rec_tag;
+  src.counts = d_counts;
+  src.err = d_err;
+  CallGuard gd(h, (cudaStream_t)stream);   // shared item table: ordered behind the previous call
+  src.table = stage_items(h->eval_match_table, (size_t)std::max(B, 1) * sizeof(yb_eval_match_item), h_items, B, stream);
+  launch_eval_match(src, h_items, B, (cudaStream_t)stream, &h->lc);
+  YB_API_END
+}
+
+int yb_eval_iou_list(yb_handle* h, const yb_eval_iou_item* h_items, int B, int ph, int pw, int k, int crop_masks,
+                     void* stream) {
+  YB_API_BEGIN
+  YB_REQUIRE(h && B >= 0 && B <= 65535 && (B == 0 || h_items), "yb_eval_iou_list: bad argument");
+  auto on_device = [h](const void* p) { return on_handle_device(h, p); };
+  for (int b = 0; b < B; ++b) {
+    const yb_eval_iou_item& it = h_items[b];
+    YB_REQUIRE(it.n >= 0 && it.n <= EVAL_MAX_DETS, "yb_eval_iou_list: n must be in [0, 1024]");
+    YB_REQUIRE(it.out_h > 0 && it.out_w > 0 && (int64_t)it.out_h * it.out_w <= (1ll << 28),
+               "yb_eval_iou_list: out_h, out_w must be > 0, at most 2^28 pixels");
+    YB_REQUIRE(it.g_all >= 0 && it.num_crowd >= 0 && it.num_crowd <= it.g_all, "yb_eval_iou_list: num_crowd outside [0, g_all]");
+    YB_REQUIRE(it.g_all - it.num_crowd <= EVAL_MAX_GT && it.num_crowd <= EVAL_MAX_GT,
+               "yb_eval_iou_list: at most 1024 ground truths and 1024 crowds per image");
+    const int g = it.g_all - it.num_crowd;
+    if (it.n > 0) {
+      YB_REQUIRE(it.proto && it.coef && it.box && it.boxes_px, "yb_eval_iou_list: null proto, coef, box or boxes_px");
+      YB_REQUIRE(it.g_all == 0 || (it.gt_bits && it.gt_boxes), "yb_eval_iou_list: null ground truth");
+      YB_REQUIRE(g == 0 || (it.box_iou && it.mask_iou), "yb_eval_iou_list: null box_iou or mask_iou");
+      YB_REQUIRE(it.num_crowd == 0 || (it.crowd_box_iou && it.crowd_mask_iou),
+                 "yb_eval_iou_list: null crowd_box_iou or crowd_mask_iou");
+    }
+    YB_REQUIRE(on_device(it.proto) && on_device(it.coef) && on_device(it.box) && on_device(it.boxes_px) &&
+                   on_device(it.gt_bits) && on_device(it.gt_boxes) && on_device(it.box_iou) && on_device(it.mask_iou) &&
+                   on_device(it.crowd_box_iou) && on_device(it.crowd_mask_iou),
+               "yb_eval_iou_list: a pointer is not device memory of the handle's device");
+  }
+  YB_REQUIRE(k % 4 == 0 && k >= 4 && k <= 128 && ph > 0 && pw > 0,
+             "yb_eval_iou_list: mask_dim must be a multiple of 4 and <= 128, ph and pw > 0");
+  CallGuard gd(h, (cudaStream_t)stream);   // shared item table: ordered behind the previous call
+  const yb_eval_iou_item* table =
+      stage_items(h->eval_iou_table, (size_t)std::max(B, 1) * sizeof(yb_eval_iou_item), h_items, B, stream);
+  launch_eval_iou(table, h_items, B, ph, pw, k, crop_masks, (cudaStream_t)stream, &h->lc);
   YB_API_END
 }
 

@@ -12,54 +12,19 @@
 //                     into runs, and the CTA writes rleToString's characters into the caller's character arena
 //                     (character lengths in parallel, a block scan for the offsets, an atomic add for the space).
 //
-// Mask pixels go through mask_math.cuh (crop_window, lincomb_sigmoid, interp_entry, bilinear4), the functions
-// mask_assembly_kernel uses, with the same crop-before-upsample order, so the runs are yb_mask_rle's of yb_postprocess's
-// masks, bit for bit.
+// Mask pixels come from staged_mask.cuh's StagedMask, which evaluates them through mask_math.cuh (crop_window,
+// lincomb_sigmoid, interp_entry, bilinear4), the functions mask_assembly_kernel uses, with the same crop-before-upsample
+// order, so the runs are yb_mask_rle's of yb_postprocess's masks, bit for bit.
 #include <algorithm>
 #include "kernels.cuh"
-#include "mask_math.cuh"
 #include "rle_walk.cuh"
+#include "staged_mask.cuh"
 
 namespace yb {
 
 namespace {
 
 constexpr int CR_MAX_THREADS = 1024;
-
-// Pixel source of the walk: the cropped sigmoid values of the prototype rows [r_lo, r_lo + nr) and the columns the
-// current chunk reads, staged in sig [nr][nc].
-struct StagedMask {
-  const float* proto;
-  const float* cf;   // the row's coefficients
-  float* sig;
-  int ph, pw, k, xa;
-  float cx1, cx2, cy1, cy2, scale_h, scale_w;
-  int r_lo, nr, c_lo, nc;
-  int staged_a, staged_b;   // output columns whose sources are staged (a chunk already staged is not staged again)
-
-  __device__ void chunk(int c0, int c1) {
-    const int a = max(c0 - 1, xa);   // column c0 - 1's last row is the first pixel's predecessor
-    if (a == staged_a && c1 == staged_b) return;   // uniform
-    staged_a = a, staged_b = c1;
-    c_lo = interp_entry(a, scale_w, pw).i0;
-    nc = interp_entry(c1 - 1, scale_w, pw).i1 - c_lo + 1;
-    __syncthreads();   // the previous chunk's values are no longer read
-    for (int idx = threadIdx.x; idx < nr * nc; idx += blockDim.x) {
-      const int rr = idx / nc, r = r_lo + rr, c = c_lo + (idx - rr * nc);
-      float v = 0.f;
-      if ((float)c >= cx1 && (float)c < cx2 && (float)r >= cy1 && (float)r < cy2)
-        v = lincomb_sigmoid(proto + ((size_t)r * pw + c) * k, cf, k);
-      sig[idx] = v;
-    }
-    __syncthreads();
-  }
-
-  __device__ __forceinline__ int operator()(int y, int x) const {
-    const ColTab rt = interp_entry(y, scale_h, ph), ct = interp_entry(x, scale_w, pw);
-    return bilinear4(rt, ct, sig + (size_t)(rt.i0 - r_lo) * nc, sig + (size_t)(rt.i1 - r_lo) * nc, ct.i0 - c_lo,
-                     ct.i1 - c_lo) > 0.5f;
-  }
-};
 
 // maskApi.c rleToString of one count: x = cnts[i] - cnts[i-2] for i > 2, 5 bits per character from the low end, 0x20
 // while more follow, + 48.  At most 7 characters for a 32-bit count.
@@ -107,22 +72,8 @@ coco_rle_kernel(const yb_post_item* __restrict__ items, int ph, int pw, int k, i
   const int h = it.out_h, w = it.out_w;
 
   StagedMask px;
-  px.proto = it.proto;
-  px.cf = it.coef + (size_t)d * k;
-  px.sig = sig;
-  px.ph = ph, px.pw = pw, px.k = k;
-  px.scale_h = __fdiv_rn((float)ph, (float)h);
-  px.scale_w = __fdiv_rn((float)pw, (float)w);
-  crop_window(it.box, d, crop, ph, pw, px.cx1, px.cx2, px.cy1, px.cy2);
   int xa, xb, ya, yb;   // the output pixels that can be set
-  window_out_bounds(px.cx1, px.cx2, px.scale_w, w, &xa, &xb);
-  window_out_bounds(px.cy1, px.cy2, px.scale_h, h, &ya, &yb);
-  if (xa >= xb || ya >= yb) xa = xb = ya = yb = 0;   // an empty mask: one run of zeros
-  px.xa = xa;
-  px.staged_a = px.staged_b = -1;
-  px.c_lo = px.nc = 0;
-  px.r_lo = ya < yb ? interp_entry(ya, px.scale_h, ph).i0 : 0;
-  px.nr = ya < yb ? interp_entry(yb - 1, px.scale_h, ph).i1 - px.r_lo + 1 : 0;
+  px.init(it.proto, it.coef, it.box, d, crop, ph, pw, k, h, w, sig, &xa, &xb, &ya, &yb);
 
   // pass 1: the number of value changes T; the mask has T + 1 runs
   const int64_t T = rle_walk(px, h, w, xa, xb, ya, yb, nullptr, 0, s_warp);
@@ -216,9 +167,7 @@ void launch_coco_rle(const yb_post_item* d_items, const yb_post_item* h_items, i
     for (int b = 0; b < B; ++b) {
       const yb_post_item& it = h_items[b];
       if (it.n == 0) continue;
-      const float scale_w = (float)pw / (float)it.out_w;
-      const int64_t cols = std::min<int64_t>(pw, (int64_t)((double)threads * scale_w) + 4);
-      sig_cap = std::max<int64_t>(sig_cap, (int64_t)ph * cols);
+      sig_cap = std::max<int64_t>(sig_cap, (int64_t)ph * staged_cols(threads, pw, it.out_w));
     }
     if (sig_cap * 4 <= 200 * 1024 || threads == 32) break;
     threads /= 2;

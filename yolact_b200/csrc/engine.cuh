@@ -176,6 +176,8 @@ struct yb_handle {
   yb::DeviceBuffer detect_ws;
   yb::DeviceBuffer scratch;   // maskiou temporaries
   yb::DeviceBuffer post_table{16 * sizeof(yb_post_item)};   // yb_postprocess_list's and yb_coco_rle_list's item table
+  yb::DeviceBuffer eval_iou_table{16 * sizeof(yb_eval_iou_item)};       // yb_eval_iou_list's item table
+  yb::DeviceBuffer eval_match_table{16 * sizeof(yb_eval_match_item)};   // yb_eval_match_list's item table
   // yb_render_list's device item table and, after it, the work table that carries the selection from the call's first
   // launch to its second
   yb::DeviceBuffer render_ws{64 * 1024};

@@ -1,6 +1,6 @@
 // eval.py's mAP bookkeeping (prep_metrics' matching loop, APDataObject.get_ap; eval.py:386-581) on the GPU.
 //
-//   eval_match : one CTA per image.  The two stable score orders (eval.py:445-446) are ranked by counting, then one
+//   eval_match : one CTA per image (yb_eval_match's one image, or every image of a yb_eval_match_list table).  The two stable score orders (eval.py:445-446) are ranked by counting, then one
 //                warp per (class with detections, IoU threshold, box|mask) job replays the greedy matching loop
 //                (eval.py:458-509) over that class's detections in rank order.  Every detection leaves one record
 //                per (type, threshold) at slot [type][thr][rank] of the image's 2*T*n-record slot: fp32 score and
@@ -31,7 +31,7 @@ constexpr int AP_THREADS = 256;
 constexpr int AP_BARS = 101;
 
 __global__ void __launch_bounds__(MATCH_THREADS)
-eval_match_kernel(EvalMatchArgs a) {
+eval_match_kernel(EvalMatchSrc s) {
   __shared__ int s_cls[EVAL_MAX_DETS];
   __shared__ int s_rank_box[EVAL_MAX_DETS], s_rank_mask[EVAL_MAX_DETS];
   __shared__ int s_ord_box[EVAL_MAX_DETS], s_ord_mask[EVAL_MAX_DETS];
@@ -40,15 +40,19 @@ eval_match_kernel(EvalMatchArgs a) {
   __shared__ int s_jobs[EVAL_MAX_DETS];       // the classes with detections
   __shared__ uint32_t s_used[MATCH_WARPS][EVAL_MAX_GT / 32];
   __shared__ int s_njobs;
-  const int n = a.n, g = a.g, nc = a.num_crowd, C = a.C, T = a.T;
+  const yb_eval_match_item a = s.table ? s.table[blockIdx.x] : s.one;
+  const int n = a.n, g = a.g, nc = a.num_crowd, C = s.C, T = s.T;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (n == 0) return;   // eval.py:405-406: an image without detections adds nothing, not even its ground truths
+  float* const rec_score = s.rec_score + a.rec_offset;
+  int32_t* const rec_tag = s.rec_tag + a.rec_offset;
 
   for (int c = tid; c < C; c += MATCH_THREADS) s_first[c] = n;
   for (int j = tid; j < g; j += MATCH_THREADS) {
     const int c = a.gt_cls[j];
     s_gt_cls[j] = c;
-    if (c >= 0 && c < C) atomicAdd(reinterpret_cast<unsigned long long*>(a.counts + c), 1ull);   // add_gt_positives
-    else atomicOr(a.err, 2);
+    if (c >= 0 && c < C) atomicAdd(reinterpret_cast<unsigned long long*>(s.counts + c), 1ull);   // add_gt_positives
+    else atomicOr(s.err, 2);
   }
   for (int j = tid; j < nc; j += MATCH_THREADS) s_crowd_cls[j] = a.crowd_cls[j];
   if (tid == 0) s_njobs = 0;
@@ -58,7 +62,7 @@ eval_match_kernel(EvalMatchArgs a) {
     const bool ok = c >= 0 && c < C;
     s_cls[i] = ok ? (int)c : -1;
     if (ok) atomicMin(&s_first[c], i);
-    else atomicOr(a.err, 1);
+    else atomicOr(s.err, 1);
   }
   // box_indices = sorted(range(n), key=-box_score): a stable sort, so rank(i) = #{j : s_j > s_i or (s_j == s_i, j < i)}
   for (int i = tid; i < n; i += MATCH_THREADS) {
@@ -95,7 +99,7 @@ eval_match_kernel(EvalMatchArgs a) {
   const int64_t n64 = n;
   for (int job = warp; job < njobs; job += MATCH_WARPS) {
     const int type = job & 1, thr = (job >> 1) % T, c = s_jobs[(job >> 1) / T];
-    const double th = a.thr[thr];
+    const double th = s.thr[thr];
     const float* iou = type ? a.mask_iou : a.box_iou;
     const float* ciou = type ? a.crowd_mask_iou : a.crowd_box_iou;
     const float* score = type ? a.mask_score : a.box_score;
@@ -104,8 +108,8 @@ eval_match_kernel(EvalMatchArgs a) {
     for (int w = lane; w < EVAL_MAX_GT / 32; w += 32) used[w] = 0u;
     __syncwarp();
     const int tag_base = 2 * ((type * T + thr) * C + c);
-    float* out_score = a.rec_score + (int64_t)(type * T + thr) * n64;
-    int32_t* out_tag = a.rec_tag + (int64_t)(type * T + thr) * n64;
+    float* out_score = rec_score + (int64_t)(type * T + thr) * n64;
+    int32_t* out_tag = rec_tag + (int64_t)(type * T + thr) * n64;
     for (int r0 = 0; r0 < n; r0 += 32) {
       const int r = r0 + lane;
       const int i_l = r < n ? ord[r] : 0;
@@ -157,8 +161,8 @@ eval_match_kernel(EvalMatchArgs a) {
     const int i = idx % n, tt = idx / n;
     if (s_cls[i] < 0) {
       const int rk = (tt >= T) ? s_rank_mask[i] : s_rank_box[i];
-      a.rec_score[(int64_t)tt * n64 + rk] = 0.f;
-      a.rec_tag[(int64_t)tt * n64 + rk] = -1;
+      rec_score[(int64_t)tt * n64 + rk] = 0.f;
+      rec_tag[(int64_t)tt * n64 + rk] = -1;
     }
   }
 }
@@ -334,10 +338,17 @@ void eval_check_limits(int n, int g, int num_crowd, int T, int C) {
   YB_REQUIRE(C >= 1 && C <= EVAL_MAX_CLASSES, "eval: 1 to 2048 classes");
 }
 
-void launch_eval_match(const EvalMatchArgs& a, cudaStream_t stream, LaunchCounter* lc) {
-  eval_check_limits(a.n, a.g, a.num_crowd, a.T, a.C);
-  if (a.n == 0) return;   // eval.py:405-406: an image without detections adds nothing, not even its ground truths
-  eval_match_kernel<<<1, MATCH_THREADS, 0, stream>>>(a);
+void launch_eval_match(const EvalMatchSrc& src, const yb_eval_match_item* h_items, int B, cudaStream_t stream,
+                       LaunchCounter* lc) {
+  YB_REQUIRE(B >= 0 && (B == 0 || h_items), "eval_match: bad image list");
+  bool any = false;
+  for (int b = 0; b < B; ++b) {
+    eval_check_limits(h_items[b].n, h_items[b].g, h_items[b].num_crowd, src.T, src.C);
+    YB_REQUIRE(h_items[b].rec_offset >= 0, "eval_match: negative record offset");
+    any |= h_items[b].n > 0;
+  }
+  if (!any) return;   // eval.py:405-406: an image without detections adds nothing, not even its ground truths
+  eval_match_kernel<<<B, MATCH_THREADS, 0, stream>>>(src);
   YB_CHECK_LAUNCH();
   if (lc) lc->n++;
 }

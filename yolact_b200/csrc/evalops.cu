@@ -109,9 +109,7 @@ mask_iou_bits_kernel(const uint32_t* __restrict__ a, const uint32_t* __restrict_
       ta += red[1][w];
       tb += red[2][w];
     }
-    // box_utils.py:113 in fp32: intersection / (area_a + area_b - intersection)   |   / area_a
-    const float fi = (float)ti, fa = (float)ta, fb = (float)tb;
-    out[(int64_t)i * m + j] = iscrowd ? __fdiv_rn(fi, fa) : __fdiv_rn(fi, __fsub_rn(__fadd_rn(fa, fb), fi));
+    out[(int64_t)i * m + j] = mask_iou_counts(ti, ta, tb, iscrowd);
   }
 }
 
@@ -121,16 +119,7 @@ box_iou_kernel(const float* __restrict__ a, int n, const float* __restrict__ b, 
   const int64_t total = (int64_t)n * m;
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
     const int i = (int)(t / m), j = (int)(t - (int64_t)i * m);
-    const float4 A = reinterpret_cast<const float4*>(a)[i];
-    const float4 Bx = reinterpret_cast<const float4*>(b)[j];
-    // box_utils.py:46-51 (intersect) and :72-79 (jaccard)
-    const float iw = fmaxf(__fsub_rn(fminf(A.z, Bx.z), fmaxf(A.x, Bx.x)), 0.f);
-    const float ih = fmaxf(__fsub_rn(fminf(A.w, Bx.w), fmaxf(A.y, Bx.y)), 0.f);
-    const float inter = __fmul_rn(iw, ih);
-    const float area_a = __fmul_rn(__fsub_rn(A.z, A.x), __fsub_rn(A.w, A.y));
-    const float area_b = __fmul_rn(__fsub_rn(Bx.z, Bx.x), __fsub_rn(Bx.w, Bx.y));
-    const float uni = __fsub_rn(__fadd_rn(area_a, area_b), inter);
-    out[t] = iscrowd ? __fdiv_rn(inter, area_a) : __fdiv_rn(inter, uni);
+    out[t] = box_jaccard(reinterpret_cast<const float4*>(a)[i], reinterpret_cast<const float4*>(b)[j], iscrowd);
   }
 }
 

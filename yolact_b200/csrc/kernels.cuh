@@ -208,21 +208,28 @@ void launch_display_blend(const float* img, int img_is_255, const void* masks, i
 
 // ---- eval.py's mAP: detection-to-ground-truth matching and get_ap (evalmap.cu) --------------------------------------
 constexpr int EVAL_MAX_DETS = 1024, EVAL_MAX_GT = 1024, EVAL_MAX_THRESHOLDS = 32, EVAL_MAX_CLASSES = 2048;
-// One image (device pointers; the IoU caches are [n,g] / [n,num_crowd] fp32, nullable when that side is empty).
-struct EvalMatchArgs {
-  const float *box_iou, *mask_iou, *crowd_box_iou, *crowd_mask_iou;
-  const int64_t* cls;                   // [n]
-  const float *box_score, *mask_score;  // [n]
-  const int32_t *gt_cls, *crowd_cls;    // [g], [num_crowd]
-  int n, g, num_crowd, T, C;
+// The images of one eval_match launch, one CTA each: a table of B items in device memory (yb_eval_match_list), or, with
+// table == nullptr, the one image `one` (yb_eval_match: passed by value, nothing uploaded).  An item's IoU caches are
+// [n,g] / [n,num_crowd] fp32 (nullable when that side is empty); its records go to rec_score / rec_tag + rec_offset.
+struct EvalMatchSrc {
+  const yb_eval_match_item* table;
+  yb_eval_match_item one;
+  int T, C;
   double thr[EVAL_MAX_THRESHOLDS];
-  float* rec_score;                     // [2][T][n] at the image's slot
+  float* rec_score;                     // [2][T][n] per image at its rec_offset
   int32_t* rec_tag;                     // [2][T][n]: 2 * cell + is_true, or -1 (crowd hit / bad class)
   int64_t* counts;                      // [C] non-crowd ground truths per class, accumulated
   int32_t* err;                         // bit 0: detection class out of range, bit 1: ground-truth class out of range
 };
 void eval_check_limits(int n, int g, int num_crowd, int T, int C);
-void launch_eval_match(const EvalMatchArgs& a, cudaStream_t stream, LaunchCounter* lc);
+// One launch for the B images of src (h_items: their host view, B entries, or &src.one with B == 1); none when no image
+// has detections.
+void launch_eval_match(const EvalMatchSrc& src, const yb_eval_match_item* h_items, int B, cudaStream_t stream,
+                       LaunchCounter* lc);
+// The four IoU caches of the B images of d_items (device; h_items is its host view) straight from the detections, in one
+// launch (evaliou.cu); none when no image has both detections and ground truth.
+void launch_eval_iou(const yb_eval_iou_item* d_items, const yb_eval_iou_item* h_items, int B, int ph, int pw, int k,
+                     int crop, cudaStream_t stream, LaunchCounter* lc);
 size_t eval_ap_workspace_bytes(int64_t R, int T, int C);
 // R records -> ap [2][T][C] double, nonempty [2][T][C] uint8 (APDataObject.get_ap / is_empty of every cell)
 void launch_eval_ap(const float* rec_score, const int32_t* rec_tag, int64_t R, const int64_t* counts, int T, int C,

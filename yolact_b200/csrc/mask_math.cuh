@@ -1,6 +1,7 @@
 // Per-pixel arithmetic shared by the mask kernels (mask.cu), the display blend (evalops.cu) and the fused mask render
 // (render.cu).  Every kernel that produces or consumes a mask pixel evaluates it through these functions, so their
-// results agree bit for bit by construction.
+// results agree bit for bit by construction.  The box IoU of jaccard is here too, for box_iou_kernel (evalops.cu) and
+// eval_iou_kernel (evaliou.cu).
 #pragma once
 #include "common.cuh"
 
@@ -115,6 +116,24 @@ __device__ __forceinline__ uint8_t blend_out(float v, float prod, float sum, boo
   if (dim) v = __fmul_rn(v, 0.6f);
   v = __fmul_rn(v, 255.f);
   return (uint8_t)(int)fminf(fmaxf(v, 0.f), 255.f);
+}
+
+// ---- jaccard (box_utils.py:46-51 intersect, :72-79 jaccard) of one pair of x1y1x2y2 boxes ---------------------------
+__device__ __forceinline__ float box_jaccard(float4 A, float4 B, int iscrowd) {
+  const float iw = fmaxf(__fsub_rn(fminf(A.z, B.z), fmaxf(A.x, B.x)), 0.f);
+  const float ih = fmaxf(__fsub_rn(fminf(A.w, B.w), fmaxf(A.y, B.y)), 0.f);
+  const float inter = __fmul_rn(iw, ih);
+  const float area_a = __fmul_rn(__fsub_rn(A.z, A.x), __fsub_rn(A.w, A.y));
+  const float area_b = __fmul_rn(__fsub_rn(B.z, B.x), __fsub_rn(B.w, B.y));
+  const float uni = __fsub_rn(__fadd_rn(area_a, area_b), inter);
+  return iscrowd ? __fdiv_rn(inter, area_a) : __fdiv_rn(inter, uni);
+}
+
+// mask_iou (box_utils.py:113) in fp32 from the popcounts: intersection / (area_a + area_b - intersection), or / area_a
+// when iscrowd; 0 / 0 is NaN as in the reference
+__device__ __forceinline__ float mask_iou_counts(unsigned inter, unsigned area_a, unsigned area_b, int iscrowd) {
+  const float fi = (float)inter, fa = (float)area_a, fb = (float)area_b;
+  return iscrowd ? __fdiv_rn(fi, fa) : __fdiv_rn(fi, __fsub_rn(__fadd_rn(fa, fb), fi));
 }
 
 }  // namespace yb

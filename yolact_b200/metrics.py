@@ -13,6 +13,7 @@ appending fixed-size records to a device buffer: no host synchronisation and no 
 call (yb_eval_ap) sorts the records stably per cell and computes every get_ap in double; get_ap() synchronises once.
 The result is the reference's to the bit: same data points in the same push order, same counts, same doubles.
 """
+import collections
 import ctypes
 
 import numpy as np
@@ -221,6 +222,212 @@ def prep_metrics(ap_data, dets, img, gt, gt_masks, h, w, num_crowd, image_id, de
     if classes.size(0) == 0:
         return
     ap_data.add(classes, scores, boxes, masks, gt, gt_masks, h, w, num_crowd)
+
+
+# ---- prep_metrics for a list of images, straight from the detections --------------------------------------------------
+# One image's ground truth as APData.add takes it: boxes fp32 [g_all,4] in pixels (scaled in fp32, eval.py:390-392),
+# classes int32 [g_all], masks [g_all,h,w] (host array or device tensor, as given), the crowds the last num_crowd rows.
+_GtImage = collections.namedtuple("_GtImage", "boxes cls masks h w g_all num_crowd")
+
+
+def _gt_image(gt, gt_masks, h, w, num_crowd, num_classes, where):
+    """APData.add's checks and staging form of one image's ground truth -> _GtImage; ValueError where APData.add
+    raises one."""
+    gt = np.asarray(gt.cpu() if isinstance(gt, torch.Tensor) else gt)
+    gt = gt.reshape(-1, 5) if gt.size else np.zeros((0, 5), np.float32)
+    g_all = int(gt.shape[0])
+    if not 0 <= num_crowd <= g_all:
+        raise ValueError("%s: num_crowd %d outside [0, %d]" % (where, num_crowd, g_all))
+    g = g_all - num_crowd
+    gt_cls = gt[:, 4].astype(int)
+    if g and (gt_cls[:g].min() < 0 or gt_cls[:g].max() >= num_classes):
+        raise ValueError("%s: a ground-truth class is outside [0, %d)" % (where, num_classes))
+    gm_shape = tuple(gt_masks.shape) if g_all else ()
+    if g_all and (len(gm_shape) < 2 or gm_shape[0] != g_all or gm_shape[-2:] != (h, w)):
+        raise ValueError("%s: gt_masks are %s, expected [%d, %d, %d]" % (where, gm_shape, g_all, h, w))
+    boxes = gt[:, :4].astype(np.float32)
+    boxes[:, [0, 2]] *= np.float32(w)
+    boxes[:, [1, 3]] *= np.float32(h)
+    return _GtImage(boxes, gt_cls.astype(np.int32), gt_masks if g_all else None, h, w, g_all, num_crowd)
+
+
+# Where _gt_layout puts each image in the staged ground truth: byte offsets of the three sections of the buffer, and
+# per image its first ground-truth row and its first mask word (YB_MASK_BITS words, one [g_all, h, ceil(w/32)] block
+# per image in image order).
+_GtLayout = collections.namedtuple("_GtLayout", "nbytes box_at cls_at mask_at rows words")
+
+
+def _gt_layout(images):
+    """The staging buffer of a list of _GtImage: boxes fp32 [G,4] | classes int32 [G] | masks uint8 [W,32], G = sum of
+    g_all, W = sum of g_all * h * ceil(w/32): each mask row padded with zeros to whole words of 32 pixels, so that
+    packing the W rows of 32 bytes gives every image's YB_MASK_BITS block at once.  Sections 16-byte aligned."""
+    rows, words = [], []
+    G = W = 0
+    for im in images:
+        rows.append(G)
+        words.append(W)
+        G += im.g_all
+        W += im.g_all * im.h * ((im.w + 31) // 32)
+    align = lambda v: (v + 15) // 16 * 16
+    box_at = 0
+    cls_at = align(16 * G)
+    mask_at = align(cls_at + 4 * G)
+    return _GtLayout(mask_at + 32 * W, box_at, cls_at, mask_at, rows, words)
+
+
+def _host_mask_bits(m, g_all, h, w, out):
+    """Host masks [g_all,h,w] -> out (bool, same shape, any strides): value > 0.5 after the fp32 conversion pack_masks
+    makes, in one pass that writes straight into the staging buffer."""
+    m = np.asarray(m.cpu() if isinstance(m, torch.Tensor) else m).reshape(g_all, h, w)
+    if m.dtype.kind == "f" and m.dtype != np.float32:
+        m = m.astype(np.float32)
+    np.greater(m, 0.5, out=out)
+
+
+def _fill_gt(buf, images, lay):
+    """Writes the host parts of images into buf (CPU uint8 tensor [lay.nbytes]) at lay's places; device masks are left
+    for the caller (their bytes are zeroed).  -> the indices of the images whose masks are device tensors."""
+    G = lay.rows[-1] + images[-1].g_all if images else 0
+    host = buf.numpy()
+    boxes = host[lay.box_at:lay.box_at + 16 * G].view(np.float32).reshape(G, 4)
+    cls = host[lay.cls_at:lay.cls_at + 4 * G].view(np.int32)
+    on_device = []
+    for j, im in enumerate(images):
+        r, wd = lay.rows[j], lay.words[j]
+        boxes[r:r + im.g_all] = im.boxes
+        cls[r:r + im.g_all] = im.cls
+        if not im.g_all:
+            continue
+        wpr = (im.w + 31) // 32
+        dst = host[lay.mask_at + 32 * wd:lay.mask_at + 32 * (wd + im.g_all * im.h * wpr)].reshape(im.g_all, im.h,
+                                                                                               32 * wpr)
+        dst[:, :, im.w:] = 0
+        if isinstance(im.masks, torch.Tensor) and im.masks.is_cuda:
+            on_device.append(j)
+            dst[:, :, :im.w] = 0
+            continue
+        _host_mask_bits(im.masks, im.g_all, im.h, im.w, dst[:, :, :im.w].view(np.bool_))
+    return on_device
+
+
+# The caches of one prep_metrics_list call: per image with detections, (image index, n, g, num_crowd, box_iou [n,g],
+# mask_iou [n,g], crowd_box_iou [n,nc], crowd_mask_iou [n,nc]); the classes, box and mask scores of those images; their
+# ground-truth classes (device int32, per image [g_all]); keep_alive, what the launches read.
+_IouList = collections.namedtuple("_IouList", "images cls box_s mask_s gt_cls keep_alive")
+
+
+def _iou_list(num_classes, dev, preds, sizes, gts, gt_masks, num_crowds, crop_masks, score_threshold,
+              where="prep_metrics_list"):
+    """Everything prep_metrics_list does before the matching: postprocess without masks, the ground truth in one
+    pinned buffer and one H2D copy, one pack launch, one yb_eval_iou_list launch -> _IouList, or None when no image
+    has detections."""
+    from .output_utils import _postprocess_list
+    B = len(preds)
+    for name, v in (("sizes", sizes), ("gts", gts), ("gt_masks", gt_masks), ("num_crowds", num_crowds)):
+        if len(v) != B:
+            raise ValueError("%s: %d %s for %d images" % (where, len(v), name, B))
+    from . import config as _config
+    live = [d['detection'] for d in preds if d['detection'] is not None]
+    if not getattr(_config.cfg, "eval_mask_branch", True) or any('proto' not in d for d in live):
+        raise ValueError("%s: the mask mAP needs masks; with cfg.eval_mask_branch off (--detect) the detections carry "
+                         "no prototypes" % where)
+    for d in live:
+        _require_cuda(d['box'], "metrics." + where)
+        if d['class'].device != dev:
+            raise ValueError("%s: the detections are on %s, the accumulator on %s" % (where, d['class'].device, dev))
+    res = _postprocess_list(preds, sizes, crop_masks=crop_masks, score_threshold=score_threshold, mask_format=None)
+    sel = [(j, i) for j, i in enumerate(res.live) if int(res.out[i][2].shape[0]) > 0]   # eval.py:405-406
+    if not sel:
+        return None
+    ph, pw, k = res.shape
+    images = []
+    for _, i in sel:
+        h, w = (int(v) for v in sizes[i])
+        images.append(_gt_image(gts[i], gt_masks[i], h, w, int(num_crowds[i]), num_classes, where))
+    # the ground truth: one pinned buffer, one H2D copy, one pack launch for every image's masks
+    lay = _gt_layout(images)
+    pinned = torch.empty(max(lay.nbytes, 16), dtype=torch.uint8, pin_memory=True)
+    on_device = _fill_gt(pinned, images, lay)
+    staged = pinned.to(dev, non_blocking=True)
+    for j in on_device:
+        im = images[j]
+        wpr = (im.w + 31) // 32
+        at = lay.mask_at + 32 * lay.words[j]
+        dst = staged[at:at + 32 * im.g_all * im.h * wpr].view(im.g_all, im.h, 32 * wpr)
+        dst[:, :, :im.w] = im.masks.to(dev).reshape(im.g_all, im.h, im.w).float() > 0.5
+    W = lay.words[-1] + images[-1].g_all * images[-1].h * ((images[-1].w + 31) // 32)
+    bits = pack_masks(staged[lay.mask_at:lay.mask_at + 32 * W].view(W, 32)) if W else staged[:4].view(torch.int32)
+    # the caches: one buffer, per image [box n*g | mask n*g | crowd box n*nc | crowd mask n*nc]
+    ns = [int(res.out[i][2].shape[0]) for _, i in sel]
+    sizes_c = [2 * n * im.g_all for n, im in zip(ns, images)]
+    caches = torch.empty(max(sum(sizes_c), 1), dtype=torch.float32, device=dev)
+    items = (_lib.YbEvalIouItem * len(sel))()
+    out, cls, box_s, mask_s, gt_cls = [], [], [], [], []
+    boxes_base = staged.data_ptr() + lay.box_at
+    cls_base = staged.data_ptr() + lay.cls_at
+    off = 0
+    for j, ((t, i), im, n) in enumerate(zip(sel, images, ns)):
+        g, nc = im.g_all - im.num_crowd, im.num_crowd
+        views = []
+        for m in (g, g, nc, nc):
+            views.append(caches[off:off + n * m].view(n, m))
+            off += n * m
+        pi = res.items[t]
+        items[j] = _lib.YbEvalIouItem(pi.proto, pi.coef, pi.box, res.out[i][2].data_ptr(),
+                                      bits.data_ptr() + 4 * lay.words[j], boxes_base + 16 * lay.rows[j],
+                                      *[v.data_ptr() if v.numel() else None for v in views], n, im.h, im.w, im.g_all,
+                                      nc)
+        out.append((i, n, g, nc) + tuple(views))
+        o = res.out[i]
+        cls.append(o[0].long().contiguous())
+        box_s.append((o[1][0] if isinstance(o[1], list) else o[1]).float().contiguous())
+        mask_s.append((o[1][1] if isinstance(o[1], list) else o[1]).float().contiguous())
+        gt_cls.append(cls_base + 4 * lay.rows[j])
+    # res.keep_alive holds the inputs res.items points at until this call has read them
+    _lib.check(_lib.load().yb_eval_iou_list(_ops_handle(dev, k), items, len(sel), ph, pw, k, 1 if crop_masks else 0,
+                                            _lib.current_stream(dev)), "yb_eval_iou_list")
+    return _IouList(out, cls, box_s, mask_s, gt_cls, [res.keep_alive, staged, bits, caches, pinned])
+
+
+def _match_list(ap_data, lst):
+    """One yb_eval_match_list call over _iou_list's images: records behind ap_data's, counts into ap_data."""
+    dev = ap_data._device
+    T = len(ap_data.iou_thresholds)
+    total = sum(2 * T * im[1] for im in lst.images)
+    ap_data._reserve(total)
+    items = (_lib.YbEvalMatchItem * len(lst.images))()
+    at = ap_data._n
+    ptr = lambda v: v.data_ptr() if v.numel() else None
+    for j, (im, cls, bs, ms, gc) in enumerate(zip(lst.images, lst.cls, lst.box_s, lst.mask_s, lst.gt_cls)):
+        _, n, g, nc, box_iou, m_iou, crowd_box, crowd_mask = im
+        items[j] = _lib.YbEvalMatchItem(ptr(box_iou), ptr(m_iou), ptr(crowd_box), ptr(crowd_mask), cls.data_ptr(),
+                                        bs.data_ptr(), ms.data_ptr(), gc if g else None, gc + 4 * g if nc else None,
+                                        at, n, g, nc)
+        at += 2 * T * n
+    _lib.check(_lib.load().yb_eval_match_list(_ops_handle(dev), items, len(lst.images), ap_data._thr, T,
+                                              ap_data.num_classes, _lib.ptr(ap_data._score), _lib.ptr(ap_data._tag),
+                                              _lib.ptr(ap_data._counts), _lib.ptr(ap_data._err),
+                                              _lib.current_stream(dev)), "yb_eval_match_list")
+    ap_data._n += total
+
+
+def prep_metrics_list(ap_data, preds, sizes, gts, gt_masks, num_crowds, *, crop_masks=True, score_threshold=0.0):
+    """prep_metrics (eval.py:386-510) for a list of images, straight from the detections: fills ap_data exactly as
+    [prep_metrics(ap_data, [p], None, gts[i], gt_masks[i], h_i, w_i, num_crowds[i], i) for i, p in enumerate(preds)]
+    would, image i at sizes[i] = (h_i, w_i).  preds: Yolact's output list (one {'net', 'detection'} per image);
+    gts [g,5] (relative x1y1x2y2 + class, crowds last), gt_masks [g,h,w] and num_crowds per image, in the dataset's form.
+
+    postprocess_list gives the classes, scores (YOLACT++'s [box, mask] included) and pixel boxes without assembling
+    masks; the ground truth of every image goes to the device in one pinned buffer and one H2D copy and is packed in
+    one launch; ONE yb_eval_iou_list launch computes every image's four IoU caches from the prototypes, and ONE
+    yb_eval_match_list launch runs the matching of every image.  No host sync at score_threshold == 0
+    (postprocess_list's one at score_threshold > 0).  ValueError, before anything is added, for lists of different
+    lengths, a ground-truth class outside [0, C), num_crowd outside [0, g], gt_masks of the wrong shape, detections
+    without masks (cfg.eval_mask_branch off) and detections on another device than ap_data."""
+    lst = _iou_list(ap_data.num_classes, ap_data._device, preds, sizes, gts, gt_masks, num_crowds, crop_masks,
+                    score_threshold)
+    if lst is not None:
+        _match_list(ap_data, lst)
 
 
 def calc_map(ap_data, print_table=True):
