@@ -280,6 +280,150 @@ def gen_detect_unit(seed=3):
     npz_save("detect_unit", **out)
 
 
+# Detect at its parameter edges: (C, P) fixtures, and per case (C, mode, top_k, max_dets, nms_thresh, conf_thresh,
+# mask_dim).  C = 2 leaves the fg-max loop empty, 96 fills K1's default 48 KB tile, 129 is the declared limit.
+DETECT_EDGE_P = {2: 400, 21: 200, 96: 64, 129: 64}
+DETECT_EDGE_MODES = ("fast", "cc", "trad")
+
+
+def detect_edge_cases():
+    cases = []
+    for ci, C in enumerate(DETECT_EDGE_P):
+        for mi, mode in enumerate(DETECT_EDGE_MODES):
+            for ki, top_k in enumerate((1, 7, 256)):
+                if mode == "trad":
+                    max_dets = 100 if top_k >= 100 else 1            # traditional NMS needs max_dets <= top_k
+                else:
+                    max_dets = (1, 100)[(ci + mi + ki) % 2]
+                cases.append((C, mode, top_k, max_dets, (0.3, 0.5, 0.7)[(ci + ki) % 3],
+                              (0.05, 0.5)[(ci + mi + ki) % 2], (1, 33)[(mi + ki) % 2]))
+    return cases
+
+
+def detect_edge_inputs(C, P, seed):
+    """B = 3 images; the middle one has no candidate at any threshold.  Every value is a short dyadic fraction drawn
+    with RandomState, which keeps the file small: probabilities k / 2^20 (foreground below 0.046, or in a prior's "hot"
+    class from 0.05 up, all distinct within an image), loc k / 128, priors k / 4096, coefficients k / 4 with a distinct
+    first column.  Every other prior has loc[:, 2:] == 0, so its box decodes with expf(0) = 1 in round-to-nearest
+    arithmetic only.  Image 0 holds four rows whose best foreground probability is exactly float32(t) or the next
+    float up, for t in (0.05, 0.5)."""
+    r = np.random.RandomState(seed)
+    B, K = 3, 33
+    q = np.float32(2.0 ** -20)
+    priors = np.concatenate([r.randint(410, 3687, (P, 2)), r.randint(205, 1639, (P, 2))], 1).astype(np.float32) / 4096
+    loc = (r.randint(-64, 65, (B, P, 4)) / 128).astype(np.float32)
+    loc[:, ::2, 2:] = 0
+    hot = r.rand(B, P) < 0.3
+    hot[1] = False
+    hot[0, 3:11] = False
+    cls = r.randint(1, C, size=(B, P))
+    big_range = np.setdiff1d(np.arange(52800, 1 << 20), [1 << 19])    # 0.5 itself is a threshold row's value
+    conf = np.zeros((B, P, C), np.float32)
+    for b in range(B):
+        conf[b, :, 0] = r.randint(0, 1 << 20, P) * q
+        small = r.choice(48000, (P, C - 1), replace=False)
+        big = r.choice(big_range, (P, C - 1), replace=False)
+        conf[b, :, 1:] = np.where(hot[b, :, None] & (cls[b, :, None] == np.arange(1, C)), big, small) * q
+    for j, t in enumerate((0.05, 0.05, 0.5, 0.5)):
+        v = np.float32(t) if j % 2 == 0 else np.nextafter(np.float32(t), np.float32(1))
+        conf[0, 3 + 2 * j, 1 + (j * 7) % (C - 1)] = v
+    mask = (r.randint(-4, 5, (B, P, K)) / 4).astype(np.float32)
+    for b in range(B):
+        mask[b, :, 0] = (r.choice(1 << 16, P, replace=False) - (1 << 15)) / np.float32(1 << 15)
+    return loc, conf, mask, priors
+
+
+def detect_nan_inputs(seed=13):
+    """NaN inputs, one image, C = 21: prior 5 has a NaN probability at class 7 (its max, 0.9 at class 1, is above
+    every threshold) and prior 6 one at class 1 (0.8 at class 4); the rows of priors 9 and 12 are strong class-3
+    candidates whose loc is NaN (all four values, and x only), ranked between other class-3 boxes."""
+    r = np.random.RandomState(seed)
+    P, C, K = 64, 21, 8
+    priors = np.concatenate([r.uniform(0.2, 0.8, (P, 2)), r.uniform(0.1, 0.5, (P, 2))], 1).astype(np.float32)
+    loc = (r.standard_normal((1, P, 4)) * 0.3).astype(np.float32)
+    logits = (r.standard_normal((1, P, C)) * 1.5).astype(np.float32)
+    logits[0, :, 0] += 1.0
+    logits[0, 20:40, 3] += r.uniform(2.0, 6.0, 20).astype(np.float32)
+    conf = to_np(torch.softmax(torch.from_numpy(logits), -1))
+    conf[0, 5] = r.uniform(1e-4, 1e-2, C).astype(np.float32)
+    conf[0, 5, 1], conf[0, 5, 7] = 0.9, np.nan
+    conf[0, 6] = r.uniform(1e-4, 1e-2, C).astype(np.float32)
+    conf[0, 6, 4], conf[0, 6, 1] = 0.8, np.nan
+    ranked = np.sort(conf[0, 20:40, 3])[::-1]
+    for p, j in ((9, 4), (12, 11)):
+        conf[0, p, 3] = (ranked[j] + ranked[j + 1]) / np.float32(2)     # strictly between two class-3 scores
+        loc[0, p, :] = np.nan if p == 9 else [np.nan, 0, 0, 0]
+    mask = r.standard_normal((1, P, K)).astype(np.float32)
+    return loc, conf, mask, priors
+
+
+def _assert_no_ties(conf, keep_scores, conf_thresh):
+    """torch.sort is unstable: a golden fixture may not hold equal scores within a class among the candidates, nor
+    among the returned rows."""
+    for b in range(conf.shape[0]):
+        cur = conf[b, :, 1:]
+        with np.errstate(invalid="ignore"):
+            cand = cur.max(axis=1) > np.float32(conf_thresh)
+        for c in range(cur.shape[1]):
+            col = cur[cand, c]
+            col = col[~np.isnan(col)]
+            assert np.unique(col).size == col.size, ("tie within a class", b, c)
+    for s in keep_scores:
+        assert np.unique(s).size == s.size, "tie among kept rows"
+
+
+def gen_detect_edges():
+    """The reference Detect (fast_nms, cc_fast_nms, traditional_nms through the reference's cython_nms) on CPU at the
+    parameter edges of DETECT_EDGE_P / detect_edge_cases, and on the NaN inputs of detect_nan_inputs."""
+    from data.config import cfg, set_cfg
+    from layers import Detect
+    set_cfg("yolact_base_config")
+    install_cython_nms()
+    out = {}
+
+    def run(tag, loc, conf, mask, priors, C, mode, top_k, max_dets, nms, conf_thresh, md):
+        cfg.max_num_detections = max_dets
+        cfg.max_size = 550
+        d = Detect(C, bkg_label=0, top_k=top_k, conf_thresh=conf_thresh, nms_thresh=nms)
+        d.use_fast_nms = mode != "trad"
+        d.use_cross_class_nms = mode == "cc"
+        res = d({"loc": torch.from_numpy(loc), "conf": torch.from_numpy(conf),
+                 "mask": torch.from_numpy(np.ascontiguousarray(mask[..., :md])), "priors": torch.from_numpy(priors)},
+                None)
+        counts, kept = [], []
+        for b, r in enumerate(res):
+            det = r["detection"]
+            counts.append(0 if det is None else int(det["score"].shape[0]))
+            if det is None:
+                continue
+            for k in ("box", "mask", "class", "score"):
+                out["%s_%d_%s" % (tag, b, k)] = to_np(det[k])
+            kept.append(to_np(det["score"]))
+        out[tag + "_counts"] = np.array(counts, np.int32)
+        _assert_no_ties(conf, kept, conf_thresh)
+        return counts
+
+    for ci, (C, P) in enumerate(DETECT_EDGE_P.items()):
+        loc, conf, mask, priors = detect_edge_inputs(C, P, 100 + ci)
+        out.update({"C%d_loc" % C: loc, "C%d_conf" % C: conf, "C%d_mask" % C: mask, "C%d_priors" % C: priors})
+    cases = detect_edge_cases()
+    out["cases"] = np.array([(C, DETECT_EDGE_MODES.index(m), k, d, n, t, md) for C, m, k, d, n, t, md in cases],
+                            np.float64)
+    for i, (C, mode, top_k, max_dets, nms, conf_thresh, md) in enumerate(cases):
+        g = {k: out["C%d_%s" % (C, k)] for k in ("loc", "conf", "mask", "priors")}
+        counts = run("case%d" % i, g["loc"], g["conf"], g["mask"], g["priors"], C, mode, top_k, max_dets, nms,
+                     conf_thresh, md)
+        print("detect_edges case %d C=%d %s top_k=%d max_dets=%d nms=%.1f conf=%.2f mask_dim=%d counts" %
+              (i, C, mode, top_k, max_dets, nms, conf_thresh, md), counts)
+    loc, conf, mask, priors = detect_nan_inputs()
+    out.update({"nan_loc": loc, "nan_conf": conf, "nan_mask": mask, "nan_priors": priors})
+    for mode in DETECT_EDGE_MODES:
+        counts = run("nan_" + mode, loc, conf, mask, priors, 21, mode, 200, 100, 0.5, 0.05, 8)
+        print("detect_edges nan", mode, counts)
+    cfg.max_num_detections = 100
+    npz_save("detect_edges", **out)
+
+
 def gen_postprocess_unit(seed=5):
     from data.config import cfg, set_cfg
     from layers.output_utils import postprocess
@@ -520,6 +664,8 @@ if __name__ == "__main__":
         gen_detect_unit()
         gen_postprocess_unit()
         gen_dcn_unit()
+    if "detect_edges" in which:
+        gen_detect_edges()
     if "units" in which or "eval" in which:
         gen_eval_unit()
     if "full" in which:

@@ -20,6 +20,9 @@
 //
 // All score / box arithmetic uses round-to-nearest intrinsics so nvcc cannot contract a*b+c into
 // FMA: given identical inputs the keep decisions are the reference's, up to expf's last ulp.
+// Scores are ordered by their float bits, which order non-negative floats only: negative or -0.0
+// "probabilities" are outside the contract (a softmax cannot produce them).  A prior with a NaN
+// foreground score is no candidate, as torch.max propagates NaN into the reference's threshold test.
 #include "kernels.cuh"
 
 namespace yb {
@@ -27,6 +30,7 @@ namespace yb {
 namespace {
 
 constexpr int K1_ROWS = 128;   // priors per CTA in K1
+constexpr int K1_HEADER_BYTES = 32;   // K1's warp counts and block base, ahead of its [K1_ROWS][C] tile
 constexpr int NT2 = 256;       // threads in K2 / K3
 constexpr int SORT_N = 256;    // bitonic sort width (>= top_k)
 constexpr int HIST_BINS = 2048;
@@ -39,9 +43,11 @@ detect_candidates_kernel(const float* __restrict__ conf, int64_t P, int C, int i
                          float conf_thresh, int cross_class, float* __restrict__ scoresT,
                          int32_t* __restrict__ cand_prior, int32_t* __restrict__ cand_cls,
                          int32_t* __restrict__ cand_count) {
-  extern __shared__ float tile[];  // [K1_ROWS][C]
-  __shared__ int warp_cnt[K1_ROWS / 32];
-  __shared__ int s_base;
+  // all of K1's shared memory is dynamic, so the launch's size is the whole footprint
+  extern __shared__ __align__(16) unsigned char k1_smem[];
+  int* warp_cnt = reinterpret_cast<int*>(k1_smem);                    // [K1_ROWS / 32]
+  int& s_base = warp_cnt[K1_ROWS / 32];
+  float* tile = reinterpret_cast<float*>(k1_smem + K1_HEADER_BYTES);   // [K1_ROWS][C]
 
   const int b = blockIdx.y;
   const int64_t p0 = (int64_t)blockIdx.x * K1_ROWS;
@@ -67,15 +73,20 @@ detect_candidates_kernel(const float* __restrict__ conf, int64_t P, int C, int i
       }
       for (int c = 0; c < C; ++c) row[c] = __fdiv_rn(row[c], s);
     }
-    // max over foreground classes (detection.py:83-84); first max wins like torch.max
+    // max over foreground classes (detection.py:83-84); first max wins like torch.max, and a NaN
+    // anywhere makes torch.max NaN, which fails `> conf_thresh`
     best = row[1];
     best_c = 0;
-    for (int c = 2; c < C; ++c)
-      if (row[c] > best) {
-        best = row[c];
+    bool nan = best != best;
+    for (int c = 2; c < C; ++c) {
+      const float v = row[c];
+      nan |= v != v;
+      if (v > best) {
+        best = v;
         best_c = c - 1;
       }
-    keep = best > conf_thresh;
+    }
+    keep = !nan && best > conf_thresh;
   }
   // block-level ordered compaction
   unsigned bal = __ballot_sync(0xffffffffu, keep);
@@ -286,8 +297,19 @@ class_nms_kernel(const float* __restrict__ scoresT, const int32_t* __restrict__ 
   const int b = blockIdx.y;
   const int tid = threadIdx.x;
   const int M = cand_count[b];
+  // CC: output rows [n, max_out) are zero, as final_select_kernel leaves them (max_out <= NT2)
+  auto cc_zero_rows_from = [&](int n) {
+    if (tid >= n && tid < max_out) {
+      const int64_t o = (int64_t)b * max_out + tid;
+      reinterpret_cast<float4*>(out_box)[o] = make_float4(0.f, 0.f, 0.f, 0.f);
+      out_score[o] = 0.f;
+      out_cls[o] = 0;
+      for (int k = 0; k < mask_dim; ++k) out_coef[o * mask_dim + k] = 0.f;
+    }
+  };
   if (M == 0) {
     if (CC) {
+      cc_zero_rows_from(0);
       if (tid == 0) out_count[b] = 0;
     } else if (tid == 0) {
       pool_n[b * (C - 1) + c] = 0;
@@ -346,6 +368,7 @@ class_nms_kernel(const float* __restrict__ scoresT, const int32_t* __restrict__ 
       const float* src = coef + ((int64_t)b * P + prior) * mask_dim;
       for (int k = 0; k < mask_dim; ++k) out_coef[o * mask_dim + k] = src[k];
     }
+    cc_zero_rows_from(min(total, max_out));
     if (tid == 0) out_count[b] = min(total, max_out);
   }
 }
@@ -579,8 +602,11 @@ void launch_detect(const DetectParams& dp, const float* loc, const float* conf, 
   YB_CHECK_CUDA(cudaMemsetAsync(ws.cand_count, 0, sizeof(int32_t) * B, stream));
   {
     dim3 grid((unsigned)ceil_div64(dp.P, K1_ROWS), B);
-    size_t smem = (size_t)K1_ROWS * C * sizeof(float);
-    YB_REQUIRE(smem <= 48 * 1024, "detect: num_classes too large for the K1 tile");
+    const size_t smem = K1_HEADER_BYTES + (size_t)K1_ROWS * C * sizeof(float);
+    // past the 48 KB a launch gets by default (C >= 96) the kernel must opt in: 66 KB at C = 129
+    if (smem > 48 * 1024)
+      YB_CHECK_CUDA(cudaFuncSetAttribute(detect_candidates_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem));
     detect_candidates_kernel<<<grid, K1_ROWS, smem, stream>>>(
         conf, dp.P, C, dp.conf_is_logits, dp.conf_thresh, dp.cross_class == YB_NMS_CROSS_CLASS ? 1 : 0, ws.scoresT,
         ws.cand_prior,
