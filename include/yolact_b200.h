@@ -51,6 +51,8 @@
  *   yb_conv2d          <- nn.Conv2d + folded BatchNorm2d + activation (+ residual), op-level test hook
  *   yb_conv2d_ex       <- the same with the network's other epilogues (residual after the activation, fp32 output,
  *                         zero-padded channels, the fused prediction head) and the tensor-core stem, op-level test hook
+ *   yb_resample_ex     <- nn.MaxPool2d(3, 2, 1) (backbone.py:80) and F.interpolate bilinear (+ lateral, + ReLU) of the
+ *                         FPN (yolact.py:332) and protonet (utils/functions.py:194), op-level test hook
  */
 #ifndef YOLACT_B200_H_
 #define YOLACT_B200_H_
@@ -296,7 +298,8 @@ YB_API int yb_coco_rle_list(yb_handle* h, const yb_post_item* h_items, int B, in
                             int32_t* d_row_len, int64_t* d_need, void* stream);
 
 /* maskiou_net on [n,1,ph,pw] fp32 masks -> d_maskiou [n] = net(mask)[i, cls[i]];
- * d_cls == NULL: d_maskiou [n, num_classes-1] = net(mask) (FastMaskIoUNet.forward itself). */
+ * d_cls == NULL: d_maskiou [n, num_classes-1] = net(mask) (FastMaskIoUNet.forward itself).
+ * ph and pw must be >= 63, the smallest mask its five unpadded 3x3/2 convs accept (YB_ERR_INVALID otherwise). */
 YB_API int yb_maskiou(yb_handle* h, const float* d_proto_masks, int n, int ph, int pw,
                const int64_t* d_cls, float* d_maskiou, void* stream);
 
@@ -553,6 +556,20 @@ typedef struct {
 YB_API int yb_conv2d_ex(yb_handle* h, const float* d_x, const float* h_w, const float* h_bias,
                         const float* d_residual, void* d_y, int B, int Ci, int H, int W, int Co, int kh, int kw,
                         int stride, int pad, int act, int precision, const yb_conv_opts* opts, void* stream);
+
+/* One launch of the network's max pool or bilinear resample (test hook), in the kernels' own layout: d_x [B,H,W,C],
+ * d_add (nullable) and d_y [B,Ho,Wo,C] are NHWC device buffers, 16-byte aligned, of fp32 (precision 0), fp16
+ * (precision 1) or hi / lo fp16 pairs [.., hi(C) | lo(C)] whose value is hi + lo * 2^-11 (precision 3).
+ *   YB_RESAMPLE_MAXPOOL:  3x3 / stride 2 / pad 1 with -inf padding (nn.MaxPool2d); Ho = (H - 1) / 2 + 1 (likewise Wo),
+ *                         no add, no relu.
+ *   YB_RESAMPLE_BILINEAR: F.interpolate(size=(Ho, Wo), mode='bilinear', align_corners=False), + add, then ReLU when
+ *                         relu; the scale is in / out, as the network's FPN and protonet resamples use it.
+ * YB_ERR_INVALID, with nothing launched, for another op or precision, C not a multiple of 4 (fp32) or 8 (fp16), or a
+ * max pool with another output size, an add or relu.  Asynchronous on `stream`. */
+#define YB_RESAMPLE_MAXPOOL 0
+#define YB_RESAMPLE_BILINEAR 1
+YB_API int yb_resample_ex(yb_handle* h, int op, int precision, const void* d_x, const void* d_add, void* d_y, int B,
+                          int H, int W, int C, int Ho, int Wo, int relu, void* stream);
 
 /* ---- introspection ----------------------------------------------------------------------------- */
 /* Kernel launches issued by this handle since creation (bench.py's gpu_launches). */

@@ -152,6 +152,7 @@ YB_MASK_F32, YB_MASK_U8, YB_MASK_BITS = 0, 1, 2
 YB_NMS_FAST, YB_NMS_CROSS_CLASS, YB_NMS_TRADITIONAL = 0, 1, 2
 YB_NMS_FLAG_SECOND_THRESHOLD = 0x100
 YB_XFORM_NORMALIZE, YB_XFORM_SUBTRACT_MEANS, YB_XFORM_TO_FLOAT, YB_XFORM_NONE = 0, 1, 2, 3
+YB_RESAMPLE_MAXPOOL, YB_RESAMPLE_BILINEAR = 0, 1
 
 # name -> (restype, argtypes); kept in one table so tests can check that every symbol the header
 # declares is exported by the library.
@@ -216,6 +217,7 @@ SIGNATURES = {
                   [POINTER(c_float), c_void_p]),
     "yb_conv2d_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 11 +
                      [POINTER(YbConvOpts), c_void_p]),
+    "yb_resample_ex": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 7 + [c_void_p]),
     "yb_launch_count": (c_int64, [c_void_p]),
     "yb_set_profiling": (c_int, [c_void_p, c_int]),
     "yb_last_forward_ms": (c_int, [c_void_p, POINTER(c_float), POINTER(c_float)]),

@@ -584,7 +584,8 @@ int yb_maskiou(yb_handle* h, const float* d_proto_masks, int n, int ph, int pw, 
   if (n <= 0) return YB_OK;
   CallGuard g(h, (cudaStream_t)stream);   // shared workspaces: ordered behind the previous call
   cudaStream_t s = (cudaStream_t)stream;
-  // FastMaskIoUNet (yolact.py:363-375, config.py:785-789): 5x (3x3 s2 p0 + ReLU), 1x1 + ReLU, global max
+  // FastMaskIoUNet (yolact.py:363-375, config.py:785-789): 5x (3x3 s2 p0 + ReLU), 1x1 + ReLU, global max.  A mask
+  // needs 63 pixels on each axis (nn.Conv2d refuses anything smaller: the fifth conv would get fewer than 3 rows).
   const char* idx[6] = {"0", "2", "4", "6", "8", "10"};
   int H = ph, W = pw, C = 1;
   size_t need = 0;
@@ -593,8 +594,9 @@ int yb_maskiou(yb_handle* h, const float* d_proto_masks, int n, int ph, int pw, 
     for (int i = 0; i < 6; ++i) {
       ConvW& cw = h->convs[std::string("maskiou_net.maskiou_net.") + idx[i]];
       int k = cw.KH, st = (i < 5) ? 2 : 1;
-      hh = (hh - k) / st + 1;
-      ww = (ww - k) / st + 1;
+      hh = conv_out(hh, k, st, 0);
+      ww = conv_out(ww, k, st, 0);
+      YB_REQUIRE(hh >= 1 && ww >= 1, "yb_maskiou: mask too small for the network (63 x 63 at least)");
       need = std::max(need, (size_t)n * hh * ww * cw.Cout * 4);
     }
   }
@@ -613,8 +615,8 @@ int yb_maskiou(yb_handle* h, const float* d_proto_masks, int n, int ph, int pw, 
     p.KW = cw.KW;
     p.stride = (i < 5) ? 2 : 1;
     p.pad = 0;
-    p.Ho = (H - cw.KH) / p.stride + 1;
-    p.Wo = (W - cw.KW) / p.stride + 1;
+    p.Ho = conv_out(H, cw.KH, p.stride, 0);
+    p.Wo = conv_out(W, cw.KW, p.stride, 0);
     YB_REQUIRE(p.Ho >= 1 && p.Wo >= 1, "yb_maskiou: mask too small for the network");
     p.Cout = cw.Cout;
     p.act = ACT_RELU;
@@ -928,7 +930,7 @@ int yb_conv2d(yb_handle* h, const float* d_x, const float* h_w, const float* h_b
   const int sp = (precision == 3) ? 1 : 0;
   CallGuard g(h);
   cudaStream_t s = (cudaStream_t)stream;
-  const int Ho = (H + 2 * pad - kh) / stride + 1, Wo = (W + 2 * pad - kw) / stride + 1;
+  const int Ho = conv_out(H, kh, stride, pad), Wo = conv_out(W, kw, stride, pad);
   YB_REQUIRE(Ho >= 1 && Wo >= 1, "yb_conv2d: empty output");
   TempPool tp;
   const bool f16 = precision != 0;
@@ -1037,7 +1039,7 @@ int yb_conv2d_ex(yb_handle* h, const float* d_x, const float* h_w, const float* 
   YB_REQUIRE(ps == CoP || (y_f32 && ps > Co && o.nseg == 0), "yb_conv2d_ex: y_pix_stride needs an fp32 output and >= Co");
   CallGuard g(h);
   cudaStream_t s = (cudaStream_t)stream;
-  const int Ho = (H + 2 * pad - kh) / stride + 1, Wo = (W + 2 * pad - kw) / stride + 1;
+  const int Ho = conv_out(H, kh, stride, pad), Wo = conv_out(W, kw, stride, pad);
   YB_REQUIRE(Ho >= 1 && Wo >= 1, "yb_conv2d_ex: empty output");
   if (o.poison && o.nseg == 0)
     YB_CHECK_CUDA(cudaMemsetAsync(d_y, 0xff, (size_t)B * Ho * Wo * (y_f32 ? 4 * ps : sp ? 4 * CoP : 2 * CoP), s));
@@ -1140,6 +1142,41 @@ int yb_conv2d_ex(yb_handle* h, const float* d_x, const float* h_w, const float* 
     launch_simt_conv(p, wd, precision == 2 ? SIMT_F16 : SIMT_F32, s, &h->lc);
   }
   YB_CHECK_CUDA(cudaStreamSynchronize(s));  // temporaries are freed on return
+  YB_API_END
+}
+
+int yb_resample_ex(yb_handle* h, int op, int precision, const void* d_x, const void* d_add, void* d_y, int B, int H,
+                   int W, int C, int Ho, int Wo, int relu, void* stream) {
+  YB_API_BEGIN
+  YB_REQUIRE(h && d_x && d_y, "yb_resample_ex: null argument");
+  YB_REQUIRE(op == YB_RESAMPLE_MAXPOOL || op == YB_RESAMPLE_BILINEAR, "yb_resample_ex: unknown op");
+  YB_REQUIRE(precision == 0 || precision == 1 || precision == 3, "yb_resample_ex: precision must be 0, 1 or 3");
+  YB_REQUIRE(B >= 1 && H >= 1 && W >= 1 && C >= 1 && Ho >= 1 && Wo >= 1, "yb_resample_ex: empty shape");
+  YB_REQUIRE(C % (precision == 0 ? 4 : 8) == 0, "yb_resample_ex: C must be a multiple of the vector width (4 fp32, 8 fp16)");
+  auto aligned = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
+  YB_REQUIRE(aligned(d_x) && aligned(d_add) && aligned(d_y), "yb_resample_ex: buffers must be 16-byte aligned");
+  YB_REQUIRE(on_handle_device(h, d_x) && on_handle_device(h, d_add) && on_handle_device(h, d_y),
+             "yb_resample_ex: a pointer is not device memory of the handle's device");
+  if (op == YB_RESAMPLE_MAXPOOL)
+    YB_REQUIRE(Ho == conv_out(H, 3, 2, 1) && Wo == conv_out(W, 3, 2, 1) && !d_add && !relu,
+               "yb_resample_ex: the max pool is 3x3/2 pad 1 (Ho = (H - 1) / 2 + 1) and takes no add or relu");
+  CallGuard g(h, (cudaStream_t)stream);
+  cudaStream_t s = (cudaStream_t)stream;
+  const int sp = precision == 3 ? 1 : 0;
+  if (op == YB_RESAMPLE_MAXPOOL) {
+    if (precision == 0)
+      launch_maxpool3x3s2<float>((const float*)d_x, (float*)d_y, B, H, W, C, Ho, Wo, s, &h->lc);
+    else
+      launch_maxpool3x3s2<__half>((const __half*)d_x, (__half*)d_y, B, H, W, C, Ho, Wo, s, &h->lc, sp);
+  } else {
+    const float sh = bilinear_scale(H, Ho), sw = bilinear_scale(W, Wo);
+    if (precision == 0)
+      launch_upsample_bilinear<float>((const float*)d_x, (const float*)d_add, (float*)d_y, B, H, W, C, Ho, Wo, sh, sw,
+                                      relu ? 1 : 0, s, &h->lc);
+    else
+      launch_upsample_bilinear<__half>((const __half*)d_x, (const __half*)d_add, (__half*)d_y, B, H, W, C, Ho, Wo, sh,
+                                       sw, relu ? 1 : 0, s, &h->lc, sp);
+  }
   YB_API_END
 }
 

@@ -108,8 +108,6 @@ void launch_multi_copy(const void* const* src, void* const* dst, const size_t* b
 // ---------------------------------------------------------------------------------------------
 // feature-map sizes and priors (PredictionModule.make_priors, yolact.py:214-263)
 // ---------------------------------------------------------------------------------------------
-static int conv_out(int h, int k, int s, int p) { return (h + 2 * p - k) / s + 1; }
-
 void compute_level_sizes(const yb_config& cfg, int H, int W, int level_hw[5][2], int* ph, int* pw) {
   int hs[8], ws[8];
   int n = 0;
@@ -796,9 +794,9 @@ void build_network(yb_handle* h, Executor* ex, bool dry) {
   // lat_layers / pred_layers are stored in reverse: index 0 <-> deepest level (yolact.py:286-289,324-341)
   Act x5 = nb.conv("fpn.lat_layers.0", "", C[2], 1, 1, 0, ACT_NONE);
   Act l4 = nb.conv("fpn.lat_layers.1", "", C[1], 1, 1, 0, ACT_NONE);
-  Act x4 = nb.upsample(x5, l4.H, l4.W, (float)x5.H / (float)l4.H, (float)x5.W / (float)l4.W, &l4, 0);
+  Act x4 = nb.upsample(x5, l4.H, l4.W, bilinear_scale(x5.H, l4.H), bilinear_scale(x5.W, l4.W), &l4, 0);
   Act l3 = nb.conv("fpn.lat_layers.2", "", C[0], 1, 1, 0, ACT_NONE);
-  Act x3 = nb.upsample(x4, l3.H, l3.W, (float)x4.H / (float)l3.H, (float)x4.W / (float)l3.W, &l3, 0);
+  Act x3 = nb.upsample(x4, l3.H, l3.W, bilinear_scale(x4.H, l3.H), bilinear_scale(x4.W, l3.W), &l3, 0);
   Act Pl[5];
   Pl[2] = nb.conv("fpn.pred_layers.0", "", x5, 3, 1, 1, ACT_RELU);
   Pl[1] = nb.conv("fpn.pred_layers.1", "", x4, 3, 1, 1, ACT_RELU);
@@ -814,7 +812,8 @@ void build_network(yb_handle* h, Executor* ex, bool dry) {
     Act p = nb.conv("proto_net.0", "", Pl[0], 3, 1, 1, ACT_RELU);
     p = nb.conv("proto_net.2", "", p, 3, 1, 1, ACT_RELU);
     p = nb.conv("proto_net.4", "", p, 3, 1, 1, ACT_RELU);
-    p = nb.upsample(p, p.H * 2, p.W * 2, 0.5f, 0.5f, nullptr, 1);  // InterpolateModule(scale_factor=2) + ReLU
+    // InterpolateModule(scale_factor=2) + ReLU
+    p = nb.upsample(p, p.H * 2, p.W * 2, bilinear_scale(p.H, p.H * 2), bilinear_scale(p.W, p.W * 2), nullptr, 1);
     p = nb.conv("proto_net.8", "", p, 3, 1, 1, ACT_RELU);
     // 1x1 -> mask_dim, then mask_proto_prototype_activation = relu (yolact.py:589); NHWC fp32 == permute(0,2,3,1)
     p = nb.conv("proto_net.10", "", p, 1, 1, 0, ACT_RELU, nullptr, /*out_f32=*/true);

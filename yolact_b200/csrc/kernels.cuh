@@ -39,6 +39,11 @@ struct ConvProblem {
   float* seg_y[3] = {nullptr, nullptr, nullptr};
 };
 
+// Output size of a k-tap window with stride s and padding p over h inputs, as nn.Conv2d / nn.MaxPool2d compute it.  0
+// when the padded input is shorter than the window, which nn.Conv2d refuses: C's truncating division alone would give
+// 1 there (a 2-pixel input to a 3x3/2 conv), and the kernel would read the missing rows as zeros.
+inline int conv_out(int h, int k, int s, int p) { return h + 2 * p < k ? 0 : (h + 2 * p - k) / s + 1; }
+
 enum SimtTypes : int {
   SIMT_F32 = 0,        // x float (NHWC or NCHW), w float, y float
   SIMT_F16,            // x half, w half, y half (or float when y_f32)
@@ -114,6 +119,8 @@ void launch_maxpool3x3s2(const T* x, T* y, int B, int H, int W, int C, int Ho, i
                          cudaStream_t stream, LaunchCounter* lc, int split = 0);
 // y = bilinear(x -> [Ho,Wo], align_corners=False) (+ add), NHWC.  scale_h/scale_w are the
 // source/destination ratios PyTorch uses (in/out, or 1/scale_factor).  relu: clamp at 0.
+// The ratio F.interpolate(size=out) uses for in -> out; for out = 2 * in it is exactly 1 / scale_factor = 0.5.
+inline float bilinear_scale(int in, int out) { return (float)in / (float)out; }
 template <typename T>
 void launch_upsample_bilinear(const T* x, const T* add, T* y, int B, int H, int W, int C, int Ho,
                               int Wo, float scale_h, float scale_w, int relu, cudaStream_t stream,

@@ -147,8 +147,8 @@ void launch_t(const ConvProblem& p, const void* w, cudaStream_t stream) {
 void launch_simt_conv(const ConvProblem& p, const void* w, int types, cudaStream_t stream,
                       LaunchCounter* lc) {
   YB_REQUIRE(p.x && p.y && w, "simt_conv: null pointer");
-  YB_REQUIRE(p.Ho == (p.H + 2 * p.pad - p.KH) / p.stride + 1, "simt_conv: bad Ho");
-  YB_REQUIRE(p.Wo == (p.W + 2 * p.pad - p.KW) / p.stride + 1, "simt_conv: bad Wo");
+  YB_REQUIRE(p.Ho >= 1 && p.Ho == conv_out(p.H, p.KH, p.stride, p.pad), "simt_conv: bad Ho");
+  YB_REQUIRE(p.Wo >= 1 && p.Wo == conv_out(p.W, p.KW, p.stride, p.pad), "simt_conv: bad Wo");
   switch (types) {
     case SIMT_F32:
       launch_t<float, float, float>(p, w, stream);

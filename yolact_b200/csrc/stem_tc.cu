@@ -323,8 +323,8 @@ StemTcPlan* stem_tc_plan_create(const float* x_nchw, const __half* w_packed, con
   q.B = B;
   q.H = H;
   q.W = W;
-  q.Ho = (H + 2 * pad - ks) / stride + 1;
-  q.Wo = (W + 2 * pad - ks) / stride + 1;
+  q.Ho = conv_out(H, ks, stride, pad);
+  q.Wo = conv_out(W, ks, stride, pad);
   q.M = (long long)B * q.Ho * q.Wo;
   q.cpad = cpad > cout ? cpad : cout;
   YB_REQUIRE(q.cpad % 8 == 0, "stem_tc: the padded channel count must be a multiple of 8");

@@ -1048,7 +1048,7 @@ static void choose_tile(int Wov, int Hov, int& best_tw, int& best_th) {
 void tc_chain_debug_deps(int B, int Hin, int Win, int k, int stride, int pad, int producer_flat, int m, int32_t* out) {
   YB_REQUIRE(B >= 1 && Hin >= 1 && Win >= 1 && (k == 1 || k == 3) && (stride == 1 || stride == 2) && pad >= 0 && out,
              "chain_debug_deps: bad argument");
-  const int Ho = (Hin + 2 * pad - k) / stride + 1, Wo = (Win + 2 * pad - k) / stride + 1;
+  const int Ho = conv_out(Hin, k, stride, pad), Wo = conv_out(Win, k, stride, pad);
   YB_REQUIRE(Ho >= 1 && Wo >= 1, "chain_debug_deps: empty output");
   auto layer = [&](int flat, int H, int W, int s, int p, int kh) {
     ChainLayer c = {};
@@ -1079,8 +1079,8 @@ void tc_chain_debug_deps(int B, int Hin, int Win, int k, int stride, int pad, in
 
 TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, const TcTiling& want) {
   YB_REQUIRE(tc_conv_supported(p), "tc_conv: unsupported problem");
-  YB_REQUIRE(p.Ho == (p.H + 2 * p.pad - p.KH) / p.stride + 1, "tc_conv: bad Ho");
-  YB_REQUIRE(p.Wo == (p.W + 2 * p.pad - p.KW) / p.stride + 1, "tc_conv: bad Wo");
+  YB_REQUIRE(p.Ho >= 1 && p.Ho == conv_out(p.H, p.KH, p.stride, p.pad), "tc_conv: bad Ho");
+  YB_REQUIRE(p.Wo >= 1 && p.Wo == conv_out(p.W, p.KW, p.stride, p.pad), "tc_conv: bad Wo");
   auto* plan = new TcConvPlan();
   TcParams& q = plan->prm;
   memset(&q, 0, sizeof(q));
