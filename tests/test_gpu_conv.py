@@ -1,7 +1,8 @@
-"""Convolution kernels through the C ABI (yb_conv2d): SIMT fp32 vs torch fp32, tensor-core (wgmma) fp16 vs the SIMT
-fp16 kernel (same quantised operands, different summation order) and vs torch on fp16-rounded inputs."""
+"""Convolution kernels through the C ABI (yb_conv2d): SIMT fp32 vs torch fp32; tensor-core (wgmma) fp16 and the SIMT
+fp16 kernel element by element against float64 on the same fp16-rounded operands, and against each other; the split
+mode against float64 on the unrounded operands (the per-element bound of tests/conv_reference.py)."""
 import ctypes
-
+import functools
 import os
 
 import numpy as np
@@ -9,6 +10,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from tests.conv_reference import K_BOUND, UNIT, act_f64, check, conv_f64, f16, report_ratios  # noqa: F401
+from tests.error_bounds import worst
 from yolact_b200 import _lib
 
 pytestmark = pytest.mark.gpu
@@ -142,6 +145,27 @@ if os.environ.get("YB_TEST_NO_PAIR"):   # escape hatch while the pair kernel is 
     TC_MODES = {k: v for k, v in TC_MODES.items() if not k.startswith("pair")}
 
 
+@functools.lru_cache(maxsize=48)
+def reference(case, seed, rounded):
+    """float64 act(conv + bias + residual) of make(*case, seed) and its per-element scale, NHWC; rounded: on the
+    fp16-rounded x, w and residual the single-pass modes consume."""
+    B, Ci, H, W, Co, k, s, p, act, wr = case
+    x, w, bias, res = make(B, Ci, H, W, Co, k, s, p, True, wr, seed=seed)
+    x, w = x.numpy(), w.numpy()
+    res = None if res is None else res.numpy()
+    if rounded:
+        x, w, res = f16(x), f16(w), f16(res)
+    pre, scale = conv_f64(x, w, bias.numpy(), s, p)
+    if res is not None:
+        rn = res.transpose(0, 2, 3, 1).astype(np.float64)
+        pre, scale = pre + rn, scale + np.abs(rn)
+    return act_f64(pre, act), scale
+
+
+def nhwc(y):
+    return y.permute(0, 2, 3, 1).double().numpy()
+
+
 @pytest.mark.parametrize("mode", sorted(TC_MODES))
 @pytest.mark.parametrize("case", TC_CASES)
 def test_tcgen05_matches_simt_f16_and_torch(ops, case, mode, monkeypatch):
@@ -151,15 +175,15 @@ def test_tcgen05_matches_simt_f16_and_torch(ops, case, mode, monkeypatch):
     x, w, bias, res = make(B, Ci, H, W, Co, k, s, p, True, wr, seed=1)
     y_tc, _ = run_conv(ops, x, w, bias, res, s, p, act, 1)
     y_simt, _ = run_conv(ops, x, w, bias, res, s, p, act, 2)
-    # reference on the SAME fp16-rounded operands, fp32 math
-    xr, wr_ = x.half().float(), w.half().float()
-    rr = res.half().float() if res is not None else None
-    ref = ref_conv(xr, wr_, bias, rr, s, p, act)
-    scale = max(1.0, ref.abs().max().item())
-    assert torch.isfinite(y_tc).all()
-    # both round the result to fp16 (rel 2^-11): allow 2 ulp of the largest value + accumulation noise
-    assert (y_tc - ref).abs().max() < 3e-3 * scale, "tensor cores vs torch(fp16 operands)"
-    assert (y_tc - y_simt).abs().max() < 3e-3 * scale, "tensor cores vs SIMT fp16"
+    # both against float64 on the SAME fp16-rounded operands, element by element
+    ref, scale = reference(case, 1, True)
+    what = "%s %s" % (case, mode)
+    check(nhwc(y_tc), ref, scale, "f16tc", what)
+    check(nhwc(y_simt), ref, scale, "f16", what)
+    # and each other: two summation orders of the same products, each within its bound
+    tol = 2 * K_BOUND["f16tc"] * UNIT["f16tc"] * scale + 2 * 2.0 ** -24
+    err = np.abs(nhwc(y_tc) - nhwc(y_simt))
+    assert (err <= tol).all(), ("tensor cores vs SIMT fp16", worst(err, tol))
 
 
 # ---- split precision (YB_PREC_F16X3): fp16 hi+lo operand pairs, three MMA passes -> fp32-equivalent results -----
@@ -184,18 +208,14 @@ SPLIT_MODES = {
 @pytest.mark.parametrize("case", TC_CASES)
 def test_tcgen05_split_matches_torch_fp32(ops, case, mode, monkeypatch):
     """The reference arithmetic is fp32 (yolact.py:564-676 under eval.py:1077-1081): the split mode is compared with
-    torch fp32 on the UNROUNDED operands.  Tolerance 2e-5 of the output range: ~30x the fp32 summation-order noise
-    of a K = 2304 dot product, 100x below the single-pass fp16 mode's error."""
+    float64 on the UNROUNDED operands, element by element, within a few units of 2^-22 of each element's scale."""
     for k_, v_ in SPLIT_MODES[mode].items():
         monkeypatch.setenv(k_, v_)
     B, Ci, H, W, Co, k, s, p, act, wr = case
     x, w, bias, res = make(B, Ci, H, W, Co, k, s, p, True, wr, seed=2)
     y, _ = run_conv(ops, x, w, bias, res, s, p, act, 3)
-    ref = ref_conv(x, w, bias, res, s, p, act)
-    scale = max(1.0, ref.abs().max().item())
-    assert torch.isfinite(y).all()
-    err = (y - ref).abs().max().item()
-    assert err < 2e-5 * scale, "split tensor cores vs torch fp32: %.3e of range" % (err / scale)
+    ref, scale = reference(case, 2, False)
+    check(nhwc(y), ref, scale, "f16x3", "%s %s" % (case, mode))
 
 
 def test_tcgen05_split_small_and_large_magnitudes(ops):

@@ -10,11 +10,8 @@
   e. the tensor-core stem: one-hot "tap probe" weights that make every output channel one element of the patch (exactly
      known), and the layer shapes the network runs with the three input transforms' value ranges.
 
-Every element is judged against K * unit * scale, scale = conv(|x|, |w|) + |bias| + |residual| (the magnitude its
-rounding error is proportional to), never against the tensor's range.  The reference is float64 F.conv2d on the CPU;
-for the fp16 modes on the fp16-rounded x, w and residual, which the kernels consume.
+Every element is judged against the per-element float64 bound of tests/conv_reference.py.
 """
-import ctypes
 import functools
 
 import numpy as np
@@ -22,20 +19,11 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests.error_bounds import UNIT as _UNIT, worst
+from tests.conv_reference import (ACT_LEAKY, ACT_NONE, ACT_RELU, ACT_TANH, K_BOUND, ROUNDED, UNIT, act_f64, check,
+                                  conv_ex, conv_f64, decode, f16, hd, he, out_hw, report_ratios, set_mode)  # noqa: F401
 from yolact_b200 import _lib
 
 pytestmark = pytest.mark.gpu
-
-PRECISION = {"f32": 0, "f16tc": 1, "f16": 2, "f16x3": 3}     # yb_conv2d's precision argument
-UNIT = dict(_UNIT, f16=_UNIT["f16tc"])
-# f16tc / f16: the fp16 rounding of the output (|y| <= scale: 1 unit) + fp32 accumulation of exact fp16 products
-#              (random-signed, a small fraction of a unit).
-# f16x3:       hi+lo encodings of x, w and the output (1 unit each) + the dropped lo*lo product + fp32 accumulation.
-# f32:         sequential fp32 accumulation, random-signed (as tests/test_gpu_dcn_edges.py).
-K_BOUND = {"f16tc": 2.0, "f16": 2.0, "f16x3": 4.0, "f32": 8.0}
-ACT_NONE, ACT_RELU, ACT_TANH, ACT_LEAKY = 0, 1, 2, 3
-ROUNDED = ("f16tc", "f16")          # modes that consume fp16-rounded operands
 
 # tiling switches of the op-level hooks; stream-K only changes plans with the staged epilogue
 MODES = {
@@ -51,117 +39,12 @@ MODES = {
 HEAD_MODES = {"default": {}, "bn32": {"YB_CONV2D_BN": "32"}, "bn64": {"YB_CONV2D_BN": "64"},
               "bn128": {"YB_CONV2D_BN": "128"}, "bn256": {"YB_CONV2D_BN": "256"}, "epi2": {"YB_CONV2D_EPI": "2"}}
 
-RATIOS = {}   # precision -> largest err / (unit * scale) seen by this module
-
-
-@pytest.fixture(scope="module", autouse=True)
-def report_ratios():
-    yield
-    for prec in sorted(RATIOS):
-        print("largest err / (unit * scale), %s: %.3f" % (prec, RATIOS[prec]))
-
-
-@pytest.fixture(scope="module")
-def hd():
-    lib = _lib.load()
-    yc = _lib.YbConfig()
-    yc.backbone = _lib.YB_BACKBONE_NONE
-    yc.num_classes, yc.mask_dim, yc.precision = 81, 32, _lib.YB_PREC_F32
-    yc.nms_top_k, yc.nms_conf_thresh, yc.nms_thresh, yc.max_num_detections = 200, 0.05, 0.5, 100
-    h = ctypes.c_void_p()
-    _lib.check(lib.yb_create(ctypes.byref(yc), 0, ctypes.byref(h)), "yb_create")
-    yield lib, h
-    lib.yb_destroy(h)
-
-
-def set_mode(monkeypatch, env):
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
-
-
-def out_hw(H, W, k, stride, pad):
-    return (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
-
 
 def guarded(a, guard=1 << 16):
     """A device copy of `a` (fp32) between two bands of `guard` NaNs: a read outside the tensor poisons the output."""
     buf = torch.full((a.size + 2 * guard,), float("nan"), device="cuda")
     buf[guard:guard + a.size] = torch.from_numpy(np.ascontiguousarray(a, np.float32).ravel()).cuda()
     return buf[guard:guard + a.size].view(a.shape)
-
-
-def conv_ex(hd, x, w, bias, res, stride, pad, act, precision, opts=None):
-    """yb_conv2d_ex with the output buffer filled with NaN first; x [B, CiP, H, W] and res are numpy fp32 NCHW, w and
-    bias numpy fp32 (host).  Returns the raw output: NHWC fp32 [.., ps], fp16 [.., Cp] or hi|lo pairs [.., 2 Cp]."""
-    lib, h = hd
-    o = opts if opts is not None else _lib.YbConvOpts()
-    o.poison = 1
-    B, _, H, W = x.shape
-    Co, Ci, kh, kw = w.shape
-    Ho, Wo = out_hw(H, W, kh, stride, pad)
-    Cp = max(Co, o.cout_pad)
-    if precision == "f32" or o.y_f32:
-        y = torch.empty(B, Ho, Wo, o.y_pix_stride or Cp, device="cuda")
-    else:
-        y = torch.empty(B, Ho, Wo, (2 if precision == "f16x3" else 1) * Cp, device="cuda", dtype=torch.float16)
-    wc = np.ascontiguousarray(w, np.float32)
-    bc = None if bias is None else np.ascontiguousarray(bias, np.float32)
-    xd = x if torch.is_tensor(x) else torch.from_numpy(np.ascontiguousarray(x, np.float32)).cuda()
-    rd = None if res is None else torch.from_numpy(np.ascontiguousarray(res, np.float32)).cuda()
-    _lib.check(lib.yb_conv2d_ex(h, _lib.ptr(xd), wc.ctypes.data_as(ctypes.c_void_p),
-                                None if bc is None else bc.ctypes.data_as(ctypes.c_void_p), _lib.ptr(rd),
-                                _lib.ptr(None if o.nseg else y), B, Ci, H, W, Co, kh, kw, stride, pad, act,
-                                PRECISION[precision], ctypes.byref(o), _lib.current_stream()), "yb_conv2d_ex")
-    torch.cuda.synchronize()
-    return y
-
-
-def decode(y, precision, Cp):
-    """The raw NHWC output as float64 values [.., Cp]; a split pair is hi + lo * 2^-11 (common.cuh split_f32)."""
-    if precision == "f16x3" and y.dtype == torch.float16:
-        y = y.cpu().numpy().astype(np.float64)
-        return y[..., :Cp] + y[..., Cp:] * 2.0 ** -11
-    return y.cpu().numpy().astype(np.float64)[..., :Cp]
-
-
-def act_f64(y, act):
-    if act == ACT_RELU:
-        return np.maximum(y, 0)
-    if act == ACT_LEAKY:
-        return np.where(y > 0, y, 0.1 * y)
-    if act == ACT_TANH:
-        return np.tanh(y)
-    return y
-
-
-def f16(a):
-    return None if a is None else a.astype(np.float16).astype(np.float32)
-
-
-def conv_f64(x, w, bias, stride, pad):
-    """float64 conv and its magnitude conv(|x|, |w|) + |bias|, NHWC numpy."""
-    xd, wd = torch.from_numpy(x).double(), torch.from_numpy(w).double()
-    bd = None if bias is None else torch.from_numpy(bias).double()
-    y = F.conv2d(xd, wd, bd, stride=stride, padding=pad)
-    s = F.conv2d(xd.abs(), wd.abs(), None if bd is None else bd.abs(), stride=stride, padding=pad)
-    return y.permute(0, 2, 3, 1).numpy(), s.permute(0, 2, 3, 1).numpy()
-
-
-def check(y, ref, scale, precision, what):
-    assert y.shape == ref.shape, (y.shape, ref.shape)
-    err = np.abs(y - ref)
-    tol = K_BOUND[precision] * UNIT[precision] * scale
-    if precision in ROUNDED:
-        tol = tol + 2.0 ** -24      # an output below 2^-14 is an fp16 subnormal
-    with np.errstate(invalid="ignore"):
-        ratio = float(np.nanmax(err / (UNIT[precision] * scale))) if np.isfinite(err).all() else float("inf")
-    RATIOS[precision] = max(RATIOS.get(precision, 0.0), ratio)
-    print("%s %s: max err / (unit * scale) = %.3f" % (what, precision, ratio))
-    assert (err <= tol).all(), (what, precision, worst(err, tol))
-
-
-def he(r, shape, fan_in):
-    return (r.standard_normal(shape) * (2.0 / fan_in) ** 0.5).astype(np.float32)
 
 
 # ----------------------------------------------------------------------------------------------------------------

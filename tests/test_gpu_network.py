@@ -211,3 +211,42 @@ def test_graph_replay_is_deterministic_and_batch_independent():
     torch.cuda.synchronize()
     assert torch.equal(d[4][0], a[4][0]) and torch.equal(d[2][0], a[2][0]) and torch.equal(d[2][1], a[2][0])
     assert net.launch_count() > 0
+
+
+# Inputs of 64 pixels or less per side leave P6 one pixel wide on that side; the second FPN downsample layer then runs a
+# 3x3/s2/p1 conv whose odd phase is empty (its taps read only the zero padding).
+SMALL_INPUT_CASES = [(c, H, W) for c in ("yolact_resnet50_config", "yolact_darknet53_config")
+                     for H, W in ((64, 64), (550, 64))]
+
+
+def _raw_heads(cfg_name, H, W, precision, seed=11):
+    cfg = cfg_for(cfg_name)
+    yolact_b200.cfg.replace(cfg.copy())
+    net = yolact_b200.Yolact(cfg, precision=precision)
+    net.load_state_dict(deterministic_state_dict(net.state_dict(), 7))
+    net.train()
+    out = net(deterministic_input(1, H, W, seed=seed).cuda())
+    return {k: out[k].cpu().numpy() for k in ("proto", "loc", "conf", "mask", "priors")}
+
+
+@pytest.mark.parametrize("cfg_name,H,W", SMALL_INPUT_CASES, ids=lambda v: str(v))
+def test_one_pixel_p6_tensor_cores_match_f32(cfg_name, H, W):
+    ref = _raw_heads(cfg_name, H, W, "f32")
+    got = _raw_heads(cfg_name, H, W, "f16x3")
+    assert np.array_equal(got["priors"], ref["priors"])
+    for k in ("proto", "loc", "conf", "mask"):
+        assert np.isfinite(got[k]).all(), k
+        e = rel_err(got[k], ref[k])
+        print(cfg_name, H, W, k, "f16x3 vs f32 rel err %.2e" % e)
+        assert e < RAW_TOL["f16x3"] + RAW_TOL["f32"], (k, e)
+
+
+@pytest.mark.parametrize("cfg_name", ["yolact_resnet50_config", "yolact_darknet53_config"])
+def test_one_pixel_p6_chain_identical_to_separate_launches(cfg_name, monkeypatch):
+    monkeypatch.setenv("YB_SK", "0")
+    heads = {}
+    for chain in (0, 2):
+        monkeypatch.setenv("YB_CHAIN", str(chain))
+        heads[chain] = _raw_heads(cfg_name, 64, 64, "f16x3")
+    for k in heads[0]:
+        assert np.array_equal(heads[0][k], heads[2][k]), (k, float(np.abs(heads[0][k] - heads[2][k]).max()))

@@ -1246,11 +1246,23 @@ TcConvPlan* tc_conv_plan_create(const ConvProblem& p, const __half* w_packed, co
         q.tap_dx[tap] = floordiv(qx - px, s);
         used[py * s + px] = true;
       }
+    // a stride-2 phase is empty on a one-pixel side (H == 1: no odd rows): its taps read only the conv's zero padding.
+    // They load from phase 0 (never empty) at a row offset past its last row instead: TMA zero-fills a box that lies
+    // wholly out of bounds and still counts its full bytes, so they add exactly zero with no kernel branch.
+    const int H0 = (p.H + s - 1) / s;
+    for (int tap = 0; tap < q.ntaps; ++tap) {
+      const int ph = q.tap_map[tap], py = ph / s, px = ph % s;
+      if (p.H - py >= 1 && p.W - px >= 1) continue;
+      q.tap_map[tap] = 0;
+      q.tap_dy[tap] = H0;
+      q.tap_dx[tap] = 0;
+      used[0] = true;
+    }
     for (int py = 0; py < s; ++py)
       for (int px = 0; px < s; ++px) {
         if (!used[py * s + px]) continue;
         int Hv = (p.H - py + s - 1) / s, Wv = (p.W - px + s - 1) / s;
-        YB_REQUIRE(Hv >= 1 && Wv >= 1, "tc_conv: empty phase view");
+        if (Hv < 1 || Wv < 1) continue;   // no tap reads it (remapped above)
         const __half* base = x + ((size_t)py * p.W + px) * CinP;
         uint64_t dims[4] = {CinP, (uint64_t)Wv, (uint64_t)Hv, (uint64_t)p.B};
         uint64_t str[3] = {(uint64_t)s * CinP * 2, (uint64_t)s * p.W * CinP * 2,
