@@ -588,6 +588,32 @@ YB_API int yb_set_graphs(yb_handle* h, int enable);
  * out[14] = consumer {flat, tw, th, tiles_x, tiles_y, m_tiles}, producer {same six}, first, last. */
 YB_API int yb_debug_chain_deps(int B, int Hin, int Win, int k, int stride, int pad, int producer_flat, int m, int32_t* out);
 
+/* ---- plan files ---------------------------------------------------------------------------------
+ * A handle plans every network input shape it meets by timing: the tensor-core tiling of each layer shape, and for
+ * each run of consecutive convolutions whether one chain launch beats the separate launches.  A plan file records
+ * these decisions as text; a handle that loads one takes them from the file and times nothing the file covers, so it
+ * runs the same kernels, and computes the same bits, as the handle that wrote it (same file, build and GPU model).
+ * The header names the build (yb_build_id), the device name, compute capability and SM count, the precision and the
+ * switches that change the candidate set (stream-K candidates, YB_CHAIN, programmatic dependent launch).
+ *
+ * yb_save_plans writes every decision the handle holds (timed or loaded), sorted, so saving right after a load writes
+ * the loaded file's bytes.  yb_load_plans merges a file into the handle's table, all or nothing: YB_ERR_INVALID, with
+ * the handle untouched and yb_last_error() naming the field, for an unreadable, truncated or malformed file, another
+ * format version or build, a header field that differs from this handle's, or an entry that disagrees with a decision
+ * the handle already made.  Shapes the file lacks are timed as usual and added to the table.  yb_create loads the
+ * file named by the environment variable YB_PLANS when it exists (a refused file is reported on stderr and ignored).
+ * yb_plan_stats: decisions made by timing, and plan decisions taken from a loaded file (every use counts), since
+ * the handle was created. */
+YB_API int yb_save_plans(yb_handle* h, const char* path);
+YB_API int yb_load_plans(yb_handle* h, const char* path);
+YB_API int yb_plan_stats(yb_handle* h, int64_t* timed, int64_t* loaded);
+/* Build id of the compiled kernels: a hash of the CUDA sources and compiler flags, the plan file's `build` field. */
+YB_API const char* yb_build_id(void);
+/* Host-only (no device needed): parses the plan file at `path` and checks its format, version and build id -- the
+ * checks yb_load_plans makes before it compares the header with a handle.  When out_path is not NULL, writes the
+ * parsed file back there as yb_save_plans would.  YB_ERR_INVALID, naming the line and field, otherwise. */
+YB_API int yb_check_plans(const char* path, const char* out_path);
+
 #ifdef __cplusplus
 }
 #endif

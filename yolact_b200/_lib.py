@@ -224,6 +224,11 @@ SIGNATURES = {
     "yb_last_forward_profile": (c_int, [c_void_p, c_char_p, c_int64]),
     "yb_debug_chain_deps": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int32)]),
     "yb_set_graphs": (c_int, [c_void_p, c_int]),
+    "yb_save_plans": (c_int, [c_void_p, c_char_p]),
+    "yb_load_plans": (c_int, [c_void_p, c_char_p]),
+    "yb_plan_stats": (c_int, [c_void_p, POINTER(c_int64), POINTER(c_int64)]),
+    "yb_build_id": (c_char_p, []),
+    "yb_check_plans": (c_int, [c_char_p, c_char_p]),
 }
 
 _lib = None

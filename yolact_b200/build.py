@@ -6,6 +6,7 @@
 Produces yolact_b200/libyolact_b200.so (C ABI of include/yolact_b200.h).  nvcc cross-compiles
 without a GPU; the .so and the objects are build products (git-ignored).
 """
+import hashlib
 import os
 import subprocess
 import sys
@@ -17,7 +18,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "csrc", "build")
 LIB = os.path.join(HERE, "libyolact_b200.so")
 
-SOURCES = ["capi.cu", "engine.cu", "tc_conv.cu", "stem_tc.cu", "simt_conv.cu", "pointwise.cu", "detect.cu", "mask.cu", "dcn.cu", "dcn_tc.cu", "evalops.cu", "evalmap.cu", "render.cu", "cocorle.cu", "evaliou.cu"]
+SOURCES = ["capi.cu", "engine.cu", "tc_conv.cu", "stem_tc.cu", "simt_conv.cu", "pointwise.cu", "detect.cu", "mask.cu", "dcn.cu", "dcn_tc.cu", "evalops.cu", "evalmap.cu", "render.cu", "cocorle.cu", "evaliou.cu", "plans.cu"]
 HEADERS = ["common.cuh", "kernels.cuh", "engine.cuh", "tc_common.cuh", "mask_math.cuh", "staged_mask.cuh", os.path.join(ROOT, "include", "yolact_b200.h")]
 
 NVCC_FLAGS = [
@@ -26,6 +27,24 @@ NVCC_FLAGS = [
     "-Xcompiler", "-fPIC",
     "-Xcompiler", "-fvisibility=hidden",
 ]
+
+
+# the one source that embeds the build id (yb_build_id, the plan file's `build` field)
+BUILD_ID_SOURCE = "plans.cu"
+
+
+def build_id(flags=NVCC_FLAGS):
+    """Hash of every compiled source, header and compiler flag: plan files written by one library are refused by a
+    library built from anything else."""
+    h = hashlib.sha256()
+    for f in list(flags) + ["--"]:
+        h.update(f.encode() + b"\0")
+    for name in SOURCES + HEADERS:
+        path = name if os.path.isabs(name) else os.path.join(CSRC, name)
+        h.update(os.path.basename(path).encode() + b"\0")
+        with open(path, "rb") as fp:
+            h.update(hashlib.sha256(fp.read()).digest())
+    return h.hexdigest()[:16]
 
 
 def _nvcc():
@@ -61,12 +80,15 @@ def _build(force, verbose, NVCC_FLAGS, OBJ, LIB):
     hdrs = [h if os.path.isabs(h) else os.path.join(CSRC, h) for h in HEADERS]
     jobs = []
     objs = []
-    for src in SOURCES:
-        s = os.path.join(CSRC, src)
+    srcs = [os.path.join(CSRC, src) for src in SOURCES]
+    for src, s in zip(SOURCES, srcs):
         o = os.path.join(OBJ, src.replace(".cu", ".o"))
         objs.append(o)
-        if force or _newer(o, [s] + hdrs):
-            jobs.append([nvcc] + NVCC_FLAGS + ["-c", s, "-o", o])
+        flags, deps = NVCC_FLAGS, [s] + hdrs
+        if src == BUILD_ID_SOURCE:   # rebuilt whenever anything the id hashes changes
+            flags, deps = NVCC_FLAGS + ['-DYB_BUILD_ID="%s"' % build_id(NVCC_FLAGS)], srcs + hdrs
+        if force or _newer(o, deps):
+            jobs.append([nvcc] + flags + ["-c", s, "-o", o])
 
     def run(cmd):
         if verbose:

@@ -247,6 +247,19 @@ int yb_create(const yb_config* cfg, int device, yb_handle** out) {
   YB_REQUIRE(cfg->mask_dim % 4 == 0 && cfg->mask_dim > 0, "mask_dim must be a positive multiple of 4");
   DeviceGuard g(device);
   YB_CHECK_CUDA(cudaFree(0));
+  // YB_PLANS=<path>: start from a saved plan file when there is one (a network handle whose header it does not match
+  // plans by timing, as without it)
+  const char* plans = getenv("YB_PLANS");
+  if (plans && *plans && !h->ops_only) {
+    if (FILE* fp = fopen(plans, "rb")) {
+      fclose(fp);
+      try {
+        h->load_plans(plans);
+      } catch (const yb::Error& e) {
+        fprintf(stderr, "[yolact_b200] YB_PLANS=%s not loaded: %s\n", plans, e.what());
+      }
+    }
+  }
   *out = h.release();
   YB_API_END
 }
@@ -1218,6 +1231,41 @@ int yb_set_graphs(yb_handle* h, int enable) {
 int yb_debug_chain_deps(int B, int Hin, int Win, int k, int stride, int pad, int producer_flat, int m, int32_t* out) {
   YB_API_BEGIN
   yb::tc_chain_debug_deps(B, Hin, Win, k, stride, pad, producer_flat, m, out);
+  YB_API_END
+}
+
+int yb_save_plans(yb_handle* h, const char* path) {
+  YB_API_BEGIN
+  YB_REQUIRE(h && path, "yb_save_plans: null argument");
+  CallGuard g(h);
+  h->save_plans(path);
+  YB_API_END
+}
+
+int yb_load_plans(yb_handle* h, const char* path) {
+  YB_API_BEGIN
+  YB_REQUIRE(h && path, "yb_load_plans: null argument");
+  CallGuard g(h);
+  h->load_plans(path);
+  YB_API_END
+}
+
+int yb_plan_stats(yb_handle* h, int64_t* timed, int64_t* loaded) {
+  YB_API_BEGIN
+  YB_REQUIRE(h, "yb_plan_stats: null handle");
+  std::lock_guard<std::recursive_mutex> lk(h->mu);
+  if (timed) *timed = h->plans_timed;
+  if (loaded) *loaded = h->plans_loaded;
+  YB_API_END
+}
+
+const char* yb_build_id(void) { return yb::build_id(); }
+
+int yb_check_plans(const char* path, const char* out_path) {
+  YB_API_BEGIN
+  YB_REQUIRE(path, "yb_check_plans: null path");
+  const PlanFile f = parse_plan_file(read_text_file(path));
+  if (out_path) write_text_file(out_path, write_plan_file(f));
   YB_API_END
 }
 

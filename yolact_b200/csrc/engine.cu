@@ -514,10 +514,30 @@ struct NetBuilder {
           }
         }
       }
-      // the chain, timed against the separately tuned launches
+      // the chain, timed against the separately tuned launches -- unless this run's decision is already in the handle's
+      // table (a plan file, or an earlier executor of this shape).  The key is the executor shape, the run's first and
+      // last layer and every layer's shape.
+      std::string ckey = std::to_string(ex->B) + "x" + std::to_string(ex->H) + "x" + std::to_string(ex->W) + ":" +
+                         ops[i].name.substr(0, ops[i].name.find(' ')) + ".." +
+                         ops[k - 1].name.substr(0, ops[k - 1].name.find(' ')) + ":";
+      for (size_t j = i; j < k; ++j) ckey += (j > i ? ";" : "") + shape_key(ops[j].prob);
+      auto known = h->chain_cache.find(ckey);
       TcChain* chain = nullptr;
       bool use = false;
-      {
+      if (known != h->chain_cache.end()) {
+        std::vector<const TcConvPlan*> cpl(cp.begin(), cp.end());
+        try {
+          chain = tc_chain_create(cpl, dep_a, dep_r);
+        } catch (const Error&) {
+          chain = nullptr;
+        }
+        if (chain && !tc_chain_graph_ok(chain)) {
+          tc_chain_destroy(chain);
+          chain = nullptr;
+        }
+        use = chain && known->second.chain;
+        if (known->second.loaded) ++h->plans_loaded;
+      } else {
         std::vector<const TcConvPlan*> cpl(cp.begin(), cp.end());
         const auto lc_before = h->lc.n;
         cudaEvent_t e0, e1;
@@ -552,6 +572,8 @@ struct NetBuilder {
             for (size_t j = i; j < k; ++j) ops[j].fn(0);
           });
           use = (h->chain_mode == 2) || ms_chain < ms_sep;
+          ++h->plans_timed;
+          h->chain_cache[ckey].chain = use;
           if (getenv("YB_CHAIN_VERBOSE"))
             fprintf(stderr, "[yolact_b200] chain %s .. %s (%zu layers): chain %.3f ms, separate %.3f ms -> %s\n",
                     ops[i].name.substr(0, ops[i].name.find(' ')).c_str(), ops[k - 1].name.substr(0, ops[k - 1].name.find(' ')).c_str(), n,
@@ -609,16 +631,24 @@ struct NetBuilder {
   // are launch/wave-quantisation bound and large-K ones L2-bandwidth bound, so no single rule fits.
   TcConvPlan* autotune_tc(const ConvProblem& p, const __half* w) {
     // identical layer shapes (e.g. the 23 blocks of stage 3) share one decision
-    const std::string tkey = std::to_string(p.B) + "," + std::to_string(p.H) + "," + std::to_string(p.W) + "," +
-                             std::to_string(p.Cin) + "," + std::to_string(p.Cout) + "," + std::to_string(p.KH) + "," +
-                             std::to_string(p.stride) + "," + std::to_string(p.pad) + "," + (p.residual ? "r" : "-") +
-                             (p.y_f32 ? "f" : "h") + (p.split ? "s" : "") + std::to_string(p.nseg) + "," + std::to_string(p.y_pix_stride) + "," + std::to_string((long long)p.y_batch_stride);
+    const std::string tkey = shape_key(p);
     auto it = h->tune_cache.find(tkey);
     if (it != h->tune_cache.end()) {
-      TcConvPlan* pl = tc_conv_plan_create(p, w, it->second);
+      TcConvPlan* pl = tc_conv_plan_create(p, w, it->second.t);
+      if (it->second.loaded) {
+        // a plan file's tiling is obeyed exactly or not at all
+        if (tc_tiling_str(tc_conv_plan_tiling(pl)) != tc_tiling_str(it->second.t)) {
+          const std::string got = tc_tiling_str(tc_conv_plan_tiling(pl));
+          tc_conv_plan_destroy(pl);
+          throw Error(YB_ERR_INVALID, "plan file tiling " + tkey + " (" + tc_tiling_str(it->second.t) +
+                                          ") does not replay on this layer: it resolves to " + got);
+        }
+        ++h->plans_loaded;
+      }
       if (tc_conv_plan_tiling(pl).stream_k) tc_conv_plan_set_sk_workspace(pl, sk_workspace());
       return pl;
     }
+    ++h->plans_timed;
     const int bns[4] = {256, 128, 64, 32};
     const int sts[3] = {0, 3, 2};
     const int grids[3] = {device_sms(), 2 * device_sms(), 1 << 30};
@@ -702,8 +732,17 @@ struct NetBuilder {
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
     YB_REQUIRE(best != nullptr, "autotune: no candidate");
-    h->tune_cache[tkey] = tc_conv_plan_tiling(best);
+    h->tune_cache[tkey].t = tc_conv_plan_tiling(best);
     return best;
+  }
+
+  // the autotuner's key of a layer: every problem field a tiling's validity or speed depends on (no pointers), so
+  // that layers of one shape share a decision within a handle and across processes (plan files)
+  static std::string shape_key(const ConvProblem& p) {
+    return std::to_string(p.B) + "," + std::to_string(p.H) + "," + std::to_string(p.W) + "," + std::to_string(p.Cin) +
+           "," + std::to_string(p.Cout) + "," + std::to_string(p.KH) + "," + std::to_string(p.stride) + "," +
+           std::to_string(p.pad) + "," + (p.residual ? "r" : "-") + (p.y_f32 ? "f" : "h") + (p.split ? "s" : "") +
+           std::to_string(p.nseg) + "," + std::to_string(p.y_pix_stride) + "," + std::to_string((long long)p.y_batch_stride);
   }
 };
 

@@ -151,6 +151,39 @@ class DeviceBuffer {
   const size_t floor_;   // 0: exact growth
 };
 
+// ---- plan files (plans.cu): the autotuner's tilings and form_chains' decisions, saved and loaded as text
+// A decision in the handle's table; `loaded` marks one taken from a plan file (yb_plan_stats counts its uses).
+struct TunedTiling {
+  TcTiling t;
+  bool loaded = false;
+};
+struct ChainChoice {
+  bool chain = false;   // one chain launch (true) or the separately tuned launches
+  bool loaded = false;
+};
+// The header fields a plan file must share with the handle that loads it, in file order.
+struct PlanHeader {
+  std::string build;     // yb_build_id() of the library that wrote it
+  std::string device;    // cudaDeviceProp::name
+  std::string cc;        // "9.0"
+  int sms = 0;
+  std::string precision; // "f32", "f16tc", "f16x3"
+  int sk_candidates = 0, chain_mode = 0, pdl = 0;
+};
+struct PlanFile {
+  PlanHeader hdr;
+  std::map<std::string, TcTiling> tilings;   // autotune_tc's key -> tiling
+  std::map<std::string, bool> chains;        // form_chains' key -> chain (true) or separate
+};
+const char* build_id();
+// Parses a whole plan file.  Throws Error(YB_ERR_INVALID) naming the line and field for anything but a complete file
+// of this format version written by this build: a wrong version or build id, a missing, reordered or unknown header
+// field, a malformed or unknown entry field, a duplicate key, or a missing entry or end line (truncation).
+PlanFile parse_plan_file(const std::string& text);
+std::string write_plan_file(const PlanFile& f);
+std::string read_text_file(const std::string& path);
+void write_text_file(const std::string& path, const std::string& text);   // via a temporary and a rename
+
 }  // namespace yb
 
 struct yb_handle {
@@ -167,7 +200,10 @@ struct yb_handle {
   std::map<std::string, yb::ConvW> convs;
   std::map<std::string, std::unique_ptr<yb::Executor>> execs;
   std::vector<void*> weight_allocs;
-  std::map<std::string, yb::TcTiling> tune_cache;  // layer shape -> the autotuner's tiling
+  std::map<std::string, yb::TunedTiling> tune_cache;   // layer shape -> the autotuner's tiling
+  std::map<std::string, yb::ChainChoice> chain_cache;  // executor shape + run of layers -> form_chains' decision
+  int64_t plans_timed = 0;        // decisions made by timing (autotune sweeps, chain-vs-separate timings)
+  int64_t plans_loaded = 0;       // plan decisions taken from a loaded plan file (every use counts)
   bool sk_candidates = true;      // the autotuner times stream-K plans: on in the split mode (YB_SK=0/1)
   int chain_mode = 1;             // runs of consecutive convs as one chain launch: 0 never, 1 when timed faster, 2 always (YB_CHAIN)
   cudaStream_t tune_stream = nullptr;   // private stream of the autotuner when PDL candidates are timed
@@ -213,6 +249,11 @@ struct yb_handle {
   void infer_on(yb::Executor* ex, yb::Executor::FrameInput* fin, const void* d_x, int cross_class, int max_out,
                 float* d_box, float* d_coef_out, int64_t* d_cls, float* d_score, int32_t* d_count, float* d_proto,
                 cudaStream_t stream);
+  // ---- plan files (plans.cu)
+  yb::PlanHeader plan_header() const;
+  void save_plans(const std::string& path) const;
+  // all or nothing: on any refusal (Error naming the field) the handle's tables are unchanged
+  void load_plans(const std::string& path);
 };
 
 namespace yb {

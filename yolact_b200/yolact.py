@@ -12,6 +12,8 @@ nn.Module tree below only HOLDS parameters under the reference's names -- its la
 called.  There is no PyTorch/CPU fallback: without the CUDA library on an H100 forward() raises.
 """
 import ctypes
+import os
+import warnings
 
 import torch
 import torch.nn as nn
@@ -226,6 +228,7 @@ class Yolact(nn.Module):
         self._version = 1       # bumped whenever the parameters may have changed
         self._pushed = {}       # device index -> version of the weights that handle holds
         self._detect_pushed = {}  # device index -> (top_k, conf_thresh, nms_thresh, max_num_detections) the handle uses
+        self._plan_files = []   # load_plans paths, loaded into every handle created later too
 
     # ---- weights ---------------------------------------------------------------------------------
     def save_weights(self, path):
@@ -270,6 +273,10 @@ class Yolact(nn.Module):
             yc = make_yb_config(self.cfg, self.precision)
             _lib.check(lib.yb_create(ctypes.byref(yc), idx, ctypes.byref(h)), "yb_create")
             self._handles[idx] = h
+            for path in self._plan_files:
+                if lib.yb_load_plans(h, path.encode()) != 0:
+                    warnings.warn("plan file %s does not apply to cuda:%d; its shapes are timed as usual: %s"
+                                  % (path, idx, lib.yb_last_error().decode()))
         h = self._handles[idx]
         if self._pushed.get(idx) != self._version:     # per device: every handle re-syncs on its next call
             self._push_weights(h)
@@ -294,6 +301,34 @@ class Yolact(nn.Module):
                 lib.yb_destroy(h)
         except Exception:
             pass
+
+    # ---- plan files ------------------------------------------------------------------------------
+    def save_plans(self, path, device=None):
+        """Writes the plan decisions (tensor-core tilings, chain-or-separate choices) the handle on `device` (default:
+        the current CUDA device) has made so far, for every input shape it has run, to the text file `path`."""
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        _lib.check(_lib.load().yb_save_plans(self._handle_for(dev), os.fspath(path).encode()), "yb_save_plans")
+
+    def load_plans(self, path):
+        """Takes plan decisions from a file written by save_plans (or `python -m yolact_b200.tune`): the shapes it
+        covers are planned without timing, with the same kernels, so outputs match the writer's bit for bit.  Loaded
+        into every existing handle (raises if one refuses it: see yb_load_plans) and into every handle created later
+        whose device and settings the file's header matches (a warning names the others)."""
+        path = os.fspath(path)
+        lib = _lib.load()
+        _lib.check(lib.yb_check_plans(path.encode(), None), "yb_check_plans")
+        for idx, h in self._handles.items():
+            _lib.check(lib.yb_load_plans(h, path.encode()), "yb_load_plans(cuda:%d)" % idx)
+        self._plan_files.append(path)
+
+    def plan_stats(self, device=None):
+        """(timed, loaded) of the handle on `device`: plan decisions made by timing, and plan decisions taken from a
+        loaded file (every use counts)."""
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        timed, loaded = ctypes.c_int64(), ctypes.c_int64()
+        _lib.check(_lib.load().yb_plan_stats(self._handle_for(dev), ctypes.byref(timed), ctypes.byref(loaded)),
+                   "yb_plan_stats")
+        return timed.value, loaded.value
 
     # ---- introspection ---------------------------------------------------------------------------
     def launch_count(self):
