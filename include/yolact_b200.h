@@ -48,6 +48,8 @@
  *                         --display_fps box (eval.py:211-219) and --display_masks=False
  *   yb_dcn_forward     <- dcn_v2_forward (external/DCNv2/src/dcn_v2.h:9-39,
  *                         src/cuda/dcn_v2_cuda.cu:42-172, src/cuda/dcn_v2_im2col_cuda.cu:125-195)
+ *   yb_dcn_forward_ex  <- the same for any kernel size, anisotropic geometry and deformable groups
+ *   yb_dcn_psroi_pool  <- dcn_v2_psroi_pooling_forward (src/cuda/dcn_v2_psroi_pooling_cuda.cu:59-146)
  *   yb_conv2d          <- nn.Conv2d + folded BatchNorm2d + activation (+ residual), op-level test hook
  *   yb_conv2d_ex       <- the same with the network's other epilogues (residual after the activation, fp32 output,
  *                         zero-padded channels, the fused prediction head) and the tensor-core stem, op-level test hook
@@ -512,12 +514,50 @@ YB_API int yb_render_list_ex(yb_handle* h, const yb_render_item* h_items, int B,
 /* ---- op-level entry points --------------------------------------------------------------------- */
 /* Mirrors dcn_v2_forward's argument list (src/dcn_v2.h:9-23); all tensors NCHW fp32 contiguous.
  * input [B,C,H,W], weight [Co,C,kh,kw], bias [Co], offset [B,2*dg*kh*kw,Ho,Wo], mask [B,dg*kh*kw,Ho,Wo],
- * output [B,Co,Ho,Wo].  deformable_group must be 1 (all YOLACT++ configs). */
+ * output [B,Co,Ho,Wo].  The narrow contract of the YOLACT++ layers: a 3x3 kernel, isotropic stride, padding and
+ * dilation, deformable_group 1 and C % 16 == 0 (YB_ERR_INVALID otherwise).  It runs yb_dcn_forward_ex, bit for bit. */
 YB_API int yb_dcn_forward(yb_handle* h, const float* d_input, const float* d_weight, const float* d_bias,
                    const float* d_offset, const float* d_mask, float* d_output,
                    int B, int C, int H, int W, int Co,
                    int kernel_h, int kernel_w, int stride_h, int stride_w, int pad_h, int pad_w,
                    int dilation_h, int dilation_w, int deformable_group, void* stream);
+
+/* Geometry of yb_dcn_forward_ex.  Output size Ho = (H + 2 pad_h - (dilation_h (kernel_h - 1) + 1)) / stride_h + 1,
+ * likewise Wo. */
+typedef struct {
+  int32_t kernel_h, kernel_w;        /* >= 1, kernel_h * kernel_w <= 1024 */
+  int32_t stride_h, stride_w;        /* >= 1 */
+  int32_t pad_h, pad_w;              /* >= 0 */
+  int32_t dilation_h, dilation_w;    /* >= 1 */
+  int32_t deformable_group;          /* dg >= 1, C % dg == 0 */
+} yb_dcn_params;
+
+/* The whole of dcn_v2_forward's domain (dcn_v2_im2col_cuda.cu:125-195).  Offset channel g*2*kh*kw + 2*tap holds the
+ * row offset and + 1 the column offset of tap = i*kw + j in deformable group g; mask channel g*kh*kw + tap; input
+ * channel c belongs to group c / (C / dg).  Where it runs, by the handle's precision:
+ *   f32    the CUDA-core kernel, any C;
+ *   f16tc  the tensor-core kernel when (C / dg) % 64 == 0, else the CUDA-core kernel, which needs (C / dg) % 16 == 0;
+ *   f16x3  the tensor-core kernel, which needs (C / dg) % 64 == 0.
+ * YB_ERR_INVALID, with the output untouched, for a null pointer (bias may be null), a geometry outside the ranges
+ * above, a precision's channel rule, B, C, H, W or Co < 1, or an empty output.  Synchronises `stream`. */
+YB_API int yb_dcn_forward_ex(yb_handle* h, const float* d_input, const float* d_weight, const float* d_bias,
+                             const float* d_offset, const float* d_mask, float* d_output, int B, int C, int H, int W,
+                             int Co, const yb_dcn_params* p, void* stream);
+
+/* Deformable position-sensitive RoI pooling, forward (DeformablePSROIPoolForwardKernel of
+ * dcn_v2_psroi_pooling_cuda.cu), fp32, one thread per output element.  input NCHW [N,C,H,W], rois [R,5] (batch index,
+ * x1, y1, x2, y2 in input-image pixels), trans [R, 2*num_classes, part_size, part_size] (ignored, and may be null,
+ * when no_trans; num_classes is then 1), output [R, output_dim, pooled, pooled], count (nullable) the same shape: the
+ * samples each bin averaged.  Output channel ctop of bin (ph, pw) reads input channel
+ * (ctop * group_size + gh) * group_size + gw.  YB_ERR_INVALID, with nothing written, for a null input, rois, output or
+ * (unless no_trans) trans, N, H, W < 1 or R < 0, C != output_dim * group_size^2, num_classes < 1 or
+ * output_dim % num_classes != 0, a non-positive pooled, group_size, part_size or sample_per_part, or a RoI whose batch
+ * index is not finite or, truncated to an integer as the reference does, outside [0, N).  Synchronises `stream` (the
+ * batch indices are checked on the host). */
+YB_API int yb_dcn_psroi_pool(yb_handle* h, const float* d_input, const float* d_rois, const float* d_trans,
+                             float* d_output, float* d_count, int N, int C, int H, int W, int R, int no_trans,
+                             int num_classes, float spatial_scale, int output_dim, int group_size, int pooled,
+                             int part_size, int sample_per_part, float trans_std, void* stream);
 
 /* Single convolution through the same kernels the network uses (test / microbench hook).
  * x NCHW fp32 [B,Ci,H,W], w OIHW fp32 (host), bias fp32[Co] (host, nullable),

@@ -145,6 +145,17 @@ class YbConvOpts(ctypes.Structure):
     ]
 
 
+class YbDcnParams(ctypes.Structure):
+    """Mirror of yb_dcn_params (yb_dcn_forward_ex)."""
+    _fields_ = [
+        ("kernel_h", c_int32), ("kernel_w", c_int32),
+        ("stride_h", c_int32), ("stride_w", c_int32),
+        ("pad_h", c_int32), ("pad_w", c_int32),
+        ("dilation_h", c_int32), ("dilation_w", c_int32),
+        ("deformable_group", c_int32),
+    ]
+
+
 YB_BACKBONE_NONE, YB_BACKBONE_RESNET, YB_BACKBONE_DARKNET = -1, 0, 1
 YB_PREC_F32, YB_PREC_F16TC, YB_PREC_F16X3 = 0, 1, 2
 PRECISIONS = {"f32": YB_PREC_F32, "f16tc": YB_PREC_F16TC, "f16x3": YB_PREC_F16X3}
@@ -213,6 +224,8 @@ SIGNATURES = {
                                   c_float, c_void_p, c_int, POINTER(YbRenderOpts), c_void_p]),
     "yb_dcn_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 14 +
                        [c_void_p]),
+    "yb_dcn_forward_ex": (c_int, [c_void_p] * 7 + [c_int] * 5 + [POINTER(YbDcnParams), c_void_p]),
+    "yb_dcn_psroi_pool": (c_int, [c_void_p] * 6 + [c_int] * 7 + [c_float] + [c_int] * 5 + [c_float, c_void_p]),
     "yb_conv2d": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 12 +
                   [POINTER(c_float), c_void_p]),
     "yb_conv2d_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 11 +

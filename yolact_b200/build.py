@@ -18,7 +18,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "csrc", "build")
 LIB = os.path.join(HERE, "libyolact_b200.so")
 
-SOURCES = ["capi.cu", "engine.cu", "tc_conv.cu", "stem_tc.cu", "simt_conv.cu", "pointwise.cu", "detect.cu", "mask.cu", "dcn.cu", "dcn_tc.cu", "evalops.cu", "evalmap.cu", "render.cu", "cocorle.cu", "evaliou.cu", "plans.cu"]
+SOURCES = ["capi.cu", "engine.cu", "tc_conv.cu", "stem_tc.cu", "simt_conv.cu", "pointwise.cu", "detect.cu", "mask.cu", "dcn.cu", "dcn_tc.cu", "dcn_pool.cu", "evalops.cu", "evalmap.cu", "render.cu", "cocorle.cu", "evaliou.cu", "plans.cu"]
 HEADERS = ["common.cuh", "kernels.cuh", "engine.cuh", "tc_common.cuh", "mask_math.cuh", "staged_mask.cuh", os.path.join(ROOT, "include", "yolact_b200.h")]
 
 NVCC_FLAGS = [

@@ -40,16 +40,16 @@ struct DeviceGuard {
   }
 };
 
-// offset [B,18,HW] + mask [B,9,HW] (NCHW fp32) -> om [B,HW,27]
+// offset [B,2n,HW] + mask [B,n,HW] (NCHW fp32, n = dg * taps) -> om [B,HW,3n]
 __global__ void pack_om_kernel(const float* __restrict__ off, const float* __restrict__ msk, float* __restrict__ om,
-                               int B, int HW) {
-  const int64_t total = (int64_t)B * HW * 27;
+                               int B, int HW, int n) {
+  const int64_t total = (int64_t)B * HW * 3 * n;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    int ch = (int)(i % 27);
-    int64_t r = i / 27;
+    int ch = (int)(i % (3 * n));
+    int64_t r = i / (3 * n);
     int p = (int)(r % HW);
     int b = (int)(r / HW);
-    om[i] = ch < 18 ? off[((int64_t)b * 18 + ch) * HW + p] : msk[((int64_t)b * 9 + (ch - 18)) * HW + p];
+    om[i] = ch < 2 * n ? off[((int64_t)b * 2 * n + ch) * HW + p] : msk[((int64_t)b * n + (ch - 2 * n)) * HW + p];
   }
 }
 
@@ -854,50 +854,42 @@ int yb_display_blend(yb_handle* h, const float* d_img, int img_is_255, const voi
   YB_API_END
 }
 
-int yb_dcn_forward(yb_handle* h, const float* d_input, const float* d_weight, const float* d_bias,
-                   const float* d_offset, const float* d_mask, float* d_output, int B, int C, int H, int W, int Co,
-                   int kernel_h, int kernel_w, int stride_h, int stride_w, int pad_h, int pad_w, int dilation_h,
-                   int dilation_w, int deformable_group, void* stream) {
-  YB_API_BEGIN
-  YB_REQUIRE(h && d_input && d_weight && d_offset && d_mask && d_output, "yb_dcn_forward: null argument");
-  YB_REQUIRE(kernel_h == 3 && kernel_w == 3, "yb_dcn_forward: only 3x3 kernels (all YOLACT++ DCN layers)");
-  YB_REQUIRE(stride_h == stride_w && pad_h == pad_w && dilation_h == dilation_w, "yb_dcn_forward: anisotropic params");
-  YB_REQUIRE(deformable_group == 1, "yb_dcn_forward: deformable_group must be 1");
-  YB_REQUIRE(C % 16 == 0, "yb_dcn_forward: C must be a multiple of 16");
-  CallGuard g(h);
-  cudaStream_t s = (cudaStream_t)stream;
-  const int Ho = (H + 2 * pad_h - (dilation_h * 2 + 1)) / stride_h + 1;
-  const int Wo = (W + 2 * pad_w - (dilation_w * 2 + 1)) / stride_w + 1;
-  TempPool tp;
-  float* om = (float*)tp.get((size_t)B * Ho * Wo * 27 * 4);
-  pack_om_kernel<<<grid1d((int64_t)B * Ho * Wo * 27), 256, 0, s>>>(d_offset, d_mask, om, B, Ho * Wo);
-  YB_CHECK_LAUNCH();
+// The one implementation behind yb_dcn_forward and yb_dcn_forward_ex; the caller has validated the arguments.
+static void dcn_forward(yb_handle* h, const float* d_input, const float* d_weight, const float* d_bias,
+                        const float* d_offset, const float* d_mask, float* d_output, int B, int C, int H, int W, int Co,
+                        const yb_dcn_params& g, int Ho, int Wo, cudaStream_t s) {
+  const int taps = g.kernel_h * g.kernel_w, dg = g.deformable_group;
+  const int npl = (h->cfg.precision == YB_PREC_F16X3) ? 2 : 1;
+  const int sp = npl - 1;
   const bool f16 = (h->cfg.precision != YB_PREC_F32);
-  const int sp = (h->cfg.precision == YB_PREC_F16X3) ? 1 : 0;
-  YB_REQUIRE(!sp || C % 64 == 0, "yb_dcn_forward: the split-precision mode needs C % 64 == 0");
-  const int npl = sp ? 2 : 1;
+  const bool tc = f16 && (C / dg) % 64 == 0;
+  CallGuard cg(h);
+  TempPool tp;
+  float* om = (float*)tp.get((size_t)B * Ho * Wo * 3 * dg * taps * 4);
+  pack_om_kernel<<<grid1d((int64_t)B * Ho * Wo * 3 * dg * taps), 256, 0, s>>>(d_offset, d_mask, om, B, Ho * Wo, dg * taps);
+  YB_CHECK_LAUNCH();
   // the weights are packed on the host (op-level hook, not the hot path)
-  std::vector<float> hw((size_t)Co * C * 9);
+  std::vector<float> hw((size_t)Co * C * taps);
   YB_CHECK_CUDA(cudaMemcpyAsync(hw.data(), d_weight, hw.size() * 4, cudaMemcpyDeviceToHost, s));
   YB_CHECK_CUDA(cudaStreamSynchronize(s));
   if (!f16) {
     float* x = (float*)tp.get((size_t)B * H * W * C * 4);
     float* y = (float*)tp.get((size_t)B * Ho * Wo * Co * 4);
-    const float* wk = (const float*)tp.put(pack_weights(hw.data(), Co, C, 3, 3, nullptr, WLayout::Simt, WFormat::F32));
+    const float* wk =
+        (const float*)tp.put(pack_weights(hw.data(), Co, C, g.kernel_h, g.kernel_w, nullptr, WLayout::Simt, WFormat::F32));
     launch_nchw_f32_to_nhwc<float>(d_input, x, B, C, H, W, s, &h->lc);
-    launch_dcn_simt<float>(x, om, wk, d_bias, y, B, H, W, C, Ho, Wo, Co, stride_h, pad_h, dilation_h, ACT_NONE, 0, s,
-                           &h->lc);
+    launch_dcn_simt<float>(x, om, wk, d_bias, y, B, H, W, C, Ho, Wo, Co, g, ACT_NONE, 0, s, &h->lc);
     launch_nhwc_to_nchw_f32<float>(y, d_output, B, Ho, Wo, Co, s, &h->lc);
   } else {
     // the fused tensor-core kernel needs Cout % 8 == 0 and Cout >= 8: a narrower layer runs with zero weight rows and
     // zero bias up to Cp output channels, of which the first Co are copied out
-    const int Cp = (C % 64 == 0) ? std::max(8, (Co + 7) / 8 * 8) : Co;
+    const int Cp = tc ? std::max(8, (Co + 7) / 8 * 8) : Co;
     __half* x = (__half*)tp.get((size_t)B * H * W * C * 2 * npl);
     __half* y = (__half*)tp.get((size_t)B * Ho * Wo * Cp * 2 * npl);
     launch_nchw_f32_to_nhwc<__half>(d_input, x, B, C, H, W, s, &h->lc, sp);
-    if (C % 64 == 0) {
-      const PackedWeights pw =
-          pack_weights(hw.data(), Co, C, 3, 3, nullptr, WLayout::Dcn, sp ? WFormat::Split : WFormat::F16, 0, Cp);
+    if (tc) {
+      const PackedWeights pw = pack_weights(hw.data(), Co, C, g.kernel_h, g.kernel_w, nullptr, WLayout::Dcn,
+                                            sp ? WFormat::Split : WFormat::F16, 0, Cp);
       const __half* wk = (const __half*)tp.put(pw);
       const float* bias = d_bias;
       if (Cp > Co && d_bias) {
@@ -906,8 +898,7 @@ int yb_dcn_forward(yb_handle* h, const float* d_input, const float* d_weight, co
         YB_CHECK_CUDA(cudaMemcpyAsync(bp, d_bias, (size_t)Co * 4, cudaMemcpyDeviceToDevice, s));
         bias = bp;
       }
-      DcnTcPlan* dp = dcn_tc_plan_create(x, om, wk, bias, y, B, H, W, C, Ho, Wo, Cp, stride_h, pad_h, dilation_h,
-                                         ACT_NONE, 0, sp, pw.out_scale);
+      DcnTcPlan* dp = dcn_tc_plan_create(x, om, wk, bias, y, B, H, W, C, Ho, Wo, Cp, g, ACT_NONE, 0, sp, pw.out_scale);
       try {
         launch_dcn_tc(dp, s, &h->lc);
       } catch (...) {
@@ -916,9 +907,9 @@ int yb_dcn_forward(yb_handle* h, const float* d_input, const float* d_weight, co
       }
       dcn_tc_plan_destroy(dp);
     } else {
-      const __half* wk = (const __half*)tp.put(pack_weights(hw.data(), Co, C, 3, 3, nullptr, WLayout::Simt, WFormat::F16));
-      launch_dcn_simt<__half>(x, om, wk, d_bias, y, B, H, W, C, Ho, Wo, Co, stride_h, pad_h, dilation_h, ACT_NONE, 0,
-                              s, &h->lc);
+      const __half* wk = (const __half*)tp.put(
+          pack_weights(hw.data(), Co, C, g.kernel_h, g.kernel_w, nullptr, WLayout::Simt, WFormat::F16));
+      launch_dcn_simt<__half>(x, om, wk, d_bias, y, B, H, W, C, Ho, Wo, Co, g, ACT_NONE, 0, s, &h->lc);
     }
     if (Cp == Co) {
       launch_nhwc_to_nchw_f32<__half>(y, d_output, B, Ho, Wo, Co, s, &h->lc, sp);
@@ -930,6 +921,94 @@ int yb_dcn_forward(yb_handle* h, const float* d_input, const float* d_weight, co
     }
   }
   YB_CHECK_CUDA(cudaStreamSynchronize(s));  // temporaries are freed on return
+}
+
+// Ho or Wo of yb_dcn_params' geometry along one axis, 0 when the dilated kernel does not fit
+static int dcn_out(int n, int k, int stride, int pad, int dil) {
+  const int64_t span = (int64_t)n + 2 * (int64_t)pad - ((int64_t)dil * (k - 1) + 1);
+  return span < 0 ? 0 : (int)(span / stride + 1);
+}
+
+int yb_dcn_forward(yb_handle* h, const float* d_input, const float* d_weight, const float* d_bias,
+                   const float* d_offset, const float* d_mask, float* d_output, int B, int C, int H, int W, int Co,
+                   int kernel_h, int kernel_w, int stride_h, int stride_w, int pad_h, int pad_w, int dilation_h,
+                   int dilation_w, int deformable_group, void* stream) {
+  YB_API_BEGIN
+  YB_REQUIRE(h && d_input && d_weight && d_offset && d_mask && d_output, "yb_dcn_forward: null argument");
+  YB_REQUIRE(kernel_h == 3 && kernel_w == 3, "yb_dcn_forward: only 3x3 kernels (all YOLACT++ DCN layers)");
+  YB_REQUIRE(stride_h == stride_w && pad_h == pad_w && dilation_h == dilation_w, "yb_dcn_forward: anisotropic params");
+  YB_REQUIRE(deformable_group == 1, "yb_dcn_forward: deformable_group must be 1");
+  YB_REQUIRE(C % 16 == 0, "yb_dcn_forward: C must be a multiple of 16");
+  YB_REQUIRE(h->cfg.precision != YB_PREC_F16X3 || C % 64 == 0,
+             "yb_dcn_forward: the split-precision mode needs C % 64 == 0");
+  const yb_dcn_params g{3, 3, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w, 1};
+  return yb_dcn_forward_ex(h, d_input, d_weight, d_bias, d_offset, d_mask, d_output, B, C, H, W, Co, &g, stream);
+  YB_API_END
+}
+
+int yb_dcn_forward_ex(yb_handle* h, const float* d_input, const float* d_weight, const float* d_bias,
+                      const float* d_offset, const float* d_mask, float* d_output, int B, int C, int H, int W, int Co,
+                      const yb_dcn_params* p, void* stream) {
+  YB_API_BEGIN
+  YB_REQUIRE(h && d_input && d_weight && d_offset && d_mask && d_output && p, "yb_dcn_forward_ex: null argument");
+  const yb_dcn_params g = *p;
+  YB_REQUIRE(B >= 1 && C >= 1 && H >= 1 && W >= 1 && Co >= 1, "yb_dcn_forward_ex: B, C, H, W and Co must be >= 1");
+  YB_REQUIRE(g.kernel_h >= 1 && g.kernel_w >= 1 && (int64_t)g.kernel_h * g.kernel_w <= 1024,
+             "yb_dcn_forward_ex: kernel_h and kernel_w must be >= 1, kernel_h * kernel_w <= 1024");
+  YB_REQUIRE(g.stride_h >= 1 && g.stride_w >= 1 && g.pad_h >= 0 && g.pad_w >= 0 && g.dilation_h >= 1 &&
+                 g.dilation_w >= 1,
+             "yb_dcn_forward_ex: stride and dilation must be >= 1, padding >= 0");
+  YB_REQUIRE(g.deformable_group >= 1 && C % g.deformable_group == 0,
+             "yb_dcn_forward_ex: deformable_group must be >= 1 and divide C");
+  const int cg = C / g.deformable_group;
+  YB_REQUIRE(h->cfg.precision != YB_PREC_F16X3 || cg % 64 == 0,
+             "yb_dcn_forward_ex: the split-precision mode needs (C / deformable_group) % 64 == 0");
+  YB_REQUIRE(h->cfg.precision != YB_PREC_F16TC || cg % 16 == 0,   // tensor cores at % 64, else the CUDA-core kernel
+             "yb_dcn_forward_ex: the fp16 mode needs (C / deformable_group) % 16 == 0");
+  const int Ho = dcn_out(H, g.kernel_h, g.stride_h, g.pad_h, g.dilation_h);
+  const int Wo = dcn_out(W, g.kernel_w, g.stride_w, g.pad_w, g.dilation_w);
+  YB_REQUIRE(Ho >= 1 && Wo >= 1, "yb_dcn_forward_ex: empty output");
+  dcn_forward(h, d_input, d_weight, d_bias, d_offset, d_mask, d_output, B, C, H, W, Co, g, Ho, Wo, (cudaStream_t)stream);
+  YB_API_END
+}
+
+int yb_dcn_psroi_pool(yb_handle* h, const float* d_input, const float* d_rois, const float* d_trans, float* d_output,
+                      float* d_count, int N, int C, int H, int W, int R, int no_trans, int num_classes,
+                      float spatial_scale, int output_dim, int group_size, int pooled, int part_size,
+                      int sample_per_part, float trans_std, void* stream) {
+  YB_API_BEGIN
+  YB_REQUIRE(h && d_input && d_rois && d_output && (no_trans || d_trans), "yb_dcn_psroi_pool: null argument");
+  YB_REQUIRE(N >= 1 && H >= 1 && W >= 1 && R >= 0, "yb_dcn_psroi_pool: N, H and W must be >= 1, R >= 0");
+  YB_REQUIRE(pooled >= 1 && group_size >= 1 && part_size >= 1 && sample_per_part >= 1,
+             "yb_dcn_psroi_pool: pooled, group_size, part_size and sample_per_part must be >= 1");
+  YB_REQUIRE(output_dim >= 1 && (int64_t)C == (int64_t)output_dim * group_size * group_size,
+             "yb_dcn_psroi_pool: C must be output_dim * group_size^2");
+  const int ncls = no_trans ? 1 : num_classes;
+  YB_REQUIRE(ncls >= 1 && output_dim % ncls == 0, "yb_dcn_psroi_pool: num_classes must be >= 1 and divide output_dim");
+  CallGuard cg(h);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (R == 0) return YB_OK;
+  // the kernel reads image rois[r, 0] (truncated, as the reference's int conversion does): checked here, before
+  // anything is written
+  std::vector<float> bidx((size_t)R);
+  YB_CHECK_CUDA(cudaMemcpy2DAsync(bidx.data(), 4, d_rois, 5 * 4, 4, (size_t)R, cudaMemcpyDeviceToHost, s));
+  YB_CHECK_CUDA(cudaStreamSynchronize(s));
+  for (int r = 0; r < R; ++r)
+    YB_REQUIRE(bidx[r] > -1.f && bidx[r] < (float)N,   // false for NaN
+               ("yb_dcn_psroi_pool: the batch index of RoI " + std::to_string(r) + " is not in [0, N)").c_str());
+  PsroiPoolArgs a;
+  a.x = d_input;
+  a.rois = d_rois;
+  a.trans = no_trans ? nullptr : d_trans;
+  a.y = d_output;
+  a.count = d_count;
+  a.N = N, a.C = C, a.H = H, a.W = W, a.R = R;
+  a.no_trans = no_trans ? 1 : 0;
+  a.num_classes = ncls;
+  a.output_dim = output_dim, a.group_size = group_size, a.pooled = pooled, a.part_size = part_size;
+  a.sample_per_part = sample_per_part;
+  a.spatial_scale = spatial_scale, a.trans_std = trans_std;
+  launch_dcn_psroi_pool(a, s, &h->lc);
   YB_API_END
 }
 

@@ -1,26 +1,30 @@
-// Fused DCNv2 (modulated deformable 3x3 convolution, deformable_groups = 1) on the tensor cores (wgmma): deformable gather ->
+// Fused DCNv2 (modulated deformable convolution, any kh x kw kernel and geometry, deformable groups of a multiple of 64
+// channels) on the tensor cores (wgmma): deformable gather ->
 // shared-memory A stage -> tensor-core contraction -> bias + ReLU, ONE kernel, no column buffer.
 //
 // Reference: DCN.forward (external/DCNv2/dcn_v2.py:118-128), modulated_deformable_im2col_gpu_kernel
 // (external/DCNv2/src/cuda/dcn_v2_im2col_cuda.cu:125-195, bilinear sampler :25-54) followed by the batched SGEMM + bias
 // of dcn_v2_cuda_forward (src/cuda/dcn_v2_cuda.cu:123-163).  The reference materialises the sampled columns
-// [B, 9*C, Ho*Wo] fp32 in HBM between the two.  Here they never leave the SM:
+// [B, taps*C, Ho*Wo] fp32 in HBM between the two.  Here they never leave the SM:
 //
-//   GEMM view   D[128 output pixels, BN couts] = sum over taps t (9) and 64-channel chunks kc of
+//   GEMM view   D[128 output pixels, BN couts] = sum over taps t (kh*kw) and 64-channel chunks kc of
 //               A_t,kc[128, 64] * W[BN, t*C + kc*64 .. +64]^T,
-//               A_t,kc[m, c] = mask(m,t) * bilinear(x, pos(m,t))[kc*64 + c]          (fp32 math, reference op order)
-//   warp 8      TMA producer of the weight tiles (B operand, [Cout][9*C] K-major)
+//               A_t,kc[m, c] = mask(m,t,g) * bilinear(x, pos(m,t,g))[kc*64 + c]      (fp32 math, reference op order)
+//               with g = kc*64 / (C/dg) the deformable group of the chunk: (C/dg) % 64 == 0, so a chunk never
+//               straddles two groups
+//   warp 8      TMA producer of the weight tiles (B operand, [Cout][taps*C] K-major)
 //   warps 0..7  two warpgroups; each gathers the A rows of its 64-row half of the tile and multiplies them with wgmma
-//               while it gathers the next k-block.  Gather: warp w owns 16 tile rows.  Once per tap, lanes 0..15 each compute the sampling geometry of ONE
-//               row (4 corner offsets, 4 bilinear weights, the modulation mask) from the 27 offset/mask channels; for
+//               while it gathers the next k-block.  Gather: warp w owns 16 tile rows.  Once per (tap, group), lanes 0..15 each compute the sampling geometry
+//               of ONE row (4 corner offsets, 4 bilinear weights, the modulation mask) from its offset/mask channels; for
 //               every 64-channel chunk the geometry reaches the lanes that need it by WARP SHUFFLE (8 lanes share a
 //               row: one 16-byte vector of 8 channels each), the four corners are fetched with 16-byte loads, blended
 //               (fp32 in the split mode, packed half2 in the fp16 mode) and written as one swizzled 16-byte piece of the K-major SWIZZLE_128B A tile -- the layout
-//               wgmma consumes directly.  Geometry is computed once per (pixel, tap), not once per
-//               (pixel, tap, 8 channels).
+//               wgmma consumes directly.  Geometry is computed once per (pixel, tap, group), not once
+//               per (pixel, tap, 8 channels).
 //   epilogue    each warpgroup: accumulator registers -> (* out_scale) + bias -> ReLU -> its rows' channel pairs.
 //   SPLIT       (YB_PREC_F16X3) x and y are [hi(C) | lo(C)] pairs, the sample is hi + lo, the A stage holds a hi (fp16)
-//               and a lo (2^11-scaled fp16) tile, the weights [Cout][hi(9C) | lo(9C)], three MMA passes per k-block.
+//               and a lo (2^11-scaled fp16) tile, the weights [Cout][hi(taps*C) | lo(taps*C)], three MMA passes per
+//               k-block.
 #include "tc_common.cuh"
 
 namespace yb {
@@ -39,14 +43,17 @@ constexpr int MAX_DSTAGES = 6;
 struct alignas(64) DcnParams {
   CUtensorMap tmW;
   const __half* x;
-  const float* om;      // [M, 27]: 18 offsets (dh, dw interleaved per tap), 9 mask logits / masks
+  const float* om;      // [M, 3*dg*taps]: per group 2*taps offsets (dh, dw interleaved per tap), then per group taps
+                        // mask logits / masks
   const float* bias;
   __half* y;
   int B, H, W, C, Ho, Wo, Cout;
   long long M;
-  int stride, pad, dil;
+  yb_dcn_params g;
+  int taps;
   int act, mask_logits;
   int stages, kchunks;
+  int gchunks;          // k-blocks per deformable group: (C / dg) / 64
   float out_scale;
 };
 
@@ -64,7 +71,7 @@ dcn_tc_kernel(const __grid_constant__ DcnParams p) {
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int stages = p.stages;
-  const int num_kb = 9 * p.kchunks;
+  const int num_kb = p.taps * p.kchunks;
   const long long m0 = (long long)blockIdx.x * DM;
   const int n0 = blockIdx.y * BN;
 
@@ -89,7 +96,7 @@ dcn_tc_kernel(const __grid_constant__ DcnParams p) {
         mbar_expect_tx(&b_full[s], (uint32_t)(NPL * B_PLANE));
 #pragma unroll
         for (int pl = 0; pl < NPL; ++pl)
-          tma_load_3d(sb + pl * B_PLANE, &p.tmW, &b_full[s], tap * p.C + kc * DK + pl * 9 * p.C, n0, 0);
+          tma_load_3d(sb + pl * B_PLANE, &p.tmW, &b_full[s], tap * p.C + kc * DK + pl * p.taps * p.C, n0, 0);
       }
     }
   } else {
@@ -112,7 +119,8 @@ dcn_tc_kernel(const __grid_constant__ DcnParams p) {
       gho = (int)(t % p.Ho);
       gb = (int)(t / p.Ho);
     }
-    const float* gom = p.om + gm * 27;
+    const int dg = p.g.deformable_group;
+    const float* gom = p.om + gm * (3 * dg * p.taps);
     const int img_base = gb * p.H * p.W;
     // this lane's items: 4 per k-block; item i -> row 16*gw + 4*i + (lane >> 3), 16-byte piece (lane & 7)
     const int piece = lane & 7;
@@ -127,20 +135,22 @@ dcn_tc_kernel(const __grid_constant__ DcnParams p) {
     int ao[4][4];        // [item][corner] pixel offsets of this lane's 4 rows, refreshed once per tap by shuffle
     float aw[4][4];      // [item][corner] weight * mask (split mode)
     __half2 hw[4][4];    // the same as broadcast half2 pairs (fp16 mode)
-    int cur_tap = -1;
+    int cur_key = -1;
     for (int kb = 0; kb < num_kb; ++kb) {
       const int s = kb % stages, it = kb / stages;
       const int tap = kb / p.kchunks, kc = kb - tap * p.kchunks;
-      if (tap != cur_tap) {
-        cur_tap = tap;
+      const int gr = kc / p.gchunks;
+      if (tap * dg + gr != cur_key) {
+        cur_key = tap * dg + gr;
         int o00 = img_base, o01 = img_base, o10 = img_base, o11 = img_base;
         float w00 = 0.f, w01 = 0.f, w10 = 0.f, w11 = 0.f;
         if (gvalid) {
           // dcn_v2_im2col_cuda.cu:151-189: h_im = h_in + i*dil + offset_h, w_im likewise; inside test (-1, H) x (-1, W)
-          const int i = tap / 3, j = tap - i * 3;
-          const float hh = __fadd_rn((float)(gho * p.stride - p.pad + i * p.dil), __ldg(gom + 2 * tap));
-          const float ww = __fadd_rn((float)(gwo * p.stride - p.pad + j * p.dil), __ldg(gom + 2 * tap + 1));
-          const float mv = __ldg(gom + 18 + tap);
+          const int i = tap / p.g.kernel_w, j = tap - i * p.g.kernel_w;
+          const float* goff = gom + gr * 2 * p.taps + 2 * tap;
+          const float hh = __fadd_rn((float)(gho * p.g.stride_h - p.g.pad_h + i * p.g.dilation_h), __ldg(goff));
+          const float ww = __fadd_rn((float)(gwo * p.g.stride_w - p.g.pad_w + j * p.g.dilation_w), __ldg(goff + 1));
+          const float mv = __ldg(gom + 2 * dg * p.taps + gr * p.taps + tap);
           const float msk = p.mask_logits ? __fdiv_rn(1.f, __fadd_rn(1.f, expf(-mv))) : mv;
           if (hh > -1.f && ww > -1.f && hh < (float)p.H && ww < (float)p.W) {
             const int hl = (int)floorf(hh), wl = (int)floorf(ww);
@@ -306,13 +316,15 @@ struct DcnTcPlan {
   dim3 grid;
 };
 
-bool dcn_tc_supported(int C, int Cout) { return C % 64 == 0 && Cout % 8 == 0 && Cout >= 8; }
+bool dcn_tc_supported(int C, int Cout, int dg) {
+  return dg >= 1 && C % dg == 0 && (C / dg) % 64 == 0 && Cout % 8 == 0 && Cout >= 8;
+}
 
-// w_packed: [Cout][9*C] fp16, k = tap*C + c  (split: [Cout][hi(9C) | lo(9C)] of w / out_scale)
+// w_packed: [Cout][taps*C] fp16, k = tap*C + c  (split: [Cout][hi(taps*C) | lo(taps*C)] of w / out_scale)
 DcnTcPlan* dcn_tc_plan_create(const __half* x, const float* om, const __half* w_packed, const float* bias, __half* y, int B,
-                              int H, int W, int C, int Ho, int Wo, int Cout, int stride, int pad, int dil, int act,
+                              int H, int W, int C, int Ho, int Wo, int Cout, const yb_dcn_params& g, int act,
                               int mask_logits, int split, float out_scale, int bn_override) {
-  YB_REQUIRE(dcn_tc_supported(C, Cout), "dcn_tc: needs C % 64 == 0 and Cout % 8 == 0");
+  YB_REQUIRE(dcn_tc_supported(C, Cout, g.deformable_group), "dcn_tc: needs (C / dg) % 64 == 0 and Cout % 8 == 0");
   auto* plan = new DcnTcPlan();
   DcnParams& q = plan->prm;
   memset(&q, 0, sizeof(q));
@@ -334,20 +346,20 @@ DcnTcPlan* dcn_tc_plan_create(const __half* x, const float* om, const __half* w_
   q.Wo = Wo;
   q.Cout = Cout;
   q.M = (long long)B * Ho * Wo;
-  q.stride = stride;
-  q.pad = pad;
-  q.dil = dil;
+  q.g = g;
+  q.taps = g.kernel_h * g.kernel_w;
   q.act = act;
   q.mask_logits = mask_logits;
   q.kchunks = C / DK;
+  q.gchunks = C / g.deformable_group / DK;
   q.out_scale = split ? out_scale : 1.f;
   const int stage = npl * (A_TILE + BN * DK * 2);
   int stages = std::min(MAX_DSTAGES, (225 * 1024) / stage);
-  stages = std::max(2, std::min(stages, 9 * q.kchunks));   // >= 2: a warpgroup keeps one wgmma group in flight
+  stages = std::max(2, std::min(stages, q.taps * q.kchunks));   // >= 2: a warpgroup keeps one wgmma group in flight
   q.stages = stages;
   plan->smem = (size_t)stages * stage + 1024;
   plan->grid = dim3((unsigned)((q.M + DM - 1) / DM), (unsigned)ceil_div(Cout, BN), 1);
-  const uint64_t KP = (uint64_t)npl * 9 * C;
+  const uint64_t KP = (uint64_t)npl * q.taps * C;
   uint64_t dims[3] = {KP, (uint64_t)Cout, 1};
   uint64_t str[2] = {KP * 2, KP * (uint64_t)Cout * 2};
   uint32_t box[3] = {(uint32_t)DK, (uint32_t)BN, 1};

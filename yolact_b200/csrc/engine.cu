@@ -372,14 +372,14 @@ struct NetBuilder {
       const int Cout = w.Cout;
       op.fn = [in, om, out, wp, bias, stride, Cout, lc](cudaStream_t s) {
         launch_dcn_simt<float>((const float*)in.ptr, (const float*)om.ptr, wp, bias, (float*)out.ptr, in.B, in.H, in.W,
-                               in.C, out.H, out.W, Cout, stride, 1, 1, ACT_RELU, 1, s, lc);
+                               in.C, out.H, out.W, Cout, dcn_3x3(stride), ACT_RELU, 1, s, lc);
       };
       push(op);
     } else {
       // one kernel: warp-shuffled tap geometry -> bilinear samples straight into the swizzled A stage -> wgmma
       const int sp = in.split ? 1 : 0;
       DcnTcPlan* dp = dcn_tc_plan_create((const __half*)in.ptr, (const float*)om.ptr, w.w_tc, w.bias, (__half*)out.ptr, in.B,
-                                         in.H, in.W, in.C, Ho, Wo, w.Cout, stride, 1, 1, ACT_RELU, 1, sp, w.out_scale);
+                                         in.H, in.W, in.C, Ho, Wo, w.Cout, dcn_3x3(stride), ACT_RELU, 1, sp, w.out_scale);
       ex->dcn_plans.push_back(dp);
       Op op;
       op.is_conv = true;

@@ -262,23 +262,41 @@ void launch_coco_rle(const yb_post_item* d_items, const yb_post_item* h_items, i
                      int32_t* row_len, int64_t* need, cudaStream_t stream, LaunchCounter* lc);
 
 // ---- DCNv2 -------------------------------------------------------------------------------------
-// x NHWC (T) [B,H,W,C]; om = offset/mask conv output NHWC fp32 [B,Ho,Wo,27] (18 offsets
-// interleaved (dh,dw) per tap, then 9 masks: logits when mask_logits, dcn_v2.py:118-124); w: [9*C][Cout] (T);
-// y NHWC (T).  Fused deformable gather + contraction + bias + activation.
+// Geometry g (yb_dcn_params: kh x kw taps, tap = i*kw + j, per-axis stride / pad / dilation, dg deformable groups).
+// x NHWC (T) [B,H,W,C]; om NHWC fp32 [B,Ho,Wo,3*dg*taps]: the offsets (channel gr*2*taps + 2*tap = dh, + 1 = dw of
+// group gr), then the masks (2*dg*taps + gr*taps + tap; logits when mask_logits, dcn_v2.py:118-124) -- for the
+// network's 3x3 layers the 27 channels of conv_offset_mask; w: [taps*C][Cout] (T), row tap*C + c; y NHWC (T).
+// Fused deformable gather + contraction + bias + activation, any C with C % dg == 0.
 template <typename T>
 void launch_dcn_simt(const T* x, const float* om, const T* w, const float* bias, T* y, int B, int H,
-                     int W, int C, int Ho, int Wo, int Cout, int stride, int pad, int dil, int act,
+                     int W, int C, int Ho, int Wo, int Cout, const yb_dcn_params& g, int act,
                      int mask_logits, cudaStream_t stream, LaunchCounter* lc);
 
 // ---- fused DCNv2 on the tensor cores (dcn_tc.cu): gather -> smem A stage -> MMA -> bias/act, no column buffer ----------------
 struct DcnTcPlan;
-bool dcn_tc_supported(int C, int Cout);
-// x NHWC half [B,H,W,C] (split: [.., hi(C) | lo(C)]), om fp32 [B,Ho,Wo,27], w_packed [Cout][9*C] half with k = tap*C + c
-// (split: [Cout][hi(9C) | lo(9C)] scaled by 1 / out_scale), y NHWC half [B,Ho,Wo,Cout] (split: pairs).
+// (C / dg) % 64 == 0: every 64-channel k-block lies inside one deformable group
+bool dcn_tc_supported(int C, int Cout, int dg = 1);
+// x NHWC half [B,H,W,C] (split: [.., hi(C) | lo(C)]), om as launch_dcn_simt's, w_packed [Cout][taps*C] half with
+// k = tap*C + c (split: [Cout][hi(taps*C) | lo(taps*C)] scaled by 1 / out_scale), y NHWC half [B,Ho,Wo,Cout] (split: pairs).
 DcnTcPlan* dcn_tc_plan_create(const __half* x, const float* om, const __half* w_packed, const float* bias, __half* y, int B,
-                              int H, int W, int C, int Ho, int Wo, int Cout, int stride, int pad, int dil, int act,
+                              int H, int W, int C, int Ho, int Wo, int Cout, const yb_dcn_params& g, int act,
                               int mask_logits, int split = 0, float out_scale = 1.f, int bn_override = 0);
 void dcn_tc_plan_destroy(DcnTcPlan* plan);
 void launch_dcn_tc(const DcnTcPlan* plan, cudaStream_t stream, LaunchCounter* lc);
+// The 3x3 geometry of the network's DCN layers (stride s, padding 1, dilation 1, one deformable group).
+inline yb_dcn_params dcn_3x3(int stride) { return yb_dcn_params{3, 3, stride, stride, 1, 1, 1, 1, 1}; }
+
+// ---- deformable PS-RoI pooling (dcn_pool.cu), fp32 NCHW, one thread per output element ------------------------------
+struct PsroiPoolArgs {
+  const float* x;        // [N, C, H, W]
+  const float* rois;     // [R, 5]
+  const float* trans;    // [R, 2 * num_classes, part, part], unread when no_trans
+  float* y;              // [R, output_dim, pooled, pooled]
+  float* count;          // same shape, nullable
+  int N, C, H, W, R;
+  int no_trans, num_classes, output_dim, group_size, pooled, part_size, sample_per_part;
+  float spatial_scale, trans_std;
+};
+void launch_dcn_psroi_pool(const PsroiPoolArgs& a, cudaStream_t stream, LaunchCounter* lc);
 
 }  // namespace yb
