@@ -136,6 +136,8 @@ def install_display(E):
     from the detections in two launches, with the --display_fps box and --display_masks, instead of postprocess writing
     fp32 masks for every row at frame size.  The image and the drawn rows come to the host in one copy, and the fps
     text, rectangles and labels are drawn on it with OpenCV from the drawn rows, as eval.py:226-259 draws them.
+    Detections on another GPU than the frame (a CustomDataParallel replica's, evalvideo) are copied to the frame's
+    device first, and the image is that of the same-device render.
     undo_transform=True (evaluate --display) and --display_lincomb go to the original prep_display."""
     import torch
     from yolact_b200 import display

@@ -102,12 +102,28 @@ def _render(items, frames, dev, ph, pw, k, crop_masks, top_k, score_threshold, c
                "yb_render_list_ex")
 
 
+def _on_device(det_output, dev):
+    """det_output with every detection that is on another GPU than dev copied to dev (det_output is left as it is).
+    The copy is torch's device-to-device copy: it runs on the detections' device's current stream, so it follows the
+    network call that enqueued them there (DataParallel's replica k enqueues on cuda:k's current stream), and dev's
+    current stream waits for it."""
+    out = []
+    for d in det_output:
+        det = d['detection']
+        if det is not None and det['box'].is_cuda and det['box'].device != dev:
+            d = dict(d, detection={k: v.to(dev) for k, v in det.items()})
+        out.append(d)
+    return out
+
+
 def render_masks(det_output, frames, top_k=5, score_threshold=0, class_color=False, mask_alpha=0.45, crop_masks=True,
                  fps_box=None, draw_masks=True):
     """frames: a list of CUDA [h_i,w_i,3] BGR tensors or one [B,h,w,3] tensor, uint8 or float32 0..255, one per entry of
     det_output (Yolact's output list).  fps_box: None or (text_w, text_h); draw_masks: blend the masks (see the module
     docstring).  Returns (images, drawn): images a list of CUDA uint8 [h_i,w_i,3]; drawn a dict of device tensors num,
-    classes, scores, boxes (see the module docstring)."""
+    classes, scores, boxes (see the module docstring).  Detections on another GPU than the frames (a DataParallel
+    replica's) are copied to the frames' device first, so the images are those of the same-device render, bit for
+    bit."""
     frames = _frame_list(frames, "render_masks")
     if len(frames) != len(det_output):
         raise ValueError("render_masks: %d frames for %d detections" % (len(frames), len(det_output)))
@@ -121,7 +137,7 @@ def render_masks(det_output, frames, top_k=5, score_threshold=0, class_color=Fal
     if B == 0:
         return [], drawn
 
-    g = _gather(det_output, "render_masks")
+    g = _gather(_on_device(det_output, dev), "render_masks")
     dets = dict(zip(g.live, g.dets))
     keep_alive = []   # the contiguous inputs, held until the call has enqueued its reads of them
     ph, pw, k = g.shape if g.eval_mask_branch else (1, 1, 4)

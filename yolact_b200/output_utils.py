@@ -20,6 +20,7 @@ through Yolact.forward_frames), in one call with one launch per kernel for the w
 """
 import collections
 import ctypes
+import threading
 
 import torch
 
@@ -28,23 +29,27 @@ from . import config as _config
 
 _FORMATS = {"f32": _lib.YB_MASK_F32, "u8": _lib.YB_MASK_U8, "bits": _lib.YB_MASK_BITS}
 _ops_handles = {}
+# One handle per (device, mask_dim) although DataParallel(FastBaseTransform()), postprocess and render_masks reach
+# the cache from several threads and devices at once.
+_ops_lock = threading.Lock()
 
 
 def _ops_handle(device, mask_dim=32):
     idx = device.index if device.index is not None else torch.cuda.current_device()
     key = (idx, mask_dim)
-    if key not in _ops_handles:
-        lib = _lib.load()
-        yc = _lib.YbConfig()
-        yc.backbone = _lib.YB_BACKBONE_NONE
-        yc.num_classes = 81
-        yc.mask_dim = mask_dim
-        yc.precision = _lib.YB_PREC_F32
-        yc.nms_top_k, yc.nms_conf_thresh, yc.nms_thresh, yc.max_num_detections = 200, 0.05, 0.5, 100
-        h = ctypes.c_void_p()
-        _lib.check(lib.yb_create(ctypes.byref(yc), idx, ctypes.byref(h)), "yb_create(ops)")
-        _ops_handles[key] = h
-    return _ops_handles[key]
+    with _ops_lock:
+        if key not in _ops_handles:
+            lib = _lib.load()
+            yc = _lib.YbConfig()
+            yc.backbone = _lib.YB_BACKBONE_NONE
+            yc.num_classes = 81
+            yc.mask_dim = mask_dim
+            yc.precision = _lib.YB_PREC_F32
+            yc.nms_top_k, yc.nms_conf_thresh, yc.nms_thresh, yc.max_num_detections = 200, 0.05, 0.5, 100
+            h = ctypes.c_void_p()
+            _lib.check(lib.yb_create(ctypes.byref(yc), idx, ctypes.byref(h)), "yb_create(ops)")
+            _ops_handles[key] = h
+        return _ops_handles[key]
 
 
 def launch_count():

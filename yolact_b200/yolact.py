@@ -10,9 +10,13 @@ eval.py assigns (eval.py:871-872); `.maskiou_net` exists for YOLACT++ configs.
 Everything numerical happens in libyolact_b200.so through the C ABI (include/yolact_b200.h); the
 nn.Module tree below only HOLDS parameters under the reference's names -- its layers are never
 called.  There is no PyTorch/CPU fallback: without the CUDA library on an H100 forward() raises.
+
+Under torch.nn.DataParallel (evalvideo's CustomDataParallel, eval.py:630-634,661) the replica on cuda:k runs on the
+net's handle for cuda:k, with the net's weights, and its detections name the net itself as 'net'.
 """
 import ctypes
 import os
+import threading
 import warnings
 
 import torch
@@ -152,6 +156,11 @@ class FastMaskIoUNet(nn.Module):
         return out
 
 
+# Held by Yolact._handle_for from the handle lookup to the end of the weight push: DataParallel's replica threads and
+# eval.py's ThreadPool make a net's first calls from several threads at once, and each device must get one handle.
+_handle_lock = threading.Lock()
+
+
 # ---------------------------------------------------------------------------------------------
 def make_yb_config(c, precision):
     yc = _lib.YbConfig()
@@ -229,6 +238,21 @@ class Yolact(nn.Module):
         self._pushed = {}       # device index -> version of the weights that handle holds
         self._detect_pushed = {}  # device index -> (top_k, conf_thresh, nms_thresh, max_num_detections) the handle uses
         self._plan_files = []   # load_plans paths, loaded into every handle created later too
+        self._replica_of = None   # [the module this one was replicated from] on a DataParallel replica (_root)
+
+    # ---- DataParallel replicas -------------------------------------------------------------------
+    def _replicate_for_data_parallel(self):
+        """torch.nn.parallel.replicate's per-call copy (DataParallel, eval.py's CustomDataParallel).  The replica's
+        parameters are broadcast copies set as plain attributes, outside its state_dict(), and the library never reads
+        them: the replica runs on its root's handles, with its root's weights (_root)."""
+        replica = super()._replicate_for_data_parallel()
+        replica._replica_of = [self._root()]   # a list, so that it is not registered as a submodule
+        return replica
+
+    def _root(self):
+        """The module whose weights, handles and pushed-state maps this one uses: itself, or the module a replica was
+        replicated from.  Replica k's detections name the root as their 'net'."""
+        return self._replica_of[0] if self._replica_of else self
 
     # ---- weights ---------------------------------------------------------------------------------
     def save_weights(self, path):
@@ -268,19 +292,22 @@ class Yolact(nn.Module):
             raise _lib.YbError("yolact_b200 runs on CUDA (H100) only; got a tensor on %s. There is no CPU path." % device)
         idx = device.index if device.index is not None else torch.cuda.current_device()
         lib = _lib.load()
-        if idx not in self._handles:
-            h = ctypes.c_void_p()
-            yc = make_yb_config(self.cfg, self.precision)
-            _lib.check(lib.yb_create(ctypes.byref(yc), idx, ctypes.byref(h)), "yb_create")
-            self._handles[idx] = h
-            for path in self._plan_files:
-                if lib.yb_load_plans(h, path.encode()) != 0:
-                    warnings.warn("plan file %s does not apply to cuda:%d; its shapes are timed as usual: %s"
-                                  % (path, idx, lib.yb_last_error().decode()))
-        h = self._handles[idx]
-        if self._pushed.get(idx) != self._version:     # per device: every handle re-syncs on its next call
-            self._push_weights(h)
-            self._pushed[idx] = self._version
+        root = self._root()
+        with _handle_lock:
+            h = root._handles.get(idx)
+            if h is None:
+                h = ctypes.c_void_p()
+                yc = make_yb_config(root.cfg, root.precision)
+                _lib.check(lib.yb_create(ctypes.byref(yc), idx, ctypes.byref(h)), "yb_create")
+                root._handles[idx] = h
+                for path in root._plan_files:
+                    if lib.yb_load_plans(h, path.encode()) != 0:
+                        warnings.warn("plan file %s does not apply to cuda:%d; its shapes are timed as usual: %s"
+                                      % (path, idx, lib.yb_last_error().decode()))
+            version = root._version
+            if root._pushed.get(idx) != version:     # per device: every handle re-syncs on its next call
+                root._push_weights(h)
+                root._pushed[idx] = version
         return h
 
     def _push_weights(self, h):
@@ -296,6 +323,8 @@ class Yolact(nn.Module):
 
     def __del__(self):
         try:
+            if self._replica_of:
+                return   # a replica's handles are its root's
             lib = _lib.load()
             for h in self._handles.values():
                 lib.yb_destroy(h)
@@ -503,9 +532,10 @@ class Yolact(nn.Module):
         d = self.detect
         dkey = (int(d.top_k), float(d.conf_thresh), float(d.nms_thresh), int(d.max_num_detections))
         idx = device.index if device.index is not None else torch.cuda.current_device()
-        if self._detect_pushed.get(idx) != dkey:
+        pushed = self._root()._detect_pushed
+        if pushed.get(idx) != dkey:
             _lib.check(lib.yb_set_detect_params(h, *dkey), "yb_set_detect_params")
-            self._detect_pushed[idx] = dkey
+            pushed[idx] = dkey
         M = dkey[0] if (mode & 0xFF) == _lib.YB_NMS_CROSS_CLASS else dkey[3]
         ph, pw = ctypes.c_int32(), ctypes.c_int32()
         _lib.check(lib.yb_proto_size(h, H, W, ctypes.byref(ph), ctypes.byref(pw)), "yb_proto_size")
@@ -531,15 +561,16 @@ class Yolact(nn.Module):
         # parallel.gather_detections (one pack kernel + one all_gather) instead of re-padding the views
         self.last_padded_detections = (box, coef, cls, score, count)
         counts = count.cpu().tolist()  # the only host sync: Detect's output is variable-size by contract
+        net = self._root()
         out = []
         for b, n in enumerate(counts):
             if n == 0:
-                out.append({"detection": None, "net": self})  # detection.py:94-95
+                out.append({"detection": None, "net": net})  # detection.py:94-95
                 continue
             det = {"box": box[b, :n], "mask": coef[b, :n], "class": cls[b, :n], "score": score[b, :n]}
             if proto is not None:
                 det["proto"] = proto[b]
-            out.append({"detection": det, "net": self})
+            out.append({"detection": det, "net": net})
         return out
 
     @staticmethod
